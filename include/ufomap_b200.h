@@ -172,6 +172,31 @@ int ufo_b200_export_leaves(ufo_b200_map* m, uint64_t* codes, float* logodds, uin
  * voxels' colours by the node's mean colour). */
 int ufo_b200_set_value_volume(ufo_b200_map* m, const double box6[6], double occupancy, uint32_t min_depth);
 
+/* Per-node writes as one ordered batch, the same as making the calls one after the other in array
+ * order (DESIGN.md section 8 states the semantics):
+ *   op[i] = 0  ADD value[i] (float log-odds): updateValue(code, value)  occupancy_map_base.h:1063-1120
+ *              -- integrateHit / integrateMiss :565-593 (value = float(prob_hit_log) / float(prob_miss_log)),
+ *              updateOccupancy :544-559 (value = float(toLogit(p))).  Every voxel below the node at
+ *              (codes[i], depths[i]) becomes clamp(v + value), one clamp per update.
+ *   op[i] = 1  SET value[i]: setOccupancy :524-538 -> setNodeValue :1037-1057 as intended (the
+ *              reference's does not compile): every voxel below the node becomes clamp(value).
+ * depths[i] 0..6.  Host arrays.  Rejected as a whole (nothing applied): a code whose depth-0 key lies
+ * outside the map (UFO_B200_E_INVALID); depth > 6, a sharded or routed map, SET at depth > 0 on a
+ * colour map (UFO_B200_E_UNSUPPORTED).  Leaf colours are not changed.  The min/max change box is not
+ * updated (the reference does not update it for these calls); change detection records the voxels
+ * whose value changed.  async != 0 returns after the work is enqueued. */
+int ufo_b200_update_nodes(ufo_b200_map* m, const uint64_t* codes, const uint32_t* depths, const uint8_t* ops,
+                          const float* values, size_t n, int async);
+
+/* insertMissOnRay (hit_end = 0) / insertRay (hit_end = 1)  occupancy_map_base.h:251-268 for n rays,
+ * origins / ends [n][3] (host arrays): integrateMiss on every node computeRay (octree.h:449-496, as
+ * ufo_b200_compute_ray) walks at `depth`, then with hit_end integrateHit on the depth-0 voxel of the
+ * GIVEN end point (not the one max_range truncates to).  Rays are applied in array order.  Rejected
+ * as a whole: an origin or end outside the map (UFO_B200_E_INVALID); depth > 6, sharded or routed
+ * maps (UFO_B200_E_UNSUPPORTED). */
+int ufo_b200_insert_rays(ufo_b200_map* m, const double* origins, const double* ends, size_t n,
+                         double max_range, uint32_t depth, int hit_end, int async);
+
 /* Octree::write(std::ostream& / filename, bounding_volume, compress = false, min_depth)
  * (octree.h:776-864, writeNodes occupancy_map_base.h:1457-1533): the map as a UFOMap file image
  * -- text header, then the pre-order node stream -- which the reference's Octree::read / the RViz

@@ -428,6 +428,47 @@ class MapFacade
 		last_status_ = ufo_b200_set_value_volume(map_, box, occupancy_value, min_depth);
 	}
 
+	//
+	// Per-node writes (occupancy_map_base.h:524-593) and ray insertion (:251-268).  Each call is a
+	// batch of one on the device (ufo_b200_update_nodes / ufo_b200_insert_rays); depth 0..6.  Like the
+	// inserts they return nothing and leave their status in lastStatus().
+	//
+	void setOccupancy(Code const& code, double occupancy_value) { writeNode(code, 1, (float)toLogit(occupancy_value)); }
+	void setOccupancy(Point3 const& coord, double occupancy_value, DepthType depth = 0)
+	{
+		setOccupancy(toCode(coord, depth), occupancy_value);
+	}
+	void setOccupancy(double x, double y, double z, double occupancy_value, DepthType depth = 0)
+	{
+		setOccupancy(toCode(x, y, z, depth), occupancy_value);
+	}
+	void updateOccupancy(Code const& code, double occupancy_value_update)
+	{
+		writeNode(code, 0, (float)toLogit(occupancy_value_update));
+	}
+	void updateOccupancy(Point3 const& coord, double occupancy_value_update, DepthType depth = 0)
+	{
+		updateOccupancy(toCode(coord, depth), occupancy_value_update);
+	}
+	void updateOccupancy(double x, double y, double z, double occupancy_value_update, DepthType depth = 0)
+	{
+		updateOccupancy(toCode(x, y, z, depth), occupancy_value_update);
+	}
+	void integrateHit(Code const& code) { writeNode(code, 0, (float)model()[2]); }
+	void integrateHit(Point3 const& coord, DepthType depth = 0) { integrateHit(toCode(coord, depth)); }
+	void integrateHit(double x, double y, double z, DepthType depth = 0) { integrateHit(toCode(x, y, z, depth)); }
+	void integrateMiss(Code const& code) { writeNode(code, 0, (float)model()[3]); }
+	void integrateMiss(Point3 const& coord, DepthType depth = 0) { integrateMiss(toCode(coord, depth)); }
+	void integrateMiss(double x, double y, double z, DepthType depth = 0) { integrateMiss(toCode(x, y, z, depth)); }
+	void insertMissOnRay(Point3 const& origin, Point3 const& end, double max_range = -1, DepthType depth = 0)
+	{
+		last_status_ = ufo_b200_insert_rays(map_, origin.data(), end.data(), 1, max_range, depth, 0, 0);
+	}
+	void insertRay(Point3 const& origin, Point3 const& end, double max_range = -1, DepthType depth = 0)
+	{
+		last_status_ = ufo_b200_insert_rays(map_, origin.data(), end.data(), 1, max_range, depth, 1, 0);
+	}
+
 	// Octree::writeData (octree.h:866-917): the node stream of a UFOMap message, whole map or the
 	// part inside an AABB, truncated at min_depth (0..4).  Returns the number of bytes written, -1
 	// on error (as the reference does).
@@ -707,6 +748,14 @@ class MapFacade
 	// occupancy_map_base.h:911 -- LogitType is float there: the argument narrows to float and the
 	// exponential is the float one, for the sensor-model getters as well as for getOccupancy
 	static double toProb(float logit) { return 1.0 / (1.0 + std::exp(-logit)); }
+	// occupancy_map_base.h:909: in double; the callers narrow to float (LogitType)
+	static double toLogit(double prob) { return std::log(prob / (1.0 - prob)); }
+	void writeNode(Code const& code, std::uint8_t op, float value)
+	{
+		std::uint64_t c = code.getCode();
+		std::uint32_t d = code.getDepth();
+		last_status_ = ufo_b200_update_nodes(map_, &c, &d, &op, &value, 1, 0);
+	}
 	double const* model() const
 	{
 		ufo_b200_sensor_model_logit(map_, model_);

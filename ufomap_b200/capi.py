@@ -63,6 +63,7 @@ SYMBOLS = [
     "ufo_b200_route_inbox_bytes", "ufo_b200_route_setup", "ufo_b200_route_connect", "ufo_b200_route_mark",
     "ufo_b200_route_apply", "ufo_b200_ipc_export", "ufo_b200_ipc_open", "ufo_b200_ipc_close",
     "ufo_b200_write_compressed", "ufo_b200_cast_rays", "ufo_b200_export_nodes", "ufo_b200_read_data", "ufo_b200_enable_change_detection", "ufo_b200_reset_change_detection", "ufo_b200_changed_codes",
+    "ufo_b200_update_nodes", "ufo_b200_insert_rays",
 ]
 
 class Cloud2(C.Structure):
@@ -104,6 +105,8 @@ def load():
     lib.ufo_b200_write_file.argtypes = [vp, C.c_char_p, vp, u32, i32]
     lib.ufo_b200_clear_resize.argtypes = [vp, dbl, u32]
     lib.ufo_b200_set_value_volume.argtypes = [vp, vp, dbl, u32]
+    lib.ufo_b200_update_nodes.argtypes = [vp, vp, vp, vp, vp, sz, i32]
+    lib.ufo_b200_insert_rays.argtypes = [vp, vp, vp, sz, dbl, u32, i32, i32]
     lib.ufo_b200_write_data.argtypes = [vp, vp, u32, vp, sz, C.POINTER(sz)]
     lib.ufo_b200_transform_points.argtypes = [vp, vp, sz, i32, vp]
     lib.ufo_b200_pose_from_rpy.argtypes = [dbl, dbl, dbl, dbl, dbl, dbl, vp]
@@ -380,6 +383,28 @@ class Map:
         """setValueVolume(AABB(min, max), occupancy probability, min_depth); box = (min xyz, max xyz)."""
         b = self._box6(box)
         self._check(self.lib.ufo_b200_set_value_volume(self.h, b.ctypes.data, float(occupancy), int(min_depth)))
+
+    # -- per-node writes ----------------------------------------------------
+    ADD, SET = 0, 1
+
+    def update_nodes(self, codes, depths, ops, values, async_=False):
+        """Ordered batch of node writes: op 0 adds values[i] (float log-odds) to every voxel below
+        the node (updateValue), op 1 sets them to it (setNodeValue); clamped after every update."""
+        c = np.ascontiguousarray(codes, dtype=np.uint64).reshape(-1)
+        n = len(c)
+        d = np.ascontiguousarray(np.broadcast_to(depths, (n,)), dtype=np.uint32)
+        o = np.ascontiguousarray(np.broadcast_to(ops, (n,)), dtype=np.uint8)
+        v = np.ascontiguousarray(np.broadcast_to(values, (n,)), dtype=np.float32)
+        self._check(self.lib.ufo_b200_update_nodes(self.h, c.ctypes.data, d.ctypes.data, o.ctypes.data,
+                                                   v.ctypes.data, n, int(async_)))
+
+    def insert_rays(self, origins, ends, max_range=-1.0, depth=0, hit_end=False, async_=False):
+        """insertMissOnRay (hit_end=False) / insertRay (hit_end=True) for every (origin, end)."""
+        e = np.ascontiguousarray(ends, dtype=np.float64).reshape(-1, 3)
+        o = np.ascontiguousarray(np.broadcast_to(np.asarray(origins, np.float64).reshape(-1, 3), e.shape),
+                                 dtype=np.float64)
+        self._check(self.lib.ufo_b200_insert_rays(self.h, o.ctypes.data, e.ctypes.data, len(e), float(max_range),
+                                                  int(depth), int(hit_end), int(async_)))
 
     def write_data(self, box=None, min_depth=0):
         """Octree::writeData(stream, AABB(min, max) or whole map, False, min_depth): node stream.

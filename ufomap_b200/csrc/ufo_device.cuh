@@ -46,7 +46,7 @@ struct Counters {
 	uint32_t item_cursor;  // next work unit of the fused walk (k_walk_mark)
 	uint32_t max_span;     // longest ray of the scan in dominant-axis steps (sets the shell thickness)
 	uint32_t n_touched_alt;  // routed mode: length of DeviceMap::touched_alt
-	uint32_t n_dirty;        // dense mode: length of DeviceMap::vol_list (also: node list of insert depth 5/6)
+	uint32_t n_dirty;        // dense mode: length of DeviceMap::vol_list (also: node list of insert depth 5/6, bricks of a write batch)
 	uint32_t list_count[3];  // dirty-list lengths of the upper-level pass (rotating by depth % 3)
 	uint32_t n_rays;
 	uint32_t ray_batch;  // next batch of 32 rays for the persistent ray-walk warps

@@ -31,6 +31,9 @@
 #include "ufo_walk.cuh"
 #include "ufo_route.cuh"
 #include "ufo_import.cuh"
+#include "ufo_write.cuh"
+
+#include <cub/device/device_radix_sort.cuh>
 
 using namespace ufo_b200;
 
@@ -99,6 +102,9 @@ struct PendingScan {
 	VolumeArgs vol{};
 	float set_value = 0.0f;
 	uint32_t regrows = 0;
+	// write batch (ufo_write.cuh): ordered node updates or rays instead of a scan
+	bool write = false;
+	WriteArgs w{};
 };
 
 struct ufo_b200_map {
@@ -133,6 +139,19 @@ struct ufo_b200_map {
 	uint32_t* d_vmask = nullptr;
 	RayConst* d_rc = nullptr;
 	size_t item_cap = 0;
+	// write batches: inputs + record regions, records (two key / index buffers for the sort), the
+	// brick segments of the sorted keys, sort scratch
+	unsigned char* d_w_in = nullptr;
+	size_t w_in_cap = 0;
+	unsigned long long* d_w_keys[2] = {nullptr, nullptr};
+	uint32_t* d_w_idx[2] = {nullptr, nullptr};
+	WriteRec* d_w_recs = nullptr;
+	size_t w_rec_cap = 0;
+	uint32_t* d_w_seg = nullptr;
+	size_t w_seg_cap = 0;
+	void* d_w_tmp = nullptr;
+	size_t w_tmp_cap = 0;
+	bool write_pass = false;  // the last pass was a write batch (its stats carry ms_update)
 	// bookkeeping
 	uint32_t n_blocks = 0, n_bricks = 0, n_upper = 0;  // host view after the last completed scan
 	size_t device_bytes = 0;
@@ -266,7 +285,9 @@ void free_pools(Map* m)
 	                M.leaf, M.leaf_rgb, M.miss_mask, M.hit_mask, M.agg2, M.meta, M.sum1, M.rgb2, M.sum1_rgb,
 	                M.alias_miss, M.alias_hit, M.uh_keys, M.uh_vals, M.up_key, M.up_agg, M.up_rgb, M.up_stamp, M.up_child, M.up_child_rgb, M.up_valid, M.up_parent, M.brick_parent, M.ctr, m->d_list[0],
 	                m->d_list[1], m->d_points[0], m->d_points[1], m->d_ray_end, m->d_hit_tab, m->d_tab_keys, m->d_tab_min,
-	                m->d_seg, m->d_seg_base, m->d_seg_count, m->d_order, m->d_nodes, m->d_items, m->d_vmask, m->d_rc};
+	                m->d_seg, m->d_seg_base, m->d_seg_count, m->d_order, m->d_nodes, m->d_items, m->d_vmask, m->d_rc,
+	                m->d_w_in, m->d_w_keys[0], m->d_w_keys[1], m->d_w_idx[0], m->d_w_idx[1], m->d_w_recs, m->d_w_seg,
+	                m->d_w_tmp};
 	for (void* p : ptrs)
 		if (p) cudaFree(p);
 }
@@ -466,7 +487,10 @@ void finish_stats(Map* m)
 	if (m->ev_valid) {
 		cudaEventElapsedTime(&st.ms_total, m->ev[0], m->ev[6]);
 		if (m->h2d_valid) cudaEventElapsedTime(&st.ms_h2d, m->ev_copy0, m->ev_copied);
-		if (m->profiling) {
+		if (m->write_pass) {
+			cudaEventElapsedTime(&st.ms_update, m->ev[3], m->ev[5]);
+			cudaEventElapsedTime(&st.ms_propagate, m->ev[5], m->ev[6]);
+		} else if (m->profiling) {
 			cudaEventElapsedTime(&st.ms_points, m->ev[0], m->ev[2]);
 			if (m->ev7_valid) {
 				cudaEventElapsedTime(&st.ms_rays, m->ev[2], m->ev[7]);
@@ -696,9 +720,88 @@ __global__ void k_reset_upper_pass(Counters* c, uint32_t n_upper)
 	c->n_upper = n_upper;
 }
 
+// (re)allocates a device buffer of at least `bytes`; called with the stream idle
+template <class T>
+void ensure_dev(Map* m, T*& p, size_t& cap_bytes, size_t bytes)
+{
+	if (bytes <= cap_bytes && p) return;
+	if (p) {
+		CK(cudaFree(p));
+		m->device_bytes -= cap_bytes;
+	}
+	p = nullptr;
+	const size_t nb = std::max<size_t>(bytes + bytes / 8, 1 << 12);
+	CK(cudaMalloc(reinterpret_cast<void**>(&p), nb));
+	cap_bytes = nb;
+	m->device_bytes += nb;
+}
+
+// Enqueues one write batch (ufo_write.cuh): expand -> sort -> segments -> apply -> aggregates.
+// Called with the stream idle.  If a pool overflows while expanding, every later kernel backs off
+// and finalize_scan() grows the pool and enqueues the whole batch again: no leaf was written, and
+// finding or creating a brick twice is harmless, so every update is applied exactly once.
+void enqueue_write(Map* m, PendingScan& p)
+{
+	DeviceMap& M = m->M;
+	cudaStream_t s = m->stream;
+	WriteArgs a = p.w;
+	M.scan_id++;
+	if (M.scan_id == 0) M.scan_id = 1;
+	M.up_epoch++;
+	if (M.up_epoch == 0) M.up_epoch = 1;
+	M.dense = 0;
+	M.mask_base = M.miss_mask;
+	{
+		size_t cap = m->w_seg_cap;
+		ensure_dev(m, m->d_w_seg, cap, (size_t)M.brick_cap * 3 * sizeof(uint32_t));
+		m->w_seg_cap = cap;
+	}
+	a.seg_begin = m->d_w_seg;
+	a.seg_end = m->d_w_seg + M.brick_cap;
+	a.seg_list = m->d_w_seg + 2 * (size_t)M.brick_cap;
+	// keys: brick slot << 32 | sequence number; only the bits a slot below brick_cap can use are sorted
+	int end_bit = 32;
+	while (end_bit < 64 && (1ull << (end_bit - 32)) <= M.brick_cap) ++end_bit;
+	size_t tmp_bytes = 0;
+	CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, m->d_w_keys[0], m->d_w_keys[1], m->d_w_idx[0],
+	                                   m->d_w_idx[1], (int)a.n_rec, 0, end_bit, s));
+	ensure_dev(m, m->d_w_tmp, m->w_tmp_cap, tmp_bytes);
+	push_counters(m);
+	a.keys = m->d_w_keys[0];
+	a.idx = m->d_w_idx[0];
+	a.recs = m->d_w_recs;
+	if (a.n) k_write_expand<<<(a.n + 127) / 128, 128, 0, s>>>(M, a);
+	tmp_bytes = m->w_tmp_cap;
+	CK(cub::DeviceRadixSort::SortPairs(m->d_w_tmp, tmp_bytes, m->d_w_keys[0], m->d_w_keys[1], m->d_w_idx[0],
+	                                   m->d_w_idx[1], (int)a.n_rec, 0, end_bit, s));
+	a.keys = m->d_w_keys[1];
+	a.idx = m->d_w_idx[1];
+	k_write_segments<<<m->sm_count * 8, 256, 0, s>>>(M, a);
+	CK(cudaEventRecord(m->ev[3], s));
+	k_write_apply<<<m->sm_count * 16, 64, 0, s>>>(M, a);
+	CK(cudaEventRecord(m->ev[5], s));
+	k_import_refresh<<<m->sm_count * 8, 256, 0, s>>>(M);
+	if (M.color) k_brick_agg<true><<<m->sm_count * 4, 256, 0, s>>>(M);
+	else k_brick_agg<false><<<m->sm_count * 4, 256, 0, s>>>(M);
+	m->launches += 6;  // the sort's own launches not counted
+	launch_upper(m);
+	CK(cudaGetLastError());
+	CK(cudaEventRecord(m->ev[6], s));
+	m->ev_valid = true;
+	m->write_pass = true;
+	CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+	m->stats_pending = true;
+	p.valid = true;
+}
+
 // Enqueues every kernel of one scan and the read-back of its counters; never waits.
 void enqueue_scan(Map* m, PendingScan& p)
 {
+	if (p.write) {
+		enqueue_write(m, p);
+		return;
+	}
+	m->write_pass = false;
 	DeviceMap& M = m->M;
 	cudaStream_t s = m->stream;
 	ScanArgs& a = p.a;
@@ -835,6 +938,11 @@ void finalize_scan(Map* m)
 				launch_upper(m);
 				CK(cudaEventRecord(m->ev[6], m->stream));
 				CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, m->stream));
+			} else if (p.write) {
+				// a brick could not be created while expanding: nothing was applied, grow and repeat
+				m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
+				grow_pools(m, ov & 6u, m->h_ctr->n_bricks, m->h_ctr->n_upper);
+				enqueue_scan(m, p);
 			} else {
 				// an allocation failed while marking: nothing was consumed (K3/K4 backed off).  Grow,
 				// keep the bricks that were created, and run the whole scan again under a new scan id
@@ -2879,6 +2987,211 @@ int ufo_b200_read_data(ufo_b200_map* m, const double* box6, const void* data, si
 			return (int)UFO_B200_E_INVALID;
 		}
 		return import_stream(m, raw.data(), (size_t)n, box6);
+	});
+}
+
+}  // extern "C"
+
+namespace
+{
+// checks shared by the two write entry points (they need no device); returns OK or the status to
+// reject the batch with
+int write_allowed(Map* m, uint32_t depth)
+{
+	if (depth > 6) {
+		m->set_error("write depth %u > 6 is not supported (a node of depth 7 covers 512 bricks of the dense value field)", depth);
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (depth > m->M.g.depth_levels) {
+		m->set_error("write depth %u exceeds the tree's depth_levels %u", depth, m->M.g.depth_levels);
+		return UFO_B200_E_INVALID;
+	}
+	if (m->M.shard_world > 1 || m->M.route_world > 1) {
+		m->set_error("per-node writes on a sharded / routed map are not supported");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (m->poisoned) {
+		m->set_error("an earlier scan failed half-way; ufo_b200_clear() the map before writing again");
+		return UFO_B200_E_INVALID;
+	}
+	return UFO_B200_OK;
+}
+
+bool depth0_key_ok(const Geometry& g, const double p[3])
+{
+	for (int k = 0; k < 3; ++k) {
+		const double kv = std::floor(p[k] * g.resolution_factor) + (double)g.max_value;  // toKey at depth 0
+		if (!(kv >= 0.0 && kv < (double)(1ull << g.depth_levels))) return false;
+	}
+	return true;
+}
+
+// Copies a batch's inputs and record offsets to the device and enqueues it (ufo_write.cuh).
+// `blobs`: host arrays copied back to back into the map's input buffer, each 8-byte aligned;
+// `bind` receives the device address of each blob and stores it into the batch's arguments.
+template <class Bind>
+int do_write(Map* m, WriteArgs w, const std::vector<std::pair<const void*, size_t>>& blobs,
+             const std::vector<unsigned long long>& offs, int async, Bind&& bind)
+{
+	finalize_scan(m);
+	const unsigned long long n_rec = offs.back();
+	if (n_rec > 0x7fffffffull) {
+		m->set_error("write batch needs %llu records (limit 2^31 - 1)", n_rec);
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	cudaStream_t s = m->stream;
+	size_t total = offs.size() * 8;
+	for (const auto& b : blobs) total += (b.second + 7) & ~size_t(7);
+	ensure_dev(m, m->d_w_in, m->w_in_cap, total);
+	size_t at = 0;
+	std::vector<const void*> ptrs;
+	for (const auto& b : blobs) {
+		if (b.second) CK(cudaMemcpyAsync(m->d_w_in + at, b.first, b.second, cudaMemcpyHostToDevice, s));
+		ptrs.push_back(m->d_w_in + at);
+		at += (b.second + 7) & ~size_t(7);
+	}
+	CK(cudaMemcpyAsync(m->d_w_in + at, offs.data(), offs.size() * 8, cudaMemcpyHostToDevice, s));
+	bind(w, ptrs);
+	w.offs = reinterpret_cast<const unsigned long long*>(m->d_w_in + at);
+	w.n_rec = n_rec;
+	if (n_rec > m->w_rec_cap) {
+		for (int i = 0; i < 2; ++i) {
+			if (m->d_w_keys[i]) CK(cudaFree(m->d_w_keys[i]));
+			if (m->d_w_idx[i]) CK(cudaFree(m->d_w_idx[i]));
+		}
+		if (m->d_w_recs) CK(cudaFree(m->d_w_recs));
+		m->device_bytes -= m->w_rec_cap * (2 * 8 + 2 * 4 + sizeof(WriteRec));
+		m->w_rec_cap = 0;
+		const size_t cap = std::max<size_t>(n_rec + n_rec / 8, 1 << 12);
+		for (int i = 0; i < 2; ++i) {
+			dev_alloc(m->d_w_keys[i], cap, 0, s, m->device_bytes);
+			dev_alloc(m->d_w_idx[i], cap, 0, s, m->device_bytes);
+		}
+		dev_alloc(m->d_w_recs, cap, 0, s, m->device_bytes);
+		m->w_rec_cap = cap;
+	}
+	PendingScan& p = m->pending;
+	p = PendingScan{};
+	p.write = true;
+	p.w = w;
+	m->stats = ufo_b200_scan_stats{};
+	m->stats.points = w.n;
+	m->launches = 0;
+	m->h2d_valid = false;
+	CK(cudaEventRecord(m->ev[0], s));
+	// the inputs above were staged from pageable memory: the caller's arrays are free again here
+	enqueue_scan(m, p);
+	if (!async) return sync_map(m);
+	return UFO_B200_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int ufo_b200_update_nodes(ufo_b200_map* m, const uint64_t* codes, const uint32_t* depths, const uint8_t* ops,
+                          const float* values, size_t n, int async)
+{
+	if (!m || (n && (!codes || !depths || !ops || !values)) || n > 0x7fffffffull) return UFO_B200_E_INVALID;
+	for (size_t i = 0; i < n; ++i) {
+		const int rc = write_allowed(m, depths[i]);
+		if (rc != UFO_B200_OK) return rc;
+	}
+	return guarded(m, [&]() {
+		CK(cudaSetDevice(m->device));
+		const Geometry& g = m->M.g;
+		std::vector<unsigned long long> offs(n + 1);
+		unsigned long long tot = 0;
+		for (size_t i = 0; i < n; ++i) {
+			const uint32_t d = depths[i];
+			if (ops[i] > 1) {
+				m->set_error("entry %zu: op %u is neither ADD (0) nor SET (1)", i, (unsigned)ops[i]);
+				return (int)UFO_B200_E_INVALID;
+			}
+			if (ops[i] == 1 && d > 0 && m->M.color) {
+				m->set_error("SET on a colour map is supported at depth 0 only");
+				return (int)UFO_B200_E_UNSUPPORTED;
+			}
+			const Key3 k = code_to_key(codes[i]);
+			if ((((k.x >> d) << d) | ((k.y >> d) << d) | ((k.z >> d) << d)) & ~g.key_mask) {
+				m->set_error("entry %zu: code %llu lies outside the map", i, (unsigned long long)codes[i]);
+				return (int)UFO_B200_E_INVALID;
+			}
+			offs[i] = tot;
+			tot += d <= 4 ? 1ull : 1ull << (3 * (d - 4));
+		}
+		offs[n] = tot;
+		if (!n) {
+			finalize_scan(m);
+			return (int)UFO_B200_OK;
+		}
+		WriteArgs w{};
+		w.n = (uint32_t)n;
+		return do_write(m, w, {{codes, n * 8}, {values, n * 4}, {depths, n * 4}, {ops, n}}, offs, async,
+		                [](WriteArgs& a, const std::vector<const void*>& p) {
+			                a.codes = static_cast<const unsigned long long*>(p[0]);
+			                a.values = static_cast<const float*>(p[1]);
+			                a.depths = static_cast<const uint32_t*>(p[2]);
+			                a.ops = static_cast<const uint8_t*>(p[3]);
+		                });
+	});
+}
+
+int ufo_b200_insert_rays(ufo_b200_map* m, const double* origins, const double* ends, size_t n, double max_range,
+                         uint32_t depth, int hit_end, int async)
+{
+	if (!m || (n && (!origins || !ends)) || n > 0x7fffffffull) return UFO_B200_E_INVALID;
+	const int rc = write_allowed(m, depth);
+	if (rc != UFO_B200_OK) return rc;
+	return guarded(m, [&]() {
+		CK(cudaSetDevice(m->device));
+		const Geometry& g = m->M.g;
+		// record region of every ray: an upper bound of the walk's records.  Every step of the walk
+		// moves one axis by one node, so a walk from key a to key b visits |a - b|_1 + 1 nodes and
+		// enters |a/4 - b/4|_1 + 1 blocks (depth <= 2, one record per block); 2 spare records cover a
+		// walk that stops on the range test instead of on the end node.
+		const uint32_t shift = depth <= 2 ? 2u : depth;
+		const unsigned long long per = depth <= 4 ? 1ull : 1ull << (3 * (depth - 4));
+		std::vector<unsigned long long> offs(n + 1);
+		unsigned long long tot = 0;
+		for (size_t i = 0; i < n; ++i) {
+			const double* po = origins + 3 * i;
+			const double* pe = ends + 3 * i;
+			if (!depth0_key_ok(g, po) || !depth0_key_ok(g, pe)) {
+				m->set_error("ray %zu: origin or end lies outside the map", i);
+				return (int)UFO_B200_E_INVALID;
+			}
+			const Vec3 o = {po[0], po[1], po[2]};
+			Vec3 e = {pe[0], pe[1], pe[2]};
+			Vec3 dir = vsub(e, o);
+			const double dist = vnorm(dir);
+			dir = vdiv(dir, dist);
+			if (0 <= max_range && dist > max_range) e = vadd(o, vscale(dir, max_range));
+			const Key3 a = point_to_key(g, o, depth), b = point_to_key(g, e, depth);
+			const unsigned long long steps = (unsigned long long)std::llabs((long long)(a.x >> shift) - (long long)(b.x >> shift)) +
+			                                 (unsigned long long)std::llabs((long long)(a.y >> shift) - (long long)(b.y >> shift)) +
+			                                 (unsigned long long)std::llabs((long long)(a.z >> shift) - (long long)(b.z >> shift));
+			offs[i] = tot;
+			tot += (steps + 3) * per + (hit_end ? 1 : 0);
+		}
+		offs[n] = tot;
+		if (!n) {
+			finalize_scan(m);
+			return (int)UFO_B200_OK;
+		}
+		WriteArgs w{};
+		w.n = (uint32_t)n;
+		w.rays = 1;
+		w.max_range = max_range;
+		w.depth = depth;
+		w.hit_end = hit_end ? 1u : 0u;
+		// integrateMiss / integrateHit: updateValue(code, float(prob_miss_log_ / prob_hit_log_))
+		w.miss = (float)m->miss_log;
+		w.hit = (float)m->hit_log;
+		return do_write(m, w, {{origins, n * 24}, {ends, n * 24}}, offs, async,
+		                [](WriteArgs& a, const std::vector<const void*>& p) {
+			                a.origins = static_cast<const double*>(p[0]);
+			                a.ends = static_cast<const double*>(p[1]);
+		                });
 	});
 }
 
