@@ -353,10 +353,15 @@ int ufo_b200_set_shard(ufo_b200_map* m, uint32_t rank, uint32_t world);
  * sensor's scan -- and the per-brick free-space masks / hit voxels of bricks another rank owns
  * are written straight into that rank's inbox over NVLink peer memory; the only collective is a
  * barrier between the two calls below (the caller's: e.g. a 4-byte NCCL all-reduce on the map's
- * stream).  Mono maps, insert depth 0, plain (non-discrete) insertion.
+ * stream).  Every option of ufo_b200_insert_pointcloud except early_stopping: mono and colour
+ * maps, discrete insertion, insert depth 0..6, simple_ray_casting (ufo_b200_route_mark_ex).
  *
  *   ufo_b200_route_setup    allocates this rank's inbox (cap_bricks brick records and cap_hits hit
- *                           voxels per source rank and parity) and returns its device pointer
+ *                           records per source rank and parity) and returns its device pointer.
+ *                           Colour maps use 16-byte hit records (voxel key, global cloud index,
+ *                           rgb): ufo_b200_route_inbox_bytes_color gives their inbox size.  A hit
+ *                           record is also what carries a whole brick below an insert-depth-5/6
+ *                           free-space node
  *   ufo_b200_ipc_export/_open   cudaIpc handle of that pointer / mapping of a peer's handle, for
  *                           one-process-per-GPU launches (handles travel through the caller's
  *                           control plane, e.g. torch.distributed.all_gather_object)
@@ -365,21 +370,38 @@ int ufo_b200_set_shard(ufo_b200_map* m, uint32_t rank, uint32_t world);
  *   ufo_b200_route_mark     enqueue: H2D, K1, fused walk, forwarding of foreign marks.  self_too != 0:
  *                           the rank's own marks go through its inbox as well, which lets the
  *                           owner apply several sensors one after the other (clamping makes the
- *                           order matter)
+ *                           order matter).  Mono maps, insert depth 0, plain insertion; a colour
+ *                           map returns UFO_B200_E_UNSUPPORTED
+ *   ufo_b200_route_mark_ex  the same with the options of ufo_b200_insert_pointcloud.  Local point i
+ *                           has the global cloud index index_base + i * index_stride (a contiguous
+ *                           sector: (offset, 1); the interleaved split buf[r::world]: (r, world)).
+ *                           On colour maps the point with the lowest global index of a hit voxel,
+ *                           over all ranks, blends its colour, as on one map; indices have to stay
+ *                           below 2^32 - 1 there.  early_stopping != 0 or depth > 6:
+ *                           UFO_B200_E_UNSUPPORTED; index_stride == 0: UFO_B200_E_INVALID
  *   -- barrier across the ranks, ordered after route_mark on the map's stream --
  *   ufo_b200_route_apply    enqueue: marks received from sources [first_source, first_source +
  *                           n_sources) -> K3; last != 0 additionally runs the inner-node
  *                           propagation and ends the pass.  One scan split over the ranks:
  *                           route_apply(0, world, 1).  One sensor per rank, merged in sensor order:
  *                           route_apply(s, 1, s == world - 1) for s = 0..world-1.
- * The union of the ranks' value fields equals the single-GPU map (tests/test_gpu_route.py).  Pools
- * do not grow during a routed pass: size the map with initial_bricks. */
+ *   ufo_b200_route_sent     waits for the map's stream; counts[0..2] = brick-mask records,
+ *                           whole-brick records and hit records this rank wrote into inboxes
+ *                           (its own included) in its last mark pass
+ * The union of the ranks' value fields equals the single-GPU map (tests/test_gpu_route.py,
+ * tests/test_gpu_route_discrete.py).  Pools do not grow during a routed pass: size the map with
+ * initial_bricks.  Maps that have seen out-of-tree keys are rejected. */
 int ufo_b200_route_inbox_bytes(uint32_t world, uint32_t cap_bricks, uint32_t cap_hits, size_t* bytes);
+int ufo_b200_route_inbox_bytes_color(uint32_t world, uint32_t cap_bricks, uint32_t cap_hits, size_t* bytes);
 int ufo_b200_route_setup(ufo_b200_map* m, uint32_t rank, uint32_t world, uint32_t cap_bricks, uint32_t cap_hits,
                          void** inbox);
 int ufo_b200_route_connect(ufo_b200_map* m, void* const* peer_inboxes);
 int ufo_b200_route_mark(ufo_b200_map* m, const double origin[3], const void* points, size_t n, int layout,
                         double max_range, int on_device, int self_too);
+int ufo_b200_route_mark_ex(ufo_b200_map* m, const double origin[3], const void* points, size_t n, int layout,
+                           double max_range, uint32_t depth, int simple_ray_casting, uint32_t early_stopping,
+                           int discrete, uint64_t index_base, uint32_t index_stride, int on_device, int self_too);
+int ufo_b200_route_sent(ufo_b200_map* m, uint32_t counts[3]);
 int ufo_b200_route_apply(ufo_b200_map* m, uint32_t first_source, uint32_t n_sources, int last);
 int ufo_b200_ipc_export(void* dev_ptr, void* handle64);
 int ufo_b200_ipc_open(const void* handle64, void** dev_ptr);

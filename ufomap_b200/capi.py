@@ -64,6 +64,7 @@ SYMBOLS = [
     "ufo_b200_route_apply", "ufo_b200_ipc_export", "ufo_b200_ipc_open", "ufo_b200_ipc_close",
     "ufo_b200_write_compressed", "ufo_b200_cast_rays", "ufo_b200_export_nodes", "ufo_b200_read_data", "ufo_b200_enable_change_detection", "ufo_b200_reset_change_detection", "ufo_b200_changed_codes",
     "ufo_b200_update_nodes", "ufo_b200_insert_rays",
+    "ufo_b200_route_inbox_bytes_color", "ufo_b200_route_mark_ex", "ufo_b200_route_sent",
 ]
 
 class Cloud2(C.Structure):
@@ -142,6 +143,9 @@ def load():
     lib.ufo_b200_route_connect.argtypes = [vp, C.POINTER(vp)]
     lib.ufo_b200_route_mark.argtypes = [vp, vp, vp, sz, i32, dbl, i32, i32]
     lib.ufo_b200_route_apply.argtypes = [vp, u32, u32, i32]
+    lib.ufo_b200_route_inbox_bytes_color.argtypes = [u32, u32, u32, C.POINTER(sz)]
+    lib.ufo_b200_route_mark_ex.argtypes = [vp, vp, vp, sz, i32, dbl, u32, i32, u32, i32, C.c_uint64, u32, i32, i32]
+    lib.ufo_b200_route_sent.argtypes = [vp, C.POINTER(C.c_uint32 * 3)]
     lib.ufo_b200_ipc_export.argtypes = [vp, vp]
     lib.ufo_b200_ipc_open.argtypes = [vp, C.POINTER(vp)]
     lib.ufo_b200_ipc_close.argtypes = [vp]
@@ -321,6 +325,23 @@ class Map:
         o = np.ascontiguousarray(origin, dtype=np.float64)
         self._check(self.lib.ufo_b200_route_mark(self.h, o.ctypes.data, buf_ptr, int(n), int(layout),
                                                  float(max_range), int(on_device), int(self_too)))
+
+    def route_mark_ex(self, origin, buf_ptr, n, layout, max_range=-1.0, depth=0, simple=False,
+                      early_stopping=0, discrete=False, index_base=0, index_stride=1, on_device=False,
+                      self_too=False):
+        """route_mark with the options of insert (mono and colour maps).  Local point i is point
+        index_base + i * index_stride of the whole cloud: (offset, 1) for a contiguous sector,
+        (rank, world) for buf[rank::world]."""
+        o = np.ascontiguousarray(origin, dtype=np.float64)
+        self._check(self.lib.ufo_b200_route_mark_ex(
+            self.h, o.ctypes.data, buf_ptr, int(n), int(layout), float(max_range), int(depth), int(simple),
+            int(early_stopping), int(discrete), int(index_base), int(index_stride), int(on_device), int(self_too)))
+
+    def route_sent(self):
+        """Records this rank wrote into inboxes in its last mark pass (waits for the map's stream)."""
+        c = (C.c_uint32 * 3)()
+        self._check(self.lib.ufo_b200_route_sent(self.h, C.byref(c)))
+        return {"brick_records": c[0], "full_brick_records": c[1], "hit_records": c[2]}
 
     def route_apply(self, first=0, count=None, last=True):
         count = self.route_world if count is None else count
@@ -582,6 +603,18 @@ def pose_from_rpy(x, y, z, roll, pitch, yaw):
     lib.ufo_b200_pose_from_rpy(float(x), float(y), float(z), float(roll), float(pitch), float(yaw),
                                out.ctypes.data)
     return out
+
+
+def route_inbox_bytes(world, cap_bricks=1 << 16, cap_hits=1 << 18, color=False):
+    """Device bytes of one rank's inbox (Map.route_setup with the same capacities); colour maps
+    carry 16-byte hit records instead of 8."""
+    lib = load()
+    out = C.c_size_t()
+    f = lib.ufo_b200_route_inbox_bytes_color if color else lib.ufo_b200_route_inbox_bytes
+    rc = f(int(world), int(cap_bricks), int(cap_hits), C.byref(out))
+    if rc != 0:
+        raise UfoError(rc, "invalid routed-mode capacities")
+    return out.value
 
 
 def ipc_export(dev_ptr):

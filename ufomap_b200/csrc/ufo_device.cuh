@@ -72,17 +72,24 @@ struct Counters {
 // straight into that rank's inbox over NVLink peer memory (ufo_route.cuh).
 constexpr uint32_t kMaxRanks = 16;
 constexpr uint32_t kMissRecWords = 65;  // brick key + 64 block masks
+// Hit-region record flag: the record is a brick key whose 64 blocks are all free space (insert
+// depth 5/6: a brick below a free-space node), not a voxel key.  Packed keys use bits 0..62.
+constexpr unsigned long long kFullBrick = 1ull << 63;
 struct RouteBox {                       // one (source -> destination) region of one parity, in the destination's memory
 	unsigned long long* miss;             // [cap_m][kMissRecWords]
-	unsigned long long* hit;              // [cap_h] packed voxel keys
+	// [cap_h] hit records.  Mono maps: one word, the packed voxel key.  Colour maps: two words,
+	// {packed voxel key, global cloud index | rgb << 32}; index kNone = a point without colour.
+	unsigned long long* hit;
 	uint32_t* hdr;                        // [0] records, [1] hit keys: published by the source when its pass is complete
 };
 struct RouteTable {
 	RouteBox out[kMaxRanks];  // where this rank's records for rank d go (peer memory)
 	RouteBox in[kMaxRanks];   // where the records of rank s arrive (own memory)
 	uint32_t out_miss[kMaxRanks], out_hit[kMaxRanks];  // cursors of the current pass
+	uint32_t out_full;  // whole-brick records of the current pass (statistics)
 	uint32_t cap_m, cap_h;
 	uint32_t overflow;  // a region was too small
+	uint32_t sent[3];   // last pass, all destinations: mask records, whole-brick records, hit records (read with overflow)
 };
 
 struct DeviceMap {

@@ -254,23 +254,56 @@ __device__ __noinline__ void scatter_slow(const DeviceMap M, const ScanArgs& a, 
 	else mark_alias(M, x >> 2, y >> 2, z >> 2, bits, false);
 }
 
-// one thread per (collected node, brick below it): find-or-create the brick, full miss masks
+// routed mode: one hit-region record into the inbox of rank `owner` (ufo_route.cuh).  `rec` is a
+// packed voxel key or a brick key | kFullBrick; colour maps add the global cloud index and rgb.
+__device__ __forceinline__ void route_hit(const DeviceMap& M, uint32_t owner, unsigned long long rec, uint32_t index,
+                                          uint32_t rgb)
+{
+	RouteTable* R = M.route;
+	const uint32_t i = atomicAdd(&R->out_hit[owner], 1u);
+	if (i >= R->cap_h) {
+		atomicOr(&R->overflow, 1u);
+		return;
+	}
+	if (M.color)
+		*reinterpret_cast<ulonglong2*>(R->out[owner].hit + 2 * (size_t)i) = make_ulonglong2(rec, ((unsigned long long)rgb << 32) | index);
+	else
+		R->out[owner].hit[i] = rec;
+}
+
+// one thread per (collected node, brick below it): find-or-create the brick, full miss masks.
+// Routed mode: a brick another rank owns (or every brick, with route_self) is not created here
+// but sent to its owner as one whole-brick record.
 __global__ void __launch_bounds__(256) k_expand_nodes(DeviceMap M, ScanArgs a)
 {
 	if (ld_volatile_u32(&M.ctr->overflow) & ~4u) return;
 	const uint32_t per = 1u << (3 * (a.depth - 4));  // bricks per node
 	const uint32_t side = 1u << (a.depth - 4);
 	const size_t n = (size_t)min(ld_volatile_u32(&M.ctr->n_dirty), a.nodes_cap) * per;
+	uint32_t sent = 0;
 	for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x) {
 		uint32_t nx, ny, nz;
 		unpack_key(a.nodes[e / per], nx, ny, nz);
 		const uint32_t j = (uint32_t)(e % per);
 		const uint32_t bx = nx * side + (j % side), by = ny * side + ((j / side) % side), bz = nz * side + j / (side * side);
-		const uint32_t brick = brick_find_or_create(M, pack_key(bx, by, bz));
+		const unsigned long long bkey = pack_key(bx, by, bz);
+		if (M.route_world > 1) {
+			const uint32_t owner = brick_owner(bkey, M.route_world);
+			if (owner != M.route_rank || M.route_self) {
+				route_hit(M, owner, bkey | kFullBrick, kNone, 0u);
+				++sent;
+				continue;
+			}
+		}
+		const uint32_t brick = brick_find_or_create(M, bkey);
 		if (brick == kNone) continue;
 		touch_brick(M, brick);
 		ulonglong2* mm = reinterpret_cast<ulonglong2*>(M.miss_mask + (size_t)brick * 64);
 		for (int c = 0; c < 32; ++c) mm[c] = make_ulonglong2(~0ull, ~0ull);
+	}
+	if (M.route_world > 1) {
+		sent = __reduce_add_sync(0xffffffffu, sent);
+		if ((threadIdx.x & 31) == 0 && sent) atomicAdd(&M.route->out_full, sent);
 	}
 }
 
@@ -304,10 +337,7 @@ __device__ __forceinline__ void mark_hit(const DeviceMap& M, Key3 k)
 		// routed mode: the hit voxel goes to the inbox of the rank that owns its brick
 		const uint32_t owner = brick_owner(bkey, M.route_world);
 		if (owner != M.route_rank || M.route_self) {
-			RouteTable* R = M.route;
-			const uint32_t i = atomicAdd(&R->out_hit[owner], 1u);
-			if (i < R->cap_h) R->out[owner].hit[i] = pack_key(k.x, k.y, k.z);
-			else atomicOr(&R->overflow, 1u);
+			route_hit(M, owner, pack_key(k.x, k.y, k.z), kNone, 0u);
 			return;
 		}
 	}
@@ -468,6 +498,29 @@ __global__ void __launch_bounds__(256) k_points(DeviceMap M, ScanArgs a)
 	}
 }
 
+// updateNodeColor (occupancy_map_color.cpp:142-171): blends `upd` into leaf li, weighted by the
+// leaf's occupancy before this scan's update
+__device__ __forceinline__ void blend_color(const DeviceMap& M, size_t li, uint32_t upd)
+{
+	uint32_t cur = M.leaf_rgb[li];
+	if (cur == upd) return;
+	if (cur == 0) {
+		M.leaf_rgb[li] = upd;
+		return;
+	}
+	double prob = M.prob_hit;
+	double total = prob + to_prob(M.leaf[li]);
+	prob = prob / total;
+	double inv = 1.0 - prob;
+	uint32_t out = 0;
+	for (int c = 0; c < 3; ++c) {
+		double cc = (double)((cur >> (8 * c)) & 0xffu), uu = (double)((upd >> (8 * c)) & 0xffu);
+		double r = dop::sqrt(dop::add(dop::mul(dop::mul(cc, cc), inv), dop::mul(dop::mul(uu, uu), prob)));
+		out |= ((uint32_t)(int)r & 0xffu) << (8 * c);
+	}
+	M.leaf_rgb[li] = out;
+}
+
 // K1b: colour maps.  The first point (lowest cloud index) of every hit voxel blends
 // its colour into the leaf BEFORE the occupancy update of this scan
 // (occupancy_map_color.h:269-287) and marks the hit bit.
@@ -506,24 +559,7 @@ __global__ void __launch_bounds__(256) k_hits(DeviceMap M, ScanArgs a)
 	Vec3 p;
 	uint32_t upd;
 	load_point(a, i, p, upd);
-	size_t li = slot * 64 + v;
-	uint32_t cur = M.leaf_rgb[li];
-	if (cur == upd) return;
-	if (cur == 0) {
-		M.leaf_rgb[li] = upd;
-		return;
-	}
-	double prob = M.prob_hit;
-	double total = prob + to_prob(M.leaf[li]);
-	prob = prob / total;
-	double inv = 1.0 - prob;
-	uint32_t out = 0;
-	for (int c = 0; c < 3; ++c) {
-		double cc = (double)((cur >> (8 * c)) & 0xffu), uu = (double)((upd >> (8 * c)) & 0xffu);
-		double r = dop::sqrt(dop::add(dop::mul(dop::mul(cc, cc), inv), dop::mul(dop::mul(uu, uu), prob)));
-		out |= ((uint32_t)(int)r & 0xffu) << (8 * c);
-	}
-	M.leaf_rgb[li] = out;
+	blend_color(M, slot * 64 + v, upd);
 }
 
 // ---------------------------------------------------------------------------

@@ -98,6 +98,7 @@ struct PendingScan {
 	ScanArgs a{};
 	bool use_color = false, need_table = false, simple = false, has_vol = false;
 	bool routed = false;  // routed multi-GPU pass: cannot be repeated locally after a pool overflow
+	bool applying = false;  // routed pass: the first apply call has run
 	bool dense = false;   // marks go to the dense scan volume
 	VolumeArgs vol{};
 	float set_value = 0.0f;
@@ -174,7 +175,11 @@ struct ufo_b200_map {
 	size_t route_region = 0, route_miss_off = 0, route_hit_off = 0;
 	void* route_peer[kMaxRanks] = {};
 	RouteTable* h_route = nullptr;  // pinned mirror, pushed before every mark pass
-	uint32_t* h_route_flag = nullptr;
+	uint32_t* h_route_flag = nullptr;  // pinned: RouteTable::overflow, then ::sent[3] of the last mark pass
+	// colour maps: apply table (minimum global cloud index per hit voxel of one apply call)
+	unsigned long long* d_route_tab_keys = nullptr;
+	uint32_t* d_route_tab_min = nullptr;
+	uint32_t route_tab_size = 0;
 	uint32_t route_parity = 0, route_cap_m = 0, route_cap_h = 0;
 	int route_stage = 0;  // 0 idle, 1 marked (waiting for the apply calls), 2 applied
 	double min_change[3], max_change[3];
@@ -287,7 +292,7 @@ void free_pools(Map* m)
 	                m->d_list[1], m->d_points[0], m->d_points[1], m->d_ray_end, m->d_hit_tab, m->d_tab_keys, m->d_tab_min,
 	                m->d_seg, m->d_seg_base, m->d_seg_count, m->d_order, m->d_nodes, m->d_items, m->d_vmask, m->d_rc,
 	                m->d_w_in, m->d_w_keys[0], m->d_w_keys[1], m->d_w_idx[0], m->d_w_idx[1], m->d_w_recs, m->d_w_seg,
-	                m->d_w_tmp};
+	                m->d_w_tmp, m->d_route_tab_keys, m->d_route_tab_min};
 	for (void* p : ptrs)
 		if (p) cudaFree(p);
 }
@@ -794,25 +799,11 @@ void enqueue_write(Map* m, PendingScan& p)
 	p.valid = true;
 }
 
-// Enqueues every kernel of one scan and the read-back of its counters; never waits.
-void enqueue_scan(Map* m, PendingScan& p)
+// (re-)binds the scan buffers to the scan's arguments: they may have been regrown since the scan
+// was first enqueued
+void bind_scan_buffers(Map* m, PendingScan& p, bool fused)
 {
-	if (p.write) {
-		enqueue_write(m, p);
-		return;
-	}
-	m->write_pass = false;
-	DeviceMap& M = m->M;
-	cudaStream_t s = m->stream;
 	ScanArgs& a = p.a;
-	M.scan_id++;
-	if (M.scan_id == 0) M.scan_id = 1;
-	M.up_epoch++;
-	if (M.up_epoch == 0) M.up_epoch = 1;
-	const bool fused = use_fused(m, p);
-	M.dense = (fused && p.dense) ? 1u : 0u;
-	M.mask_base = M.dense ? M.vol : M.miss_mask;
-	// (re-)bind the scan buffers: they may have been regrown since the scan was first enqueued
 	a.ray_end = m->d_ray_end;
 	a.tab_keys = m->d_tab_keys;
 	a.tab_min = m->d_tab_min;
@@ -834,10 +825,31 @@ void enqueue_scan(Map* m, PendingScan& p)
 		a.order = m->d_order;
 	}
 	if (a.depth >= 5) {
-		if (!m->d_nodes) dev_alloc(m->d_nodes, (size_t)1 << 20, 0, s, m->device_bytes);
+		if (!m->d_nodes) dev_alloc(m->d_nodes, (size_t)1 << 20, 0, m->stream, m->device_bytes);
 		a.nodes = m->d_nodes;
 		a.nodes_cap = 1u << 20;
 	}
+}
+
+// Enqueues every kernel of one scan and the read-back of its counters; never waits.
+void enqueue_scan(Map* m, PendingScan& p)
+{
+	if (p.write) {
+		enqueue_write(m, p);
+		return;
+	}
+	m->write_pass = false;
+	DeviceMap& M = m->M;
+	cudaStream_t s = m->stream;
+	ScanArgs& a = p.a;
+	M.scan_id++;
+	if (M.scan_id == 0) M.scan_id = 1;
+	M.up_epoch++;
+	if (M.up_epoch == 0) M.up_epoch = 1;
+	const bool fused = use_fused(m, p);
+	M.dense = (fused && p.dense) ? 1u : 0u;
+	M.mask_base = M.dense ? M.vol : M.miss_mask;
+	bind_scan_buffers(m, p, fused);
 	m->ev7_valid = false;
 	push_counters(m);
 	if (p.need_table) {
@@ -1189,11 +1201,13 @@ int do_insert(Map* m, const double origin[3], const void* points, bool on_device
 }
 
 // ---- routed multi-GPU mode (ufo_route.cuh) -------------------------------------------------
-size_t route_layout(uint32_t world, uint32_t cap_m, uint32_t cap_h, size_t* region, size_t* miss_off, size_t* hit_off)
+// hit_words: 1 for mono maps (packed voxel key), 2 for colour maps (+ global cloud index and rgb)
+size_t route_layout(uint32_t world, uint32_t cap_m, uint32_t cap_h, uint32_t hit_words, size_t* region, size_t* miss_off,
+                    size_t* hit_off)
 {
 	const size_t mo = 256;
 	const size_t ho = mo + (((size_t)cap_m * kMissRecWords * 8 + 255) & ~(size_t)255);
-	const size_t reg = ho + (((size_t)cap_h * 8 + 255) & ~(size_t)255);
+	const size_t reg = ho + (((size_t)cap_h * 8 * hit_words + 255) & ~(size_t)255);
 	if (region) *region = reg;
 	if (miss_off) *miss_off = mo;
 	if (hit_off) *hit_off = ho;
@@ -1220,8 +1234,12 @@ void route_fill_table(Map* m)
 	}
 }
 
+// The mark phase of a routed pass.  Takes every option of do_insert except early_stopping, frames and
+// PointCloud2 records; `ex` = false is ufo_b200_route_mark (mono maps only).  Local point i has the
+// global cloud index index_base + i * index_stride (colour maps: it picks the voxel's colour winner).
 int do_route_mark(Map* m, const double origin[3], const void* points, bool on_device, size_t n, int layout,
-                  double max_range, int self_too)
+                  double max_range, uint32_t depth, int simple, uint32_t early_stopping, int discrete,
+                  uint64_t index_base, uint32_t index_stride, int self_too, bool ex)
 {
 	if (!m || !origin || (!points && n)) return UFO_B200_E_INVALID;
 	const size_t stride = layout_stride(layout);
@@ -1231,10 +1249,29 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 		m->set_error("routed mode is not set up (ufo_b200_route_setup + ufo_b200_route_connect)");
 		return UFO_B200_E_INVALID;
 	}
-	if (M.color || M.alias_miss || m->poisoned || m->route_stage == 1) {
-		m->set_error(m->route_stage == 1 ? "ufo_b200_route_mark: the previous pass was not applied"
-		                                 : "routed mode needs a healthy mono map without out-of-tree keys");
+	if (early_stopping != 0) {
+		m->set_error("early_stopping is order-dependent in the reference (occupancy_map_base.h:1289-1298) and is not supported");
 		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (depth > 6) {
+		m->set_error("insert depth %u > 6 is not supported", depth);
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (index_stride == 0) {
+		m->set_error("ufo_b200_route_mark_ex: index_stride must be at least 1");
+		return UFO_B200_E_INVALID;
+	}
+	if ((!ex && M.color) || M.alias_miss || m->poisoned || m->route_stage == 1) {
+		m->set_error(m->route_stage == 1 ? "ufo_b200_route_mark: the previous pass was not applied"
+		             : (!ex && M.color) ? "ufo_b200_route_mark takes mono maps; colour maps use ufo_b200_route_mark_ex"
+		                                : "routed mode needs a healthy map without out-of-tree keys");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	const bool has_rgb = layout == UFO_B200_XYZRGB_F64 || layout == UFO_B200_XYZRGB_F32;
+	const bool use_color = M.color && has_rgb;
+	if (use_color && n && (index_base >= kNone || (uint64_t)(n - 1) > (kNone - 1 - index_base) / index_stride)) {
+		m->set_error("ufo_b200_route_mark_ex: global cloud indices must stay below 2^32 - 1");
+		return UFO_B200_E_INVALID;
 	}
 	CK(cudaSetDevice(m->device));
 	const size_t bytes = n * stride;
@@ -1260,15 +1297,24 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 	PendingScan& p = m->pending;
 	p = PendingScan{};
 	p.routed = true;
+	p.use_color = use_color;
+	p.need_table = discrete || use_color || depth >= 5;  // as do_insert
+	p.simple = simple != 0;
 	ScanArgs& a = p.a;
 	a.origin = {origin[0], origin[1], origin[2]};
 	a.max_range = max_range;
 	a.n = (uint32_t)n;
+	a.depth = depth;
 	a.layout = layout;
-	a.miss = (float)m->miss_log;
+	a.discrete = discrete;
+	a.use_color = use_color;
+	a.miss = (float)(m->miss_log / (double)((2.0 * depth) + 1));
 	a.count_visits = m->profiling >= 2;
-	ensure_scan_buffers(m, n, false, false, true);
-	{
+	// the marking path is chosen as for a single-GPU insert
+	const bool fused = use_fused(m, p);
+	const bool records = !fused && !p.simple;
+	ensure_scan_buffers(m, n, p.need_table, records, fused);
+	if (fused) {
 		const uint32_t db = volume_bricks(m, p);
 		p.dense = db != 0;
 		if (p.dense) setup_volume(m, p, db);
@@ -1277,11 +1323,10 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 	M.mask_base = M.dense ? M.vol : M.miss_mask;
 	a.points = on_device ? points : m->d_points[stg];
 	if (copied) m->stage = stg;
-	a.ray_end = m->d_ray_end;
-	a.items = m->d_items;
-	a.item_stride = m->item_cap;
-	a.vmask = m->d_vmask;
-	a.rc = m->d_rc;
+	bind_scan_buffers(m, p, fused);
+	// a routed pass cannot be repeated after a record buffer overflow: K1 reserves without a
+	// bound, and the buffer is sized to the reservation before the walk (below)
+	if (records) a.seg_cap = ~0ull;
 	m->stats = ufo_b200_scan_stats{};
 	m->stats.points = n;
 	m->launches = 0;
@@ -1290,18 +1335,38 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 	M.route_self = self_too ? 1u : 0u;
 	m->route_parity ^= 1u;
 	route_fill_table(m);
-	*m->h_route_flag = 0;
+	m->h_route_flag[0] = 0;
 	CK(cudaEventRecord(m->ev[0], s));
 	CK(cudaMemcpyAsync(M.route, m->h_route, sizeof(RouteTable), cudaMemcpyHostToDevice, s));
 	if (copied) CK(cudaStreamWaitEvent(s, m->ev_copied, 0));
 	M.scan_id += 1;
 	if (M.scan_id == 0) M.scan_id = 1;
 	push_counters(m);
+	if (p.need_table) {
+		CK(cudaMemsetAsync(m->d_tab_keys, 0xff, (size_t)m->tab_size * sizeof(unsigned long long), s));
+		CK(cudaMemsetAsync(m->d_tab_min, 0xff, (size_t)m->tab_size * sizeof(uint32_t), s));
+	}
 	if (n) {
-		k_points<<<(uint32_t)((n + 255) / 256), 256, 0, s>>>(M, a);
+		const uint32_t grid = (uint32_t)((n + 255) / 256);
+		k_points<<<grid, 256, 0, s>>>(M, a);
 		++m->launches;
+		if (use_color) {
+			k_route_hits<<<grid, 256, 0, s>>>(M, a, (unsigned long long)index_base, index_stride);
+			++m->launches;
+		}
 		if (m->profiling) CK(cudaEventRecord(m->ev[2], s));
-		launch_rays_fused(m, a);
+		if (fused) {
+			launch_rays_fused(m, a);
+		} else {
+			if (records) {
+				CK(cudaMemcpyAsync(&m->h_ctr->seg_total, &M.ctr->seg_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+				CK(cudaStreamSynchronize(s));
+				ensure_seg(m, std::max<unsigned long long>(m->h_ctr->seg_total, 1024));
+				a.seg = m->d_seg;
+				a.seg_cap = m->seg_cap;
+			}
+			launch_rays_records(m, a, p.simple);
+		}
 	} else if (m->profiling) {
 		CK(cudaEventRecord(m->ev[2], s));
 	}
@@ -1310,7 +1375,7 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 	m->launches += 2;
 	if (m->profiling) CK(cudaEventRecord(m->ev[3], s));
 	CK(cudaGetLastError());
-	CK(cudaMemcpyAsync(m->h_route_flag, &M.route->overflow, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+	CK(cudaMemcpyAsync(m->h_route_flag, &M.route->overflow, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
 	CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
 	p.valid = true;
 	m->route_stage = 1;
@@ -1334,19 +1399,33 @@ int do_route_apply(Map* m, uint32_t first, uint32_t count, int last)
 	// following ones from an empty list
 	M.scan_id += 1;
 	if (M.scan_id == 0) M.scan_id = 1;
-	if (!p.a.seg_cap) {  // first apply call of this pass (seg_cap is unused in routed passes: reused as a flag)
+	if (!p.applying) {
 		std::swap(M.touched, M.touched_alt);
 		std::swap(M.touched_mi, M.touched_alt_mi);
 		M.dense = 0;
 		M.mask_base = M.miss_mask;
 		M.up_epoch++;
 		if (M.up_epoch == 0) M.up_epoch = 1;
-		p.a.seg_cap = 1;
+		p.applying = true;
 	} else {
 		CK(cudaMemsetAsync(&M.ctr->n_touched, 0, sizeof(uint32_t), s));
 	}
-	k_inbox<<<m->sm_count * 4, 256, 0, s>>>(M, first, count);
+	ScanArgs t{};
+	if (M.color) {
+		// apply table for the hit records of these sources: at most count * cap_h keys, half full
+		const uint32_t size = std::min(m->route_tab_size, std::max(1u << 12, next_pow2(2ull * count * m->route_cap_h)));
+		CK(cudaMemsetAsync(m->d_route_tab_keys, 0xff, (size_t)size * sizeof(unsigned long long), s));
+		CK(cudaMemsetAsync(m->d_route_tab_min, 0xff, (size_t)size * sizeof(uint32_t), s));
+		t.tab_keys = m->d_route_tab_keys;
+		t.tab_min = m->d_route_tab_min;
+		t.tab_mask = size - 1;
+	}
+	k_inbox<<<m->sm_count * 4, 256, 0, s>>>(M, first, count, t);
 	++m->launches;
+	if (M.color) {
+		k_inbox_color<<<m->sm_count * 4, 256, 0, s>>>(M, first, count, t);
+		++m->launches;
+	}
 	launch_update(m, p.a.miss, false);
 	launch_upper_seed(m);
 	if (last) {
@@ -2435,7 +2514,14 @@ int ufo_b200_clear_resize(ufo_b200_map* m, double resolution, uint32_t depth_lev
 int ufo_b200_route_inbox_bytes(uint32_t world, uint32_t cap_bricks, uint32_t cap_hits, size_t* bytes)
 {
 	if (!bytes || world < 2 || world > kMaxRanks || !cap_bricks || !cap_hits) return UFO_B200_E_INVALID;
-	*bytes = route_layout(world, cap_bricks, cap_hits, nullptr, nullptr, nullptr);
+	*bytes = route_layout(world, cap_bricks, cap_hits, 1, nullptr, nullptr, nullptr);
+	return UFO_B200_OK;
+}
+
+int ufo_b200_route_inbox_bytes_color(uint32_t world, uint32_t cap_bricks, uint32_t cap_hits, size_t* bytes)
+{
+	if (!bytes || world < 2 || world > kMaxRanks || !cap_bricks || !cap_hits) return UFO_B200_E_INVALID;
+	*bytes = route_layout(world, cap_bricks, cap_hits, 2, nullptr, nullptr, nullptr);
 	return UFO_B200_OK;
 }
 
@@ -2446,19 +2532,28 @@ int ufo_b200_route_setup(ufo_b200_map* m, uint32_t rank, uint32_t world, uint32_
 	return guarded(m, [&]() {
 		CK(cudaSetDevice(m->device));
 		sync_map(m);
-		if (m->n_bricks != 0 || m->route_inbox || m->M.shard_world > 1 || m->M.color) {
-			m->set_error("ufo_b200_route_setup: needs an empty, unsharded mono map and may be called once");
+		if (m->n_bricks != 0 || m->route_inbox || m->M.shard_world > 1) {
+			m->set_error("ufo_b200_route_setup: needs an empty, unsharded map and may be called once");
 			return (int)UFO_B200_E_INVALID;
 		}
-		const size_t total = route_layout(world, cap_bricks, cap_hits, &m->route_region, &m->route_miss_off, &m->route_hit_off);
+		const uint32_t hit_words = m->M.color ? 2u : 1u;
+		const size_t total = route_layout(world, cap_bricks, cap_hits, hit_words, &m->route_region, &m->route_miss_off,
+		                                  &m->route_hit_off);
 		CK(cudaMalloc(reinterpret_cast<void**>(&m->route_inbox), total));
 		CK(cudaMemset(m->route_inbox, 0, total));
 		CK(cudaMalloc(reinterpret_cast<void**>(&m->M.route), sizeof(RouteTable)));
 		CK(cudaMemset(m->M.route, 0, sizeof(RouteTable)));
 		CK(cudaHostAlloc(reinterpret_cast<void**>(&m->h_route), sizeof(RouteTable), cudaHostAllocDefault));
-		CK(cudaHostAlloc(reinterpret_cast<void**>(&m->h_route_flag), sizeof(uint32_t), cudaHostAllocDefault));
-		*m->h_route_flag = 0;
+		CK(cudaHostAlloc(reinterpret_cast<void**>(&m->h_route_flag), 4 * sizeof(uint32_t), cudaHostAllocDefault));
+		memset(m->h_route_flag, 0, 4 * sizeof(uint32_t));
 		m->device_bytes += total + sizeof(RouteTable);
+		if (m->M.color) {
+			// apply table: every hit record of every source of one apply call, at most half full
+			m->route_tab_size = std::max(1u << 12, next_pow2(2ull * world * cap_hits));
+			dev_alloc(m->d_route_tab_keys, m->route_tab_size, 0xff, m->stream, m->device_bytes);
+			dev_alloc(m->d_route_tab_min, m->route_tab_size, 0xff, m->stream, m->device_bytes);
+			CK(cudaStreamSynchronize(m->stream));
+		}
 		m->route_cap_m = cap_bricks;
 		m->route_cap_h = cap_hits;
 		m->M.route_rank = rank;
@@ -2481,7 +2576,34 @@ int ufo_b200_route_connect(ufo_b200_map* m, void* const* peer_inboxes)
 int ufo_b200_route_mark(ufo_b200_map* m, const double origin[3], const void* points, size_t n, int layout,
                         double max_range, int on_device, int self_too)
 {
-	return guarded(m, [&]() { return do_route_mark(m, origin, points, on_device != 0, n, layout, max_range, self_too); });
+	return guarded(m, [&]() {
+		return do_route_mark(m, origin, points, on_device != 0, n, layout, max_range, 0, 0, 0, 0, 0, 1, self_too, false);
+	});
+}
+
+int ufo_b200_route_mark_ex(ufo_b200_map* m, const double origin[3], const void* points, size_t n, int layout,
+                           double max_range, uint32_t depth, int simple_ray_casting, uint32_t early_stopping,
+                           int discrete, uint64_t index_base, uint32_t index_stride, int on_device, int self_too)
+{
+	return guarded(m, [&]() {
+		return do_route_mark(m, origin, points, on_device != 0, n, layout, max_range, depth, simple_ray_casting,
+		                     early_stopping, discrete, index_base, index_stride, self_too, true);
+	});
+}
+
+int ufo_b200_route_sent(ufo_b200_map* m, uint32_t counts[3])
+{
+	if (!m || !counts) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() {
+		if (!m->h_route_flag) {
+			m->set_error("routed mode is not set up");
+			return (int)UFO_B200_E_INVALID;
+		}
+		CK(cudaSetDevice(m->device));
+		CK(cudaStreamSynchronize(m->stream));
+		for (int i = 0; i < 3; ++i) counts[i] = m->h_route_flag[1 + i];
+		return (int)UFO_B200_OK;
+	});
 }
 
 int ufo_b200_route_apply(ufo_b200_map* m, uint32_t first_source, uint32_t n_sources, int last)

@@ -15,6 +15,23 @@
 // followed by the ordinary K3 / K4 over the touched list.  With route_self the rank's own marks
 // take the same way, so that the owner can apply the sensors ONE AFTER THE OTHER in sensor order
 // (clamping makes the order matter): k_inbox(source s) + K3 for s = 0..G-1.
+//
+// Every marking path of a single-GPU insert works here (fused, record, fixed-step; discrete; insert
+// depth 0-6); the record paths mark through the brick hash, which k_outbox reads like the fused
+// walk's non-dense marks.  Two kinds of hit-region record come on top of the voxel keys:
+//   whole bricks   insert depth 5/6: k_expand_nodes does not create the bricks another rank owns
+//                  below a free-space node; it sends the brick key | kFullBrick, and k_inbox sets
+//                  all 64 masks on the owner (a node collected by several ranks arrives several
+//                  times: OR is idempotent)
+//   colour hits    only the point with the lowest GLOBAL cloud index of a hit voxel blends its
+//                  colour (occupancy_map_color.h:269-287), and that point may sit on any rank.
+//                  k_route_hits sends each rank's own winner (the scan table's minimum) with its
+//                  global index and rgb -- own voxels included, since the owner cannot blend before
+//                  it has seen the other ranks' candidates.  k_inbox takes the minimum index per
+//                  voxel over the sources of the apply call (apply table, atomicMin) and
+//                  k_inbox_color lets the winner blend and set the hit bit, before K3 of those
+//                  sources.  Applied per source (merge mode), this is the single map inserting the
+//                  sensors' clouds one after the other.
 // Inbox regions are double-buffered by scan parity; the barrier of scan k+1 orders the reads of
 // scan k before the writes of scan k+2.
 #pragma once
@@ -71,14 +88,22 @@ __global__ void k_outbox_publish(DeviceMap M)
 {
 	RouteTable* R = M.route;
 	const uint32_t d = threadIdx.x;
+	uint32_t nm = 0, nh = 0;
 	if (d < M.route_world) {
-		const uint32_t nm = min(R->out_miss[d], R->cap_m), nh = min(R->out_hit[d], R->cap_h);
+		nm = min(R->out_miss[d], R->cap_m);
+		nh = min(R->out_hit[d], R->cap_h);
 		R->out[d].hdr[0] = nm;
 		R->out[d].hdr[1] = nh;
 		R->out_miss[d] = 0;
 		R->out_hit[d] = 0;
 	}
+	nm = __reduce_add_sync(0xffffffffu, nm);
+	nh = __reduce_add_sync(0xffffffffu, nh);
 	if (d == 0) {
+		R->sent[0] = nm;
+		R->sent[1] = R->out_full;
+		R->sent[2] = nh - R->out_full;
+		R->out_full = 0;
 		// the apply phase starts from the own bricks that kept local marks
 		M.ctr->n_touched = M.ctr->n_touched_alt;
 		M.ctr->n_touched_alt = 0;
@@ -86,13 +111,36 @@ __global__ void k_outbox_publish(DeviceMap M)
 	__threadfence_system();
 }
 
-// applies the records of sources [first, first + count)
-__global__ void __launch_bounds__(256) k_inbox(DeviceMap M, uint32_t first, uint32_t count)
+// K1b of a routed colour pass: every hit voxel's winner on this rank (lowest local index, as k_hits)
+// goes to the voxel's owner with its global cloud index index_base + i * index_stride and its rgb
+__global__ void __launch_bounds__(256) k_route_hits(DeviceMap M, ScanArgs a, unsigned long long index_base,
+                                                     uint32_t index_stride)
+{
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= a.n) return;
+	const uint32_t t = a.hit_tab[i];
+	if (t == kNone || a.tab_min[t] != i) return;
+	const Key3 k = code_to_key(a.tab_keys[t]);
+	if ((k.x | k.y | k.z) & ~M.g.key_mask) {
+		atomicOr(&M.ctr->overflow, 32u);  // out-of-tree key: routed maps do not take them
+		return;
+	}
+	Vec3 p;
+	uint32_t rgb;
+	load_point(a, i, p, rgb);
+	const uint32_t owner = brick_owner(pack_key(k.x >> 4, k.y >> 4, k.z >> 4), M.route_world);
+	route_hit(M, owner, pack_key(k.x, k.y, k.z), (uint32_t)(index_base + (unsigned long long)i * index_stride), rgb);
+}
+
+// applies the records of sources [first, first + count).  Colour maps: hit records only enter the
+// apply table t (minimum global index per voxel); k_inbox_color applies them.
+__global__ void __launch_bounds__(256) k_inbox(DeviceMap M, uint32_t first, uint32_t count, ScanArgs t)
 {
 	const uint32_t lane = threadIdx.x & 31;
 	constexpr uint32_t FULL = 0xffffffffu;
 	const RouteTable* R = M.route;
 	const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, warps = (gridDim.x * blockDim.x) >> 5;
+	const uint32_t hw = M.color ? 2u : 1u;  // words per hit record
 	for (uint32_t s = first; s < first + count; ++s) {
 		const RouteBox box = R->in[s];
 		const uint32_t nm = ld_volatile_u32(&box.hdr[0]), nh = ld_volatile_u32(&box.hdr[1]);
@@ -111,12 +159,55 @@ __global__ void __launch_bounds__(256) k_inbox(DeviceMap M, uint32_t first, uint
 			if (m1) atomicOr(mp + 1, m1);
 		}
 		for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nh; i += gridDim.x * blockDim.x) {
+			const unsigned long long rec = box.hit[(size_t)i * hw];
+			if (rec & kFullBrick) {
+				const uint32_t brick = brick_find_or_create(M, rec & ~kFullBrick);
+				if (brick == kNone) continue;
+				touch_brick(M, brick);
+				ulonglong2* mm = reinterpret_cast<ulonglong2*>(M.miss_mask + (size_t)brick * 64);
+				for (int c = 0; c < 32; ++c) mm[c] = make_ulonglong2(~0ull, ~0ull);
+				continue;
+			}
 			uint32_t x, y, z;
-			unpack_key(box.hit[i], x, y, z);
+			unpack_key(rec, x, y, z);
 			const uint32_t brick = brick_find_or_create(M, pack_key(x >> 4, y >> 4, z >> 4));
 			if (brick == kNone) continue;
 			touch_brick(M, brick);
+			if (M.color) {
+				bool fresh;
+				const uint32_t ts = table_insert(t, rec, &fresh);
+				atomicMin(&t.tab_min[ts], (uint32_t)box.hit[2 * (size_t)i + 1]);
+				continue;
+			}
 			atomicOr(&M.hit_mask[(size_t)brick * 64 + morton2(x >> 2, y >> 2, z >> 2)], 1ull << linear2(x, y, z));
+		}
+	}
+}
+
+// colour maps, after k_inbox: the record that holds its voxel's minimum global index sets the hit
+// bit and blends its colour, as k_hits does on one GPU (same guard against blending twice)
+__global__ void __launch_bounds__(256) k_inbox_color(DeviceMap M, uint32_t first, uint32_t count, ScanArgs t)
+{
+	const RouteTable* R = M.route;
+	for (uint32_t s = first; s < first + count; ++s) {
+		const RouteBox box = R->in[s];
+		const uint32_t nh = ld_volatile_u32(&box.hdr[1]);
+		for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nh; i += gridDim.x * blockDim.x) {
+			const ulonglong2 r = reinterpret_cast<const ulonglong2*>(box.hit)[i];
+			if (r.x & kFullBrick) continue;
+			const uint32_t index = (uint32_t)r.y;
+			bool fresh;
+			const uint32_t ts = table_insert(t, r.x, &fresh);
+			if (t.tab_min[ts] != index) continue;
+			uint32_t x, y, z;
+			unpack_key(r.x, x, y, z);
+			const uint32_t brick = brick_find(M, pack_key(x >> 4, y >> 4, z >> 4));
+			if (brick == kNone) continue;
+			const size_t slot = (size_t)brick * 64 + morton2(x >> 2, y >> 2, z >> 2);
+			const unsigned long long hbit = 1ull << linear2(x, y, z);
+			const unsigned long long old = atomicOr(&M.hit_mask[slot], hbit);
+			if ((old & hbit) || index == kNone) continue;  // already blended, or a point without colour
+			blend_color(M, slot * 64 + morton2(x, y, z), (uint32_t)(r.y >> 32));
 		}
 	}
 }
