@@ -330,6 +330,18 @@ int ufo_b200_last_scan_stats(ufo_b200_map* m, ufo_b200_scan_stats* out);
  * when scan k was enqueued).  For callers that stream scans with async = 1 and still want each
  * scan's result.  points == 0 in *out: no scan has completed yet. */
 int ufo_b200_completed_scan_stats(ufo_b200_map* m, ufo_b200_scan_stats* out);
+
+/* What the fused ray walk sent to the dense scan volume in the most recent insert (waits for it
+ * to finish).  Counted at profiling level 2 only; all zero otherwise, and for scans that took
+ * another marking path (generic record path, brick-hash probes, routed passes without a volume). */
+typedef struct {
+	uint64_t records;          /* block records pushed: a ray segment left a 4^3 block or ended */
+	uint64_t mask_reductions;  /* global 64-bit OR reductions on block masks (records merged per word first) */
+	uint64_t words_marked;     /* of those, the ones that found the word empty: distinct words the walk marked */
+	uint64_t dirty_reductions; /* reductions on the bitmap of touched bricks */
+} ufo_b200_walk_stats;
+int ufo_b200_last_walk_stats(ufo_b200_map* m, ufo_b200_walk_stats* out);
+
 /* Octree::clear(resolution, depth_levels)  octree.h:541-560 -- the server's reset service
  * (server.cpp:364-378): empties the map and changes its geometry. */
 int ufo_b200_clear_resize(ufo_b200_map* m, double resolution, uint32_t depth_levels);

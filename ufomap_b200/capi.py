@@ -47,6 +47,13 @@ class ScanStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class WalkStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("records", "mask_reductions", "words_marked", "dirty_reductions")]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 # every symbol include/ufomap_b200.h declares
 SYMBOLS = [
     "ufo_b200_default_params", "ufo_b200_create", "ufo_b200_destroy", "ufo_b200_last_error",
@@ -65,6 +72,7 @@ SYMBOLS = [
     "ufo_b200_write_compressed", "ufo_b200_cast_rays", "ufo_b200_export_nodes", "ufo_b200_read_data", "ufo_b200_enable_change_detection", "ufo_b200_reset_change_detection", "ufo_b200_changed_codes",
     "ufo_b200_update_nodes", "ufo_b200_insert_rays",
     "ufo_b200_route_inbox_bytes_color", "ufo_b200_route_mark_ex", "ufo_b200_route_sent",
+    "ufo_b200_last_walk_stats",
 ]
 
 class Cloud2(C.Structure):
@@ -129,6 +137,7 @@ def load():
     lib.ufo_b200_reset_change_bbox.argtypes = [vp]
     lib.ufo_b200_last_scan_stats.argtypes = [vp, C.POINTER(ScanStats)]
     lib.ufo_b200_completed_scan_stats.argtypes = [vp, C.POINTER(ScanStats)]
+    lib.ufo_b200_last_walk_stats.argtypes = [vp, C.POINTER(WalkStats)]
     lib.ufo_b200_set_sensor_model_field.argtypes = [vp, i32, dbl]
     lib.ufo_b200_set_profiling.argtypes = [vp, i32]
     lib.ufo_b200_write_compressed.argtypes = [vp, vp, u32, i32, i32, i32, vp, sz, C.POINTER(sz), C.POINTER(sz)]
@@ -295,6 +304,13 @@ class Map:
         """Statistics of the last COMPLETED scan (no wait for the scan in flight)."""
         st = ScanStats()
         self._check(self.lib.ufo_b200_completed_scan_stats(self.h, C.byref(st)))
+        return st.as_dict()
+
+    def walk_stats(self):
+        """What the fused walk of the last insert sent to the scan volume (profiling level 2):
+        records pushed, mask reductions issued, words they found empty, dirty-bit reductions."""
+        st = WalkStats()
+        self._check(self.lib.ufo_b200_last_walk_stats(self.h, C.byref(st)))
         return st.as_dict()
 
     def set_sensor_model_field(self, index, probability):

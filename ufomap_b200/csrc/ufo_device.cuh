@@ -62,6 +62,9 @@ struct Counters {
 	unsigned long long touched_bricks;
 	unsigned long long upper_nodes;
 	unsigned long long bbox[6];  // order-preserving encoding of min xyz / max xyz of this scan
+	// dense fused walk, profiling level 2 only (k_walk_mark<COUNT = true>): block records pushed,
+	// global mask reductions issued, of those the ones that found the word empty, dirty-bit reductions
+	unsigned long long walk_records, walk_mask_reds, walk_words, walk_dirty_reds;
 	// k_update statistics spread over slots: [slot][0 voxels, 1 hit voxels, 2 octets, 3 blocks,
 	// 4 first-touched blocks, 5 bricks, 6 depth-3 nodes, 7 touched 128 B leaf lines]
 	unsigned long long stat[64][8];

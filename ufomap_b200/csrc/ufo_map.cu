@@ -166,6 +166,7 @@ struct ufo_b200_map {
 	bool ev_valid = false, ev7_valid = false, h2d_valid = false;
 	ufo_b200_scan_stats stats{};       // scan in flight / last scan
 	ufo_b200_scan_stats done_stats{};  // last scan whose counters are folded into the host view
+	ufo_b200_walk_stats walk_stats{};  // last scan, profiling level 2
 	bool stats_pending = false;
 	PendingScan pending;
 	bool poisoned = false;
@@ -468,6 +469,7 @@ void finish_stats(Map* m)
 		for (int k = 0; k < 8; ++k) sum[k] += c.stat[sl][k];
 	st.rays = c.n_rays;
 	st.visits = c.visits;
+	m->walk_stats = ufo_b200_walk_stats{c.walk_records, c.walk_mask_reds, c.walk_words, c.walk_dirty_reds};
 	st.touched_voxels = sum[0];
 	st.hit_voxels = sum[1];
 	st.touched_octets = sum[2];
@@ -2412,6 +2414,16 @@ int ufo_b200_last_scan_stats(ufo_b200_map* m, ufo_b200_scan_stats* out)
 	return guarded(m, [&]() {
 		sync_map(m);
 		*out = m->stats;
+		return (int)UFO_B200_OK;
+	});
+}
+
+int ufo_b200_last_walk_stats(ufo_b200_map* m, ufo_b200_walk_stats* out)
+{
+	if (!m || !out) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() {
+		sync_map(m);
+		*out = m->walk_stats;
 		return (int)UFO_B200_OK;
 	});
 }

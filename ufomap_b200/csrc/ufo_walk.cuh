@@ -123,6 +123,13 @@ __global__ void __launch_bounds__(256) k_gather(DeviceMap M)
 	}
 }
 
+// component i (0, 1, 2) of (x, y, z)
+template <class T>
+__device__ __forceinline__ T pick3(T x, T y, T z, int i)
+{
+	return i == 0 ? x : (i == 1 ? y : z);
+}
+
 template <int DEPTH, bool COUNT>
 __global__ void __launch_bounds__(128) k_split(DeviceMap M, ScanArgs a)
 {
@@ -196,16 +203,14 @@ __global__ void __launch_bounds__(128) k_split(DeviceMap M, ScanArgs a)
 	Item* const out = a.items + i;
 	const size_t stride = a.item_stride;
 	// segment m = 0 is the outermost one (it starts at the ray's end point) and lies in shell J-1
-	Vec3 t0 = {w.tx, w.ty, w.tz};
-	const Vec3 dl = {w.dx, w.dy, w.dz};
-	const int sv[3] = {w.sx, w.sy, w.sz};
+	// per-axis values are picked with selects: an array indexed by A, B, C would live in local memory
 	const int B = (A == 0) ? 1 : 0, C = (A == 2) ? 1 : 2;  // the other two axes, B < C
-	const double dA = dl[A], dB = dl[B], dC = dl[C];
-	const int sA = sv[A], sB = sv[B], sC = sv[C];
-	double TA = t0[A], tB = t0[B], tC = t0[C];
+	const double dA = pick3(w.dx, w.dy, w.dz, A), dB = pick3(w.dx, w.dy, w.dz, B), dC = pick3(w.dx, w.dy, w.dz, C);
+	const int sA = pick3(w.sx, w.sy, w.sz, A), sB = pick3(w.sx, w.sy, w.sz, B), sC = pick3(w.sx, w.sy, w.sz, C);
+	double TA = pick3(w.tx, w.ty, w.tz, A), tB = pick3(w.tx, w.ty, w.tz, B), tC = pick3(w.tx, w.ty, w.tz, C);
 	uint32_t a_done = 0, cntB = 0, cntC = 0;
 	Key3 seg_cur = w.cur;
-	Vec3 seg_t = t0;
+	Vec3 seg_t = {w.tx, w.ty, w.tz};
 	uint32_t m = 0;
 	uint32_t a_k = nA - (J - 1) * S;  // dominant-axis steps before the first cut, in 1..S
 	for (; m + 1 < J; ++m, a_k += S) {
@@ -231,15 +236,12 @@ __global__ void __launch_bounds__(128) k_split(DeviceMap M, ScanArgs a)
 				tC = dop::add(tC, dC);
 				++cntC;
 			}
-		uint32_t kc[3] = {w.cur.x, w.cur.y, w.cur.z};
-		kc[A] += a_k * (uint32_t)sA;
-		kc[B] += cntB * (uint32_t)sB;
-		kc[C] += cntC * (uint32_t)sC;
-		const Key3 cut = {kc[0], kc[1], kc[2]};
-		Vec3 tcut;
-		tcut[A] = TA;
-		tcut[B] = tB;
-		tcut[C] = tC;
+		// axis i moved by a_k (A), cntB (B) or cntC (C) steps; {A, B, C} = {0, 1, 2}
+		const uint32_t mA = a_k * (uint32_t)sA, mB = cntB * (uint32_t)sB, mC = cntC * (uint32_t)sC;
+		const Key3 cut = {w.cur.x + (A == 0 ? mA : (B == 0 ? mB : mC)), w.cur.y + (A == 1 ? mA : (B == 1 ? mB : mC)),
+		                  w.cur.z + (A == 2 ? mA : (B == 2 ? mB : mC))};
+		const Vec3 tcut = {A == 0 ? TA : (B == 0 ? tB : tC), A == 1 ? TA : (B == 1 ? tB : tC),
+		                   A == 2 ? TA : (B == 2 ? tB : tC)};
 		// the next segment exists iff the walk gets here: loop condition of freeSpaceNormal
 		const bool exists = cut != w.end && (tcut.x <= dist || tcut.y <= dist || tcut.z <= dist);
 		if (!exists) break;
@@ -422,14 +424,26 @@ __device__ __forceinline__ bool walk_iteration_ring(double& tx, double& ty, doub
 	return any != 0;
 }
 
+// What the dense walk sent, per lane (profiling level 2 only; see Counters::walk_*).
+struct WalkCounts {
+	uint32_t records, mask_reds, words, dirty_reds;
+};
+
 // Drains up to 32 records of the warp's ring, starting at `head`: lane l takes record head + l.
-// One reduction per record into the scan volume; the brick's dirty bit is set by one lane per
-// distinct brick among the 32 records.
-__device__ __forceinline__ void drain_marks(const DeviceMap& M, const ulonglong2* ring, uint32_t head, uint32_t n,
-                                            uint32_t lane)
+// Records that mark the same word of the scan volume (rays of a batch crossing the same 4^3 block;
+// near the sensor, all of them) are merged first: the group's non-leaders OR their mask into the
+// leader's ring slot, and the leader issues the one global reduction.  OR is idempotent and
+// commutative, so no merge order can change a mask.  The brick's dirty bit is set by one lane per
+// distinct brick, and not at all when a lane of the group already set it earlier in this kernel
+// (`last_vb`: the brick of the lane's last drained record; the bitmap is only cleared by k_gather,
+// after the walk).
+template <bool COUNT>
+__device__ __forceinline__ void drain_marks(const DeviceMap& M, ulonglong2* ring, uint32_t head, uint32_t n,
+                                            uint32_t lane, uint32_t& last_vb, WalkCounts& wc)
 {
 	constexpr uint32_t FULL = 0xffffffffu;
-	uint32_t vb = kNone;
+	uint32_t vb = kNone, word = kNone;  // word = vb * 64 + block < 325^3 * 64 < 2^32 (volume_bricks)
+	unsigned long long mask = 0;
 	if (lane < n) {
 		const ulonglong2 e = ring[(head + lane) & (kRing - 1)];
 		uint32_t x, y, z;
@@ -441,11 +455,47 @@ __device__ __forceinline__ void drain_marks(const DeviceMap& M, const ulonglong2
 			atomicOr(&M.ctr->overflow, ((x | y | z) & ~M.g.key_mask) ? 32u : 64u);
 			vb = kNone;
 		} else {
-			atomicOr(&M.vol[(size_t)vb * 64 + morton2(x >> 2, y >> 2, z >> 2)], e.x);
+			word = vb * 64u + morton2(x >> 2, y >> 2, z >> 2);
+			mask = e.x;
+		}
+		if (COUNT) ++wc.records;
+	}
+	const uint32_t grp = __match_any_sync(FULL, word);
+	const uint32_t leader = __ffs(grp) - 1;
+	const bool alone = grp == (1u << lane);
+	if (word != kNone && lane != leader) {
+		// two 32-bit ORs: native shared-memory atomics (a 64-bit one is a compare-and-swap loop)
+		uint32_t* const lm = reinterpret_cast<uint32_t*>(&ring[(head + leader) & (kRing - 1)].x);
+		atomicOr(lm, (uint32_t)mask);
+		atomicOr(lm + 1, (uint32_t)(mask >> 32));
+	}
+	__syncwarp();
+	if (word != kNone && lane == leader) {
+		if (!alone) mask = ring[(head + lane) & (kRing - 1)].x;
+#ifdef UFO_WALK_NO_RED
+		// timing-only build: every address is computed but no reduction is issued (a pushed mask is
+		// never 0); the map comes out wrong
+		if (mask == 0ull)
+#endif
+		if (COUNT) {
+			wc.words += atomicOr(&M.vol[word], mask) == 0ull;
+			++wc.mask_reds;
+		} else {
+			atomicOr(&M.vol[word], mask);
 		}
 	}
-	const uint32_t grp = __match_any_sync(FULL, vb);
-	if (vb != kNone && lane == (uint32_t)(__ffs(grp) - 1)) vol_touch(M, vb);
+	const uint32_t bgrp = __match_any_sync(FULL, vb);
+	const bool seen = (__ballot_sync(FULL, last_vb == vb) & bgrp) != 0u;
+	if (vb != kNone) {
+		if (!seen && lane == (uint32_t)(__ffs(bgrp) - 1)) {
+#ifdef UFO_WALK_NO_RED
+			if (vb == 0xfffffffeu)
+#endif
+			vol_touch(M, vb);
+			if (COUNT) ++wc.dirty_reds;
+		}
+		last_vb = vb;
+	}
 }
 
 // brick slot of `bkey` for marking: one probe of the two-entry bucket (L1-cached: neighbouring
@@ -503,10 +553,12 @@ __global__ void __launch_bounds__(kWalkThreads, UFO_WALK_MINBLOCKS) k_walk_mark(
 	uint32_t cslot = kNone;
 #ifndef UFO_WALK_BRANCH
 	__shared__ ulonglong2 s_ring[DENSE ? kWalkThreads / 32 : 1][DENSE ? kRing : 1];
-	const ulonglong2* ring = s_ring[DENSE ? (threadIdx.x >> 5) : 0];
+	ulonglong2* ring = s_ring[DENSE ? (threadIdx.x >> 5) : 0];
 	const uint32_t ring_base = (uint32_t)__cvta_generic_to_shared(ring);
 	const uint32_t lt_mask = (1u << lane) - 1u;
 	uint32_t q_head = 0, q_tail = 0;  // warp-uniform running counters
+	uint32_t last_vb = kNone;         // drain_marks: brick whose dirty bit this lane's group last set
+	WalkCounts wc = {0, 0, 0, 0};
 #endif
 	while (true) {
 		uint32_t u0 = 0;
@@ -572,7 +624,7 @@ __global__ void __launch_bounds__(kWalkThreads, UFO_WALK_MINBLOCKS) k_walk_mark(
 					                          voxel_bits<DEPTH>(Key3{kx, ky, kz}), active, q_tail, ring_base, lt_mask);
 					if (q_tail - q_head >= 32u) {
 						__syncwarp();
-						drain_marks(M, ring, q_head, 32u, lane);
+						drain_marks<COUNT>(M, ring, q_head, 32u, lane, last_vb, wc);
 						__syncwarp();
 						q_head += 32u;
 					}
@@ -616,7 +668,13 @@ __global__ void __launch_bounds__(kWalkThreads, UFO_WALK_MINBLOCKS) k_walk_mark(
 #ifndef UFO_WALK_BRANCH
 	if (DENSE && q_tail != q_head) {
 		__syncwarp();
-		drain_marks(M, ring, q_head, q_tail - q_head, lane);
+		drain_marks<COUNT>(M, ring, q_head, q_tail - q_head, lane, last_vb, wc);
+	}
+	if (COUNT && DENSE) {
+		if (wc.records) atomicAdd(&M.ctr->walk_records, (unsigned long long)wc.records);
+		if (wc.mask_reds) atomicAdd(&M.ctr->walk_mask_reds, (unsigned long long)wc.mask_reds);
+		if (wc.words) atomicAdd(&M.ctr->walk_words, (unsigned long long)wc.words);
+		if (wc.dirty_reds) atomicAdd(&M.ctr->walk_dirty_reds, (unsigned long long)wc.dirty_reds);
 	}
 #endif
 	if (COUNT && visits) atomicAdd(&M.ctr->visits, (unsigned long long)visits);
