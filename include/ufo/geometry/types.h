@@ -1,0 +1,4 @@
+// Drop-in include path of the reference (ufo/geometry/types.h): forwards to the H100-native facade, so a
+// caller's #include <ufo/geometry/types.h> stays as it is when include/ of this repository is on the path.
+#pragma once
+#include <ufomap_b200/ufomap.hpp>

@@ -269,6 +269,76 @@ int ufo_b200_write_compressed(ufo_b200_map* m, const double* box6, uint32_t min_
 int ufo_b200_read_data(ufo_b200_map* m, const double* box6, const void* data, size_t size, int compressed,
                        size_t uncompressed_size);
 
+/* Bounding volumes (ufo::geometry::BoundingVolume, geometry/bounding_volume.h): a union of shapes,
+ * each one ufo_b200_volume.  type follows the order of ufo::geometry::BoundingVar
+ * (geometry/types.h); v holds the shape's members as the reference stores them:
+ *   0 AABB         centre xyz, half_size xyz
+ *   1 Frustum      six planes (top, bottom, left, right, near, far), each normal xyz, distance
+ *   2 LineSegment  start xyz, end xyz
+ *   3 OBB          centre xyz, half_size xyz, rotation w x y z
+ *   4 Plane        normal xyz, distance
+ *   5 Point        xyz
+ *   6 Ray          origin xyz, direction xyz (already normalised, as the Ray constructor leaves it)
+ *   7 Sphere       centre xyz, radius
+ * A node's cube passes a shape as intersects(AABB, shape) of collision_checks.cpp:53-356 decides,
+ * bit for bit; it passes the volume if it passes any of its shapes.  A node is inside the filter
+ * iff every cube on its path from the root down passes (the reference's recursions and iterator
+ * decide this way).  n_bv == 0: the whole map.  An unknown type: UFO_B200_E_INVALID.  reserved is
+ * ignored (set it to 0).
+ * Each *_bv entry point is its box6 twin with the volume in place of the AABB; the box6 forms are
+ * the *_bv forms with one AABB record. */
+#define UFO_B200_VOLUME_AABB 0
+#define UFO_B200_VOLUME_FRUSTUM 1
+#define UFO_B200_VOLUME_LINE_SEGMENT 2
+#define UFO_B200_VOLUME_OBB 3
+#define UFO_B200_VOLUME_PLANE 4
+#define UFO_B200_VOLUME_POINT 5
+#define UFO_B200_VOLUME_RAY 6
+#define UFO_B200_VOLUME_SPHERE 7
+typedef struct {
+	uint32_t type;
+	uint32_t reserved;
+	double v[24];
+} ufo_b200_volume;
+
+int ufo_b200_write_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, uint32_t min_depth, int expanded,
+                      void* buf, size_t cap, size_t* size);
+int ufo_b200_write_data_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, uint32_t min_depth, void* buf,
+                           size_t cap, size_t* size);
+int ufo_b200_write_compressed_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, uint32_t min_depth,
+                                 int data_only, int acceleration_level, int compression_level, void* buf, size_t cap,
+                                 size_t* size, size_t* uncompressed_size);
+int ufo_b200_read_data_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, const void* data, size_t size,
+                          int compressed, size_t uncompressed_size);
+/* Leaf iteration as ufo_b200_export_nodes, with the reference iterator's rule: a node is returned
+ * iff every cube on its path from the root passes the volume (ufo_b200_export_nodes tests the
+ * node's own cube only). */
+int ufo_b200_export_nodes_bv(ufo_b200_map* m, uint32_t depth, int occupied, int free_space, int unknown,
+                             const ufo_b200_volume* bv, size_t n_bv, uint64_t* codes, float* logodds, uint8_t* rgb,
+                             size_t cap, size_t* n);
+/* setValueVolume(BoundingVar, occupancy, min_depth) for one shape (the mapping server loops over the
+ * shapes of a volume, server.cpp:345-354).  The bricks whose path passes are found by a descent on
+ * the device, one level per kernel; more than 2^22 nodes at any level of it is UFO_B200_E_UNSUPPORTED
+ * before anything is written.  Otherwise as ufo_b200_set_value_volume. */
+int ufo_b200_set_value_volume_bv(ufo_b200_map* m, const ufo_b200_volume* bv, double occupancy, uint32_t min_depth);
+/* The node-vs-volume predicate on the host (the code the kernels run): out[i] = 1 iff the cube of
+ * centre centres[i] and half size half_sizes[i] (per axis; the node cubes of a map have three equal
+ * ones) passes the volume.  No map needed. */
+int ufo_b200_volume_intersects(const ufo_b200_volume* bv, size_t n_bv, const double* centres, const double* half_sizes,
+                               size_t n, uint8_t* out);
+
+/* Shape constructors whose arithmetic decides a shape's doubles, on the host in the library (no FMA
+ * contraction, whatever flags the caller compiles with), as the facade's geometry types use them:
+ *   ufo_b200_geometry_frustum: Frustum(pos, target, up, vertical_angle, horizontal_angle, near, far)
+ *     (geometry/frustum.h) -> planes[24] = 6 x (normal xyz, distance), top bottom left right near far
+ *   ufo_b200_geometry_plane:   Plane(v1, v2, v3) (geometry/plane.h) -> plane[4] = normal xyz, distance
+ *   ufo_b200_geometry_ray:     Ray(origin, direction) (geometry/ray.h) -> ray[6] = origin, direction
+ *     divided by its norm */
+int ufo_b200_geometry_frustum(const double pos[3], const double target[3], const double up[3], double vertical_angle,
+                              double horizontal_angle, double near_distance, double far_distance, double planes[24]);
+int ufo_b200_geometry_plane(const double v1[3], const double v2[3], const double v3[3], double plane[4]);
+int ufo_b200_geometry_ray(const double origin[3], const double direction[3], double ray[6]);
+
 /* Sensor model  occupancy_map_base.h:734-773.  out6/in: occupied_thres,
  * free_thres, prob_hit, prob_miss, clamping_thres_min, clamping_thres_max as
  * probabilities (setters) or as stored double log-odds (ufo_b200_sensor_model_logit). */

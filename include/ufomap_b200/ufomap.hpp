@@ -34,6 +34,7 @@
 #include <ostream>
 #include <string>
 #include <type_traits>
+#include <variant>
 #include <vector>
 
 #include "../ufomap_b200.h"
@@ -183,6 +184,172 @@ struct AABB {
 	Point getMin() const { return center - half_size; }
 	Point getMax() const { return center + half_size; }
 };
+
+// The other shapes of a bounding volume (geometry/*.h), with the reference's members and
+// constructors.  The constructors whose arithmetic decides the doubles run in the library
+// (ufo_b200_geometry_*, compiled without FMA contraction), so every caller gets the reference's
+// values whatever flags it is built with.
+struct Sphere {
+	Point center;
+	double radius;
+	Sphere() : center(0.0, 0.0, 0.0), radius(0.0) {}
+	Sphere(Point const& center, double radius) : center(center), radius(radius) {}
+};
+
+struct OBB {
+	Point center;
+	Point half_size;
+	math::Quaternion rotation;
+	OBB() {}
+	OBB(Point const& center, Point const& half_size) : center(center), half_size(half_size) {}
+	OBB(Point const& center, Point const& half_size, math::Quaternion const& rotation)
+	    : center(center), half_size(half_size), rotation(rotation)
+	{
+	}
+	// rotation = (roll, pitch, yaw)
+	OBB(Point const& center, Point const& half_size, Point const& rotation)
+	    : center(center), half_size(half_size), rotation(rotation[0], rotation[1], rotation[2])
+	{
+	}
+};
+
+struct Plane {
+	Point normal;
+	double distance;
+	Plane() : normal(1.0, 0.0, 0.0), distance(0.0) {}
+	Plane(Point const& normal, double distance) : normal(normal), distance(distance) {}
+	Plane(Point const& v_1, Point const& v_2, Point const& v_3)
+	{
+		double p[4];
+		ufo_b200_geometry_plane(v_1.data(), v_2.data(), v_3.data(), p);
+		normal = Point(p[0], p[1], p[2]);
+		distance = p[3];
+	}
+};
+
+struct Ray {
+	Point origin;
+	Point direction;
+	Ray() : direction(0.0, 0.0, 1.0) {}
+	// the direction is normalised
+	Ray(Point const& origin, Point const& direction)
+	{
+		double r[6];
+		ufo_b200_geometry_ray(origin.data(), direction.data(), r);
+		this->origin = Point(r[0], r[1], r[2]);
+		this->direction = Point(r[3], r[4], r[5]);
+	}
+};
+
+struct LineSegment {
+	Point start;
+	Point end;
+	LineSegment() {}
+	LineSegment(Point const& start, Point const& end) : start(start), end(end) {}
+};
+
+struct Frustum {
+	std::array<Plane, 6> planes;
+	Frustum() {}
+	Frustum(Point const& pos, Point const& target, Point const& up, double vertical_angle, double horizontal_angle,
+	        double near_distance, double far_distance)
+	{
+		double p[24];
+		ufo_b200_geometry_frustum(pos.data(), target.data(), up.data(), vertical_angle, horizontal_angle, near_distance,
+		                          far_distance, p);
+		for (int i = 0; i < 6; ++i) planes[i] = Plane(Point(p[4 * i], p[4 * i + 1], p[4 * i + 2]), p[4 * i + 3]);
+	}
+	Plane const& top() const { return planes[0]; }
+	Plane& top() { return planes[0]; }
+	Plane const& bottom() const { return planes[1]; }
+	Plane& bottom() { return planes[1]; }
+	Plane const& left() const { return planes[2]; }
+	Plane& left() { return planes[2]; }
+	Plane const& right() const { return planes[3]; }
+	Plane& right() { return planes[3]; }
+	Plane const& near() const { return planes[4]; }
+	Plane& near() { return planes[4]; }
+	Plane const& far() const { return planes[5]; }
+	Plane& far() { return planes[5]; }
+};
+
+// geometry/types.h: the shapes in this order (the C ABI's ufo_b200_volume type numbers)
+using BoundingVar = std::variant<AABB, Frustum, LineSegment, OBB, Plane, Point, Ray, Sphere>;
+
+// geometry/bounding_volume.h: a union of shapes; empty = the whole map
+class BoundingVolume
+{
+ public:
+	void add(BoundingVar const& bv) { bounding_volume_.push_back(bv); }
+	std::size_t size() const { return bounding_volume_.size(); }
+	bool empty() const { return bounding_volume_.empty(); }
+	std::vector<BoundingVar>::iterator begin() { return bounding_volume_.begin(); }
+	std::vector<BoundingVar>::const_iterator begin() const { return bounding_volume_.begin(); }
+	std::vector<BoundingVar>::const_iterator cbegin() const { return bounding_volume_.cbegin(); }
+	std::vector<BoundingVar>::iterator end() { return bounding_volume_.end(); }
+	std::vector<BoundingVar>::const_iterator end() const { return bounding_volume_.end(); }
+	std::vector<BoundingVar>::const_iterator cend() const { return bounding_volume_.cend(); }
+
+ private:
+	std::vector<BoundingVar> bounding_volume_;
+};
+
+// one shape as the C ABI's record
+inline ufo_b200_volume toRecord(BoundingVar const& bv)
+{
+	ufo_b200_volume r{};
+	r.type = (std::uint32_t)bv.index();
+	double* v = r.v;
+	auto put = [&v](Point const& p) {
+		*v++ = p[0];
+		*v++ = p[1];
+		*v++ = p[2];
+	};
+	std::visit(
+	    [&](auto const& s) {
+		    using T = std::decay_t<decltype(s)>;
+		    if constexpr (std::is_same_v<T, AABB>) {
+			    put(s.center);
+			    put(s.half_size);
+		    } else if constexpr (std::is_same_v<T, Frustum>) {
+			    for (Plane const& p : s.planes) {
+				    put(p.normal);
+				    *v++ = p.distance;
+			    }
+		    } else if constexpr (std::is_same_v<T, LineSegment>) {
+			    put(s.start);
+			    put(s.end);
+		    } else if constexpr (std::is_same_v<T, OBB>) {
+			    put(s.center);
+			    put(s.half_size);
+			    *v++ = s.rotation.w();
+			    *v++ = s.rotation.x();
+			    *v++ = s.rotation.y();
+			    *v++ = s.rotation.z();
+		    } else if constexpr (std::is_same_v<T, Plane>) {
+			    put(s.normal);
+			    *v++ = s.distance;
+		    } else if constexpr (std::is_same_v<T, Point>) {
+			    put(s);
+		    } else if constexpr (std::is_same_v<T, Ray>) {
+			    put(s.origin);
+			    put(s.direction);
+		    } else {
+			    put(s.center);
+			    *v++ = s.radius;
+		    }
+	    },
+	    bv);
+	return r;
+}
+
+inline std::vector<ufo_b200_volume> toRecords(BoundingVolume const& bv)
+{
+	std::vector<ufo_b200_volume> out;
+	out.reserve(bv.size());
+	for (BoundingVar const& b : bv) out.push_back(toRecord(b));
+	return out;
+}
 }  // namespace ufo::geometry
 
 namespace ufo::map
@@ -417,6 +584,39 @@ class MapFacade
 		return s.good();
 	}
 
+	// Octree::write with a BoundingVolume (octree.h:796-864): the save_map service (server.cpp:381-390)
+	bool write(std::string const& filename, ufo::geometry::BoundingVolume const& bounding_volume, bool compress = false,
+	           DepthType min_depth = 0, int compression_acceleration_level = 1, int compression_level = 0) const
+	{
+		std::ofstream f(filename.c_str(), std::ios_base::out | std::ios_base::binary);
+		return f.is_open() && write(f, bounding_volume, compress, min_depth, compression_acceleration_level, compression_level) &&
+		       (f.close(), !f.fail());
+	}
+	bool write(std::ostream& s, ufo::geometry::BoundingVolume const& bounding_volume, bool compress = false,
+	           DepthType min_depth = 0, int compression_acceleration_level = 1, int compression_level = 0) const
+	{
+		auto const bv = ufo::geometry::toRecords(bounding_volume);
+		if (compress)
+			return writeCompressedBv(s, bv, false, min_depth, compression_acceleration_level, compression_level) >= 0;
+		std::size_t n = 0;
+		if (UFO_B200_OK != ufo_b200_write_bv(map_, bv.data(), bv.size(), min_depth, 0, nullptr, 0, &n)) return false;
+		std::vector<char> image(n ? n : 1);
+		if (UFO_B200_OK != ufo_b200_write_bv(map_, bv.data(), bv.size(), min_depth, 0, image.data(), n, &n)) return false;
+		s.write(image.data(), (std::streamsize)n);
+		return s.good();
+	}
+
+	// setValueVolume (occupancy_map_base.h:492-518) for any one shape: the clear_volume service loops
+	// over the shapes of its BoundingVolume (server.cpp:345-354).  min_depth 0..4, colour maps at 0;
+	// other cases, and more than 2^22 nodes of one level inside the shape, set lastStatus() to
+	// UFO_B200_E_UNSUPPORTED.
+	void setValueVolume(ufo::geometry::BoundingVar const& bounding_volume, double occupancy_value,
+	                    DepthType min_depth = 0)
+	{
+		const ufo_b200_volume r = ufo::geometry::toRecord(bounding_volume);
+		last_status_ = ufo_b200_set_value_volume_bv(map_, &r, occupancy_value, min_depth);
+	}
+
 	// setValueVolume (occupancy_map_base.h:492-518) for the bounding volume the mapping server uses
 	// (robot clearing server.cpp:152-154, clear_volume service :354): AABB, min_depth 0..4; colour
 	// maps at min_depth 0.  Other cases set lastStatus() to UFO_B200_E_UNSUPPORTED.
@@ -486,6 +686,32 @@ class MapFacade
 		packBox(bounding_volume, box);
 		if (compress) return writeCompressed(s, box, true, min_depth, compression_acceleration_level, compression_level);
 		return writeDataImpl(s, box, compress, min_depth);
+	}
+
+	// Octree::writeData with a BoundingVolume (octree.h:885-917): what ufoToMsg publishes for the
+	// get_map service (server.cpp:327-336, ufomap_msgs/conversions.h:161-185)
+	int writeData(std::ostream& s, ufo::geometry::BoundingVolume const& bounding_volume, bool compress = false,
+	              DepthType min_depth = 0, int compression_acceleration_level = 1, int compression_level = 0) const
+	{
+		auto const bv = ufo::geometry::toRecords(bounding_volume);
+		if (compress) return writeCompressedBv(s, bv, true, min_depth, compression_acceleration_level, compression_level);
+		std::size_t n = 0;
+		if (UFO_B200_OK != ufo_b200_write_data_bv(map_, bv.data(), bv.size(), min_depth, nullptr, 0, &n)) return -1;
+		std::vector<char> data(n ? n : 1);
+		if (UFO_B200_OK != ufo_b200_write_data_bv(map_, bv.data(), bv.size(), min_depth, data.data(), n, &n)) return -1;
+		s.write(data.data(), (std::streamsize)n);
+		return s.good() ? (int)n : -1;
+	}
+
+	// Octree::readData with a BoundingVolume (octree.h:751-774; msgToUfo, conversions.h:122-134)
+	bool readData(std::istream& s, ufo::geometry::BoundingVolume const& bounding_volume, double resolution,
+	              DepthType depth_levels, int uncompressed_data_size = 1, bool compressed = false)
+	{
+		if (getResolution() != resolution || getTreeDepthLevels() != depth_levels) clear(resolution, depth_levels);
+		auto const bv = ufo::geometry::toRecords(bounding_volume);
+		std::vector<char> data((std::istreambuf_iterator<char>(s)), std::istreambuf_iterator<char>());
+		return UFO_B200_OK == ufo_b200_read_data_bv(map_, bv.data(), bv.size(), data.data(), data.size(), compressed,
+		                                            compressed ? (std::size_t)uncompressed_data_size : 0);
 	}
 
 	// Octree::readData (octree.h:733-770): merges a node stream (the data of a UFOMap message,
@@ -824,6 +1050,20 @@ class MapFacade
 		if (UFO_B200_OK != ufo_b200_write_compressed(map_, box, min_depth, data_only, accel, level, nullptr, 0, &n, &u)) return -1;
 		std::vector<char> data(n ? n : 1);
 		if (UFO_B200_OK != ufo_b200_write_compressed(map_, box, min_depth, data_only, accel, level, data.data(), n, &n, &u)) return -1;
+		s.write(data.data(), (std::streamsize)n);
+		return s.good() ? (int)u : -1;
+	}
+	int writeCompressedBv(std::ostream& s, std::vector<ufo_b200_volume> const& bv, bool data_only, DepthType min_depth,
+	                      int accel, int level) const
+	{
+		std::size_t n = 0, u = 0;
+		if (UFO_B200_OK != ufo_b200_write_compressed_bv(map_, bv.data(), bv.size(), min_depth, data_only, accel, level, nullptr,
+		                                                0, &n, &u))
+			return -1;
+		std::vector<char> data(n ? n : 1);
+		if (UFO_B200_OK != ufo_b200_write_compressed_bv(map_, bv.data(), bv.size(), min_depth, data_only, accel, level,
+		                                                data.data(), n, &n, &u))
+			return -1;
 		s.write(data.data(), (std::streamsize)n);
 		return s.good() ? (int)u : -1;
 	}

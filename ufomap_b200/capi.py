@@ -6,6 +6,7 @@ include/ufomap_b200/ufomap.hpp.  Loading fails loudly when the library has not
 been built -- there is no CPU fallback.
 """
 import ctypes as C
+import math
 import os
 
 import numpy as np
@@ -73,7 +74,109 @@ SYMBOLS = [
     "ufo_b200_update_nodes", "ufo_b200_insert_rays",
     "ufo_b200_route_inbox_bytes_color", "ufo_b200_route_mark_ex", "ufo_b200_route_sent",
     "ufo_b200_last_walk_stats",
+    "ufo_b200_write_bv", "ufo_b200_write_data_bv", "ufo_b200_write_compressed_bv", "ufo_b200_read_data_bv",
+    "ufo_b200_export_nodes_bv", "ufo_b200_set_value_volume_bv", "ufo_b200_volume_intersects",
+    "ufo_b200_geometry_frustum", "ufo_b200_geometry_plane", "ufo_b200_geometry_ray",
 ]
+
+# ufo_b200_volume: one shape of a bounding volume (type in BoundingVar order, members in v)
+VOLUME_DTYPE = np.dtype([("type", "<u4"), ("reserved", "<u4"), ("v", "<f8", (24,))])
+AABB, FRUSTUM, LINE_SEGMENT, OBB, PLANE, POINT, RAY, SPHERE = range(8)
+
+
+def volume_record(kind, values):
+    """One ufo_b200_volume: kind = AABB .. SPHERE, values = the shape's members in the reference's
+    order (see include/ufomap_b200.h)."""
+    r = np.zeros(1, VOLUME_DTYPE)
+    v = np.asarray(values, np.float64).reshape(-1)
+    r["type"] = kind
+    r["v"][0, :len(v)] = v
+    return r
+
+
+def aabb(mn, mx):
+    """AABB(min, max): half = (max - min) / 2, centre = min + half (geometry/aabb.h)."""
+    mn, mx = np.asarray(mn, np.float64), np.asarray(mx, np.float64)
+    half = (mx - mn) / 2.0
+    return volume_record(AABB, np.concatenate([mn + half, half]))
+
+
+def sphere(centre, radius):
+    return volume_record(SPHERE, np.concatenate([np.asarray(centre, np.float64), [radius]]))
+
+
+def obb(centre, half_size, quaternion_wxyz):
+    return volume_record(OBB, np.concatenate([np.asarray(centre, np.float64), np.asarray(half_size, np.float64),
+                                              np.asarray(quaternion_wxyz, np.float64)]))
+
+
+def plane(normal, distance):
+    return volume_record(PLANE, np.concatenate([np.asarray(normal, np.float64), [distance]]))
+
+
+def point(xyz):
+    return volume_record(POINT, np.asarray(xyz, np.float64))
+
+
+def line_segment(start, end):
+    return volume_record(LINE_SEGMENT, np.concatenate([np.asarray(start, np.float64), np.asarray(end, np.float64)]))
+
+
+def ray(origin, direction):
+    """Ray(origin, direction): the direction is normalised like the Ray constructor does (each
+    component divided by sqrt((x*x + y*y) + z*z))."""
+    d = [float(x) for x in direction]
+    n = math.sqrt((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2])
+    return volume_record(RAY, list(origin) + [d[0] / n, d[1] / n, d[2] / n])
+
+
+def frustum(planes):
+    """Frustum from its six planes (top, bottom, left, right, near, far), each (normal xyz, distance)."""
+    return volume_record(FRUSTUM, np.asarray(planes, np.float64).reshape(24))
+
+
+def frustum7(pos, target, up, vertical_angle, horizontal_angle, near_distance, far_distance):
+    """Frustum(pos, target, up, vertical_angle, horizontal_angle, near, far), computed by the library."""
+    out = np.empty(24)
+    args = [np.ascontiguousarray(v, np.float64) for v in (pos, target, up)]
+    load().ufo_b200_geometry_frustum(*(a.ctypes.data for a in args), float(vertical_angle), float(horizontal_angle),
+                                     float(near_distance), float(far_distance), out.ctypes.data)
+    return volume_record(FRUSTUM, out)
+
+
+def plane3(v1, v2, v3):
+    """Plane(v1, v2, v3), computed by the library."""
+    out = np.empty(4)
+    args = [np.ascontiguousarray(v, np.float64) for v in (v1, v2, v3)]
+    load().ufo_b200_geometry_plane(*(a.ctypes.data for a in args), out.ctypes.data)
+    return volume_record(PLANE, out)
+
+
+def as_volume(volume):
+    """A bounding volume as a contiguous array of ufo_b200_volume records: None / [] (the whole
+    map), one record, or a sequence of records (their union)."""
+    if volume is None:
+        return np.zeros(0, VOLUME_DTYPE)
+    if isinstance(volume, np.ndarray) and volume.dtype == VOLUME_DTYPE:
+        return np.ascontiguousarray(volume.reshape(-1))
+    parts = [as_volume(v) for v in volume]
+    return np.ascontiguousarray(np.concatenate(parts)) if parts else np.zeros(0, VOLUME_DTYPE)
+
+
+def volume_intersects(volume, centres, half_sizes):
+    """The device's node-vs-volume predicate, run on the host: bool per cube (centres [n, 3],
+    half_sizes [n, 3] or [n] for cubes)."""
+    lib = load()
+    bv = as_volume(volume)
+    c = np.ascontiguousarray(centres, np.float64).reshape(-1, 3)
+    h = np.asarray(half_sizes, np.float64)
+    h = np.ascontiguousarray(np.broadcast_to(h.reshape(-1, 1) if h.ndim <= 1 else h, c.shape))
+    out = np.zeros(len(c), np.uint8)
+    rc = lib.ufo_b200_volume_intersects(bv.ctypes.data if len(bv) else None, len(bv), c.ctypes.data, h.ctypes.data,
+                                        len(c), out.ctypes.data)
+    if rc != OK:
+        raise UfoError(rc, "invalid bounding volume")
+    return out.astype(bool)
 
 class Cloud2(C.Structure):
     """ufo_b200_cloud2: a sensor_msgs/PointCloud2 data buffer + field offsets."""
@@ -158,6 +261,16 @@ def load():
     lib.ufo_b200_ipc_export.argtypes = [vp, vp]
     lib.ufo_b200_ipc_open.argtypes = [vp, C.POINTER(vp)]
     lib.ufo_b200_ipc_close.argtypes = [vp]
+    lib.ufo_b200_write_bv.argtypes = [vp, vp, sz, u32, i32, vp, sz, C.POINTER(sz)]
+    lib.ufo_b200_write_data_bv.argtypes = [vp, vp, sz, u32, vp, sz, C.POINTER(sz)]
+    lib.ufo_b200_write_compressed_bv.argtypes = [vp, vp, sz, u32, i32, i32, i32, vp, sz, C.POINTER(sz), C.POINTER(sz)]
+    lib.ufo_b200_read_data_bv.argtypes = [vp, vp, sz, vp, sz, i32, sz]
+    lib.ufo_b200_export_nodes_bv.argtypes = [vp, u32, i32, i32, i32, vp, sz, vp, vp, vp, sz, C.POINTER(sz)]
+    lib.ufo_b200_set_value_volume_bv.argtypes = [vp, vp, dbl, u32]
+    lib.ufo_b200_volume_intersects.argtypes = [vp, sz, vp, vp, sz, vp]
+    lib.ufo_b200_geometry_frustum.argtypes = [vp, vp, vp, dbl, dbl, dbl, dbl, vp]
+    lib.ufo_b200_geometry_plane.argtypes = [vp, vp, vp, vp]
+    lib.ufo_b200_geometry_ray.argtypes = [vp, vp, vp]
     lib.ufo_b200_clear.argtypes = [vp]
     lib.ufo_b200_set_shard.argtypes = [vp, u32, u32]
     lib.ufo_b200_version.restype = C.c_char_p
@@ -454,6 +567,73 @@ class Map:
         self._check(self.lib.ufo_b200_write_data(self.h, bp, int(min_depth), buf.ctypes.data, n.value,
                                                  C.byref(n)))
         return buf[:n.value].tobytes()
+
+    # -- bounding volumes (volume: see as_volume) -----------------------------
+    @staticmethod
+    def _bv(volume):
+        bv = as_volume(volume)
+        return bv, (bv.ctypes.data if len(bv) else None), len(bv)
+
+    def write_bv(self, volume=None, min_depth=0, expanded=False):
+        """Octree::write(stream, BoundingVolume, compress=False, min_depth): file image (bytes)."""
+        bv, bp, nb = self._bv(volume)
+        n = C.c_size_t()
+        self._check(self.lib.ufo_b200_write_bv(self.h, bp, nb, int(min_depth), int(expanded), None, 0, C.byref(n)))
+        buf = np.empty(max(n.value, 1), np.uint8)
+        self._check(self.lib.ufo_b200_write_bv(self.h, bp, nb, int(min_depth), int(expanded), buf.ctypes.data, n.value,
+                                               C.byref(n)))
+        return buf[:n.value].tobytes()
+
+    def write_data_bv(self, volume=None, min_depth=0):
+        """Octree::writeData(stream, BoundingVolume, compress=False, min_depth): node stream (bytes)."""
+        bv, bp, nb = self._bv(volume)
+        n = C.c_size_t()
+        self._check(self.lib.ufo_b200_write_data_bv(self.h, bp, nb, int(min_depth), None, 0, C.byref(n)))
+        buf = np.empty(max(n.value, 1), np.uint8)
+        self._check(self.lib.ufo_b200_write_data_bv(self.h, bp, nb, int(min_depth), buf.ctypes.data, n.value, C.byref(n)))
+        return buf[:n.value].tobytes()
+
+    def write_compressed_bv(self, volume=None, min_depth=0, data_only=False, acceleration=1, level=0):
+        """Octree::write / writeData with a BoundingVolume and compress=True: (bytes, uncompressed size)."""
+        bv, bp, nb = self._bv(volume)
+        n, u = C.c_size_t(), C.c_size_t()
+        args = (int(min_depth), int(data_only), int(acceleration), int(level))
+        self._check(self.lib.ufo_b200_write_compressed_bv(self.h, bp, nb, *args, None, 0, C.byref(n), C.byref(u)))
+        buf = np.empty(max(n.value, 1), np.uint8)
+        self._check(self.lib.ufo_b200_write_compressed_bv(self.h, bp, nb, *args, buf.ctypes.data, n.value, C.byref(n),
+                                                          C.byref(u)))
+        return buf[:n.value].tobytes(), int(u.value)
+
+    def read_data_bv(self, data, volume=None, compressed=False, uncompressed_size=0):
+        """Octree::readData(stream, BoundingVolume, ...): merge a node stream into the map."""
+        bv, bp, nb = self._bv(volume)
+        buf = np.frombuffer(data, np.uint8)
+        self._check(self.lib.ufo_b200_read_data_bv(self.h, bp, nb, buf.ctypes.data if len(buf) else None, len(buf),
+                                                   int(compressed), int(uncompressed_size)))
+
+    def export_nodes_bv(self, volume=None, depth=0, occupied=True, free=True, unknown=False):
+        """beginLeaves(BoundingVolume, occupied, free, unknown, false, depth) as a batch: (codes sorted,
+        occ, rgb) of the depth-`depth` nodes whose whole path from the root passes the volume."""
+        bv, bp, nb = self._bv(volume)
+        flt = (int(depth), int(occupied), int(free), int(unknown))
+        n = C.c_size_t()
+        self._check(self.lib.ufo_b200_export_nodes_bv(self.h, *flt, bp, nb, None, None, None, 0, C.byref(n)))
+        cnt = n.value
+        codes = np.empty(cnt, np.uint64)
+        occ = np.empty(cnt, np.float32)
+        rgb = np.zeros((cnt, 3), np.uint8)
+        if cnt:
+            self._check(self.lib.ufo_b200_export_nodes_bv(self.h, *flt, bp, nb, codes.ctypes.data, occ.ctypes.data,
+                                                          rgb.ctypes.data if self.color else None, cnt, C.byref(n)))
+        order = np.argsort(codes, kind="stable")
+        return codes[order], occ[order], rgb[order]
+
+    def set_value_volume_bv(self, shape, occupancy, min_depth=0):
+        """setValueVolume(BoundingVar, occupancy probability, min_depth) for one shape record."""
+        bv = as_volume(shape)
+        if len(bv) != 1:
+            raise ValueError("set_value_volume_bv takes exactly one shape")
+        self._check(self.lib.ufo_b200_set_value_volume_bv(self.h, bv.ctypes.data, float(occupancy), int(min_depth)))
 
     # -- state ----------------------------------------------------------------
     def value_field(self, sort=True):

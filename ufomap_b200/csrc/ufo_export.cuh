@@ -23,6 +23,7 @@
 #pragma once
 
 #include "ufo_device.cuh"
+#include "ufo_volume.cuh"
 
 namespace ufo_b200
 {
@@ -30,26 +31,9 @@ constexpr int kBrickStreamMax = 1 + 8 * (1 + 8 * (1 + 64 * 7));  // colour paylo
 
 // Partial / truncated export (Octree::writeData(stream, bounding_volume, false, min_depth),
 // octree.h:885-917): children at min_depth are written as leaves carrying their aggregate
-// payload; a child whose cube misses the box is skipped.  lo/hi are getMin()/getMax() of the
-// reference's AABB(min, max) (geometry/aabb.h:62-69); the test is intersects(AABB, AABB) of
-// collision_checks.cpp:256-264; node centres are accumulated top-down like getChildCenter
+// payload; a child whose cube misses the volume is skipped.  The cube test is vol_hits
+// (ufo_volume.cuh); node centres are accumulated top-down like getChildCenter
 // (octree.h:625-633) so that the comparisons see the same doubles.
-struct ExportBox {
-	int on;
-	double lo[3], hi[3];
-};
-
-UFO_HD bool box_hits(const ExportBox& bx, const double c[3], double hs)
-{
-	if (!bx.on) return true;
-	for (int k = 0; k < 3; ++k) {
-		const double mn = dop::sub(c[k], hs), mx = dop::add(c[k], hs);
-		if (!(mn <= bx.hi[k])) return false;
-		if (!(bx.lo[k] <= mx)) return false;
-	}
-	return true;
-}
-
 UFO_HD void child_center(const double c[3], double hs, uint32_t i, double out[3])
 {
 	out[0] = dop::add(c[0], (i & 1u) ? hs : -hs);
@@ -81,19 +65,19 @@ __device__ __forceinline__ void put_payload(uint8_t* p, float occ, uint32_t rgb)
 }
 
 // One octet of block b: returns its bytes in the stream and writes them when dst != nullptr.
-template <bool COLOR>
+template <bool COLOR, bool G>
 __device__ __forceinline__ uint32_t octet_record(const DeviceMap& M, size_t b, uint32_t o, bool has,
                                                  float leaf_occ, uint32_t leaf_rgb, uint32_t min_depth,
-                                                 const ExportBox& bx, const double oc[3], uint8_t* dst)
+                                                 const Volume& bx, const double oc[3], uint8_t* dst)
 {
 	constexpr uint32_t P = COLOR ? 7u : 4u;
-	if (!box_hits(bx, oc, M.g.half_size[1])) return 0;
+	if (!vol_hits_t<G>(bx, oc, M.g.half_size[1])) return 0;
 	if (has && min_depth == 0) {
 		uint32_t n = 0;
 		for (uint32_t j = 0; j < 8; ++j) {
 			double vc[3];
 			child_center(oc, M.g.half_size[0], j, vc);
-			if (!box_hits(bx, vc, M.g.half_size[0])) continue;
+			if (!vol_hits_t<G>(bx, vc, M.g.half_size[0])) continue;
 			if (dst) put_payload<COLOR>(dst + n, M.leaf[b * 64 + 8 * o + j], COLOR ? M.leaf_rgb[b * 64 + 8 * o + j] : 0u);
 			n += P;
 		}
@@ -108,9 +92,9 @@ __device__ __forceinline__ uint32_t octet_record(const DeviceMap& M, size_t b, u
 
 // offsets == nullptr: size pass (fills info); otherwise the record of every brick whose info has
 // bit 2 set is written to out + offsets[brick].
-template <bool COLOR>
+template <bool COLOR, bool G>
 __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bricks, int pruned, uint32_t min_depth,
-                                                     ExportBox bx, BrickInfo* info,
+                                                     Volume bx, BrickInfo* info,
                                                      const unsigned long long* offsets, uint8_t* out)
 {
 	extern __shared__ uint8_t s_buf[];
@@ -152,9 +136,9 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 	bc[2] = s_center[2];
 	child_center(bc, M.g.half_size[3], j3, d3c);
 	child_center(d3c, M.g.half_size[2], k3, blkc);
-	const bool brick_hit = box_hits(bx, bc, M.g.half_size[4]);
-	const bool d3_hit = box_hits(bx, d3c, M.g.half_size[3]);
-	const bool blk_hit = box_hits(bx, blkc, M.g.half_size[2]);
+	const bool brick_hit = vol_hits_t<G>(bx, bc, M.g.half_size[4]);
+	const bool d3_hit = vol_hits_t<G>(bx, d3c, M.g.half_size[3]);
+	const bool blk_hit = vol_hits_t<G>(bx, blkc, M.g.half_size[2]);
 
 	const size_t b = (size_t)brick * 64 + t;
 	const uint32_t init8 = (M.meta[b] >> 16) & 0xffu;
@@ -198,7 +182,7 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 			for (uint32_t o = 0; o < 8; ++o) {
 				double oc[3];
 				child_center(blkc, M.g.half_size[1], o, oc);
-				blk_size += octet_record<COLOR>(M, b, o, (oct_has >> o) & 1u, oocc[o], orgb[o], min_depth, bx, oc, nullptr);
+				blk_size += octet_record<COLOR, G>(M, b, o, (oct_has >> o) & 1u, oocc[o], orgb[o], min_depth, bx, oc, nullptr);
 			}
 		} else {
 			blk_size = P;
@@ -213,7 +197,7 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 	if (t < 8) {
 		double c3[3];
 		child_center(bc, M.g.half_size[3], t, c3);
-		const bool hit = brick_hit && box_hits(bx, c3, M.g.half_size[3]);
+		const bool hit = brick_hit && vol_hits_t<G>(bx, c3, M.g.half_size[3]);
 		bool has = false;
 		uint32_t size = 1, mask = 0;
 		for (int k = 0; k < 8; ++k) {
@@ -277,7 +261,7 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 					for (uint32_t o = 0; o < 8; ++o) {
 						double oc[3];
 						child_center(blkc, M.g.half_size[1], o, oc);
-						at += octet_record<COLOR>(M, b, o, (oct_has >> o) & 1u, oocc[o], orgb[o], min_depth, bx, oc, s_buf + at);
+						at += octet_record<COLOR, G>(M, b, o, (oct_has >> o) & 1u, oocc[o], orgb[o], min_depth, bx, oc, s_buf + at);
 					}
 				} else {
 					put_payload<COLOR>(s_buf + at, s_blk_occ[t], s_blk_rgb[t]);
@@ -299,13 +283,21 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 // field: every node of depth `depth` inside the known space (existing bricks / upper nodes) whose
 // own state -- occupied: value > occupied threshold, free: value < free threshold, unknown: in
 // between, the value of an inner node being the maximum of its subtree -- passes the filter and
-// whose cube intersects the box.  The reference returns a collapsed leaf above `depth` as one
-// node; here it appears as its depth-`depth` cells (same space, same state).
+// whose cube passes the volume filter.  The reference returns a collapsed leaf above `depth` as
+// one node; here it appears as its depth-`depth` cells (same space, same state).
+// Volume filter (CHAIN, a template parameter of the kernels): chain == 0 tests the node's own cube
+// (centre from toCoord) -- ufo_b200_export_nodes;
+// chain != 0 tests every cube on the node's path from the root down, centres accumulated like
+// getChildCenter, as the reference's iterator does (validNode, iterator/octree.h:213-245) --
+// ufo_b200_export_nodes_bv.  The chain above depth 4 comes from k_brick_chain (brick_ok, brick_c).
 // One thread per (brick, block) for depth 0..4; k_export_upper for depth >= 5.
 struct NodeFilter {
 	uint32_t depth;
 	int occupied, free_, unknown;
-	ExportBox box;
+	Volume vol;
+	int chain;
+	const uint8_t* brick_ok;
+	const double* brick_c;
 };
 
 __device__ __forceinline__ bool node_passes(const DeviceMap& M, const NodeFilter& f, float v)
@@ -314,18 +306,20 @@ __device__ __forceinline__ bool node_passes(const DeviceMap& M, const NodeFilter
 	return (f.occupied && occ) || (f.free_ && fre) || (f.unknown && !occ && !fre);
 }
 
+// inside: the chain test of the caller (chain mode)
+template <bool CHAIN>
 __device__ __forceinline__ void node_emit(const DeviceMap& M, const NodeFilter& f, uint32_t x, uint32_t y, uint32_t z,
                                           float v, uint32_t rgb, unsigned long long* codes, float* occ, uint32_t* rgbs,
-                                          unsigned long long cap, unsigned long long* count)
+                                          unsigned long long cap, unsigned long long* count, bool inside = true)
 {
-	if (!node_passes(M, f, v)) return;
+	if (!inside || !node_passes(M, f, v)) return;
 	const uint32_t d = f.depth;
 	const uint32_t centre = d ? (1u << (d - 1)) : 0u, snap = ~((1u << d) - 1u);
 	const Key3 k = {(x & snap) | centre, (y & snap) | centre, (z & snap) | centre};
-	if (f.box.on) {
+	if (!CHAIN && f.vol.n) {
 		const Vec3 c = key_to_coord(M.g, k, d);
 		const double cc[3] = {c.x, c.y, c.z};
-		if (!box_hits(f.box, cc, M.g.half_size[d])) return;
+		if (!vol_hits_t<false>(f.vol, cc, M.g.half_size[d])) return;
 	}
 	const unsigned long long at = atomicAdd(count, 1ull);
 	if (codes && at < cap) {
@@ -335,6 +329,33 @@ __device__ __forceinline__ void node_emit(const DeviceMap& M, const NodeFilter& 
 	}
 }
 
+// Per brick: the centre of its cube accumulated from the root, and whether every cube from the
+// root's children down to the brick itself passes the volume (the root is tested on the host).
+__global__ void __launch_bounds__(256) k_brick_chain(DeviceMap M, uint32_t n_bricks, Volume vol, uint8_t* ok_out, double* c_out)
+{
+	const uint32_t brick = blockIdx.x * blockDim.x + threadIdx.x;
+	if (brick >= n_bricks) return;
+	uint32_t kx, ky, kz;
+	unpack_key(M.brick_key[brick], kx, ky, kz);
+	double c[3] = {0.0, 0.0, 0.0};
+	bool ok = !((kx | ky | kz) & ~(M.g.key_mask >> 4));  // alias collector bricks own no voxels
+	for (uint32_t d = M.g.depth_levels; d > 4 && ok; --d) {
+		const uint32_t bit = d - 5;
+		const uint32_t i = ((kx >> bit) & 1u) | (((ky >> bit) & 1u) << 1) | (((kz >> bit) & 1u) << 2);
+		double n[3];
+		child_center(c, M.g.half_size[d - 1], i, n);
+		c[0] = n[0];
+		c[1] = n[1];
+		c[2] = n[2];
+		ok = vol_hits(vol, c, M.g.half_size[d - 1]);
+	}
+	ok_out[brick] = ok ? 1 : 0;
+	c_out[3 * (size_t)brick] = c[0];
+	c_out[3 * (size_t)brick + 1] = c[1];
+	c_out[3 * (size_t)brick + 2] = c[2];
+}
+
+template <bool CHAIN>
 __global__ void __launch_bounds__(256) k_export_nodes(DeviceMap M, uint32_t n_bricks, NodeFilter f, unsigned long long* codes,
                                                       float* occ, uint32_t* rgbs, unsigned long long cap,
                                                       unsigned long long* count)
@@ -349,14 +370,31 @@ __global__ void __launch_bounds__(256) k_export_nodes(DeviceMap M, uint32_t n_br
 	               cz = ((ch >> 2) & 1u) | ((ch >> 4) & 2u);
 	const uint32_t x0 = (bx << 4) | (cx << 2), y0 = (by << 4) | (cy << 2), z0 = (bz << 4) | (cz << 2);
 	const uint32_t d = f.depth;
+	// chain mode: the cubes of the brick's depth-3 node and of this block, below the brick's chain
+	double blkc[3] = {0.0, 0.0, 0.0};
+	bool in3 = true, in2 = true;
+	if (CHAIN) {
+		if (!f.brick_ok[brick]) return;
+		if (d <= 3) {
+			const double bc[3] = {f.brick_c[3 * (size_t)brick], f.brick_c[3 * (size_t)brick + 1], f.brick_c[3 * (size_t)brick + 2]};
+			double d3c[3];
+			child_center(bc, M.g.half_size[3], ch >> 3, d3c);
+			in3 = vol_hits_t<true>(f.vol, d3c, M.g.half_size[3]);
+			if (d <= 2 && in3) {
+				child_center(d3c, M.g.half_size[2], ch & 7u, blkc);
+				in2 = vol_hits_t<true>(f.vol, blkc, M.g.half_size[2]);
+			}
+			if (!in3 || !in2) return;
+		}
+	}
 	if (d == 4) {
-		if (ch == 0) node_emit(M, f, x0, y0, z0, M.brick_sum4[brick].occ, M.color ? M.brick_rgb4[brick] : 0u, codes, occ, rgbs, cap, count);
+		if (ch == 0) node_emit<CHAIN>(M, f, x0, y0, z0, M.brick_sum4[brick].occ, M.color ? M.brick_rgb4[brick] : 0u, codes, occ, rgbs, cap, count);
 		return;
 	}
 	if (d == 3) {
 		if ((ch & 7u) == 0) {
 			const uint32_t j = ch >> 3;
-			node_emit(M, f, x0, y0, z0, M.brick_sum3[(size_t)brick * 8 + j].occ, M.color ? M.brick_rgb3[(size_t)brick * 8 + j] : 0u, codes,
+			node_emit<CHAIN>(M, f, x0, y0, z0, M.brick_sum3[(size_t)brick * 8 + j].occ, M.color ? M.brick_rgb3[(size_t)brick * 8 + j] : 0u, codes,
 			          occ, rgbs, cap, count);
 		}
 		return;
@@ -364,25 +402,37 @@ __global__ void __launch_bounds__(256) k_export_nodes(DeviceMap M, uint32_t n_br
 	const uint32_t meta = M.meta[blk];
 	const bool init = (meta >> 16) != 0;
 	if (d == 2) {
-		node_emit(M, f, x0, y0, z0, init ? M.agg2[blk].occ : 0.0f, (init && M.color) ? M.rgb2[blk] : 0u, codes, occ, rgbs, cap, count);
+		node_emit<CHAIN>(M, f, x0, y0, z0, init ? M.agg2[blk].occ : 0.0f, (init && M.color) ? M.rgb2[blk] : 0u, codes, occ, rgbs, cap, count);
 		return;
 	}
 	for (uint32_t o = 0; o < 8; ++o) {
 		const bool oi = init && ((meta >> (16 + o)) & 1u);
 		const uint32_t ox = x0 | ((o & 1u) << 1), oy = y0 | (o & 2u), oz = z0 | ((o & 4u) >> 1);
+		double oc[3] = {0.0, 0.0, 0.0};
+		if (CHAIN) {
+			child_center(blkc, M.g.half_size[1], o, oc);
+			if (!vol_hits_t<true>(f.vol, oc, M.g.half_size[1])) continue;
+		}
 		if (d == 1) {
-			node_emit(M, f, ox, oy, oz, oi ? M.sum1[blk * 8 + o] : 0.0f, (oi && M.color) ? M.sum1_rgb[blk * 8 + o] : 0u, codes, occ, rgbs,
+			node_emit<CHAIN>(M, f, ox, oy, oz, oi ? M.sum1[blk * 8 + o] : 0.0f, (oi && M.color) ? M.sum1_rgb[blk * 8 + o] : 0u, codes, occ, rgbs,
 			          cap, count);
 			continue;
 		}
 		for (uint32_t j = 0; j < 8; ++j) {
 			const float v = oi ? M.leaf[blk * 64 + 8 * o + j] : 0.0f;
 			const uint32_t c = (oi && M.color) ? M.leaf_rgb[blk * 64 + 8 * o + j] : 0u;
-			node_emit(M, f, ox | (j & 1u), oy | ((j >> 1) & 1u), oz | (j >> 2), v, c, codes, occ, rgbs, cap, count);
+			bool in0 = true;
+			if (CHAIN) {
+				double vc[3];
+				child_center(oc, M.g.half_size[0], j, vc);
+				in0 = vol_hits_t<true>(f.vol, vc, M.g.half_size[0]);
+			}
+			node_emit<CHAIN>(M, f, ox | (j & 1u), oy | ((j >> 1) & 1u), oz | (j >> 2), v, c, codes, occ, rgbs, cap, count, in0);
 		}
 	}
 }
 
+template <bool CHAIN>
 __global__ void __launch_bounds__(256) k_export_upper(DeviceMap M, uint32_t n_upper, NodeFilter f, unsigned long long* codes,
                                                       float* occ, uint32_t* rgbs, unsigned long long cap,
                                                       unsigned long long* count)
@@ -395,7 +445,23 @@ __global__ void __launch_bounds__(256) k_export_upper(DeviceMap M, uint32_t n_up
 	const uint32_t d = x >> 16;  // depth tag (upper_key)
 	if (d != f.depth) return;
 	x &= 0xffffu;
-	node_emit(M, f, x << d, y << d, z << d, M.up_agg[i].occ, M.color ? M.up_rgb[i] : 0u, codes, occ, rgbs, cap, count);
+	const uint32_t X = x << d, Y = y << d, Z = z << d;
+	bool inside = true;
+	if (CHAIN) {
+		// every cube from the root's children down to the node (the root is tested on the host)
+		double c[3] = {0.0, 0.0, 0.0};
+		for (uint32_t D = M.g.depth_levels; D > d && inside; --D) {
+			const uint32_t bit = D - 1;
+			const uint32_t ci = ((X >> bit) & 1u) | (((Y >> bit) & 1u) << 1) | (((Z >> bit) & 1u) << 2);
+			double n[3];
+			child_center(c, M.g.half_size[D - 1], ci, n);
+			c[0] = n[0];
+			c[1] = n[1];
+			c[2] = n[2];
+			inside = vol_hits_t<true>(f.vol, c, M.g.half_size[D - 1]);
+		}
+	}
+	node_emit<CHAIN>(M, f, X, Y, Z, M.up_agg[i].occ, M.color ? M.up_rgb[i] : 0u, codes, occ, rgbs, cap, count, inside);
 }
 
 // ---------------------------------------------------------------------------
@@ -409,19 +475,28 @@ __global__ void __launch_bounds__(256) k_export_upper(DeviceMap M, uint32_t n_up
 // thread, and leaves the result as a bit mask in the block's miss mask; the set itself is the K3
 // update kernel in SET mode, followed by the usual aggregate passes.
 struct VolumeArgs {
-	ExportBox box;
+	Volume vol;
 	uint32_t min_depth;       // 0..4
 	uint32_t bx0, by0, bz0;   // first candidate brick (brick coordinates)
 	uint32_t nx, ny, nz;      // candidate bricks per axis
+	const unsigned long long* cand;  // != nullptr: the candidates are these packed brick keys (nx of them)
+	int general;                     // the volume holds a shape other than an AABB (k_volume_mark<true>)
 };
 
+template <bool G>
 __global__ void __launch_bounds__(64) k_volume_mark(DeviceMap M, VolumeArgs v)
 {
 	__shared__ double s_center[3];
 	__shared__ uint32_t s_slot;
 	const uint32_t t = threadIdx.x;
-	const uint32_t ix = blockIdx.x % v.nx, iy = (blockIdx.x / v.nx) % v.ny, iz = blockIdx.x / (v.nx * v.ny);
-	const uint32_t kx = v.bx0 + ix, ky = v.by0 + iy, kz = v.bz0 + iz;
+	uint32_t kx, ky, kz;
+	if (v.cand) {
+		unpack_key(v.cand[blockIdx.x], kx, ky, kz);
+	} else {
+		kx = v.bx0 + blockIdx.x % v.nx;
+		ky = v.by0 + (blockIdx.x / v.nx) % v.ny;
+		kz = v.bz0 + blockIdx.x / (v.nx * v.ny);
+	}
 	if (t == 0) {
 		double c[3] = {0.0, 0.0, 0.0};
 		bool ok = true;
@@ -433,7 +508,7 @@ __global__ void __launch_bounds__(64) k_volume_mark(DeviceMap M, VolumeArgs v)
 			c[0] = n[0];
 			c[1] = n[1];
 			c[2] = n[2];
-			ok = ok && box_hits(v.box, c, M.g.half_size[d - 1]);  // cube of the depth d-1 ancestor
+			ok = ok && vol_hits_t<G>(v.vol, c, M.g.half_size[d - 1]);  // cube of the depth d-1 ancestor
 		}
 		uint32_t slot = kNone;
 		if (ok) {
@@ -455,17 +530,17 @@ __global__ void __launch_bounds__(64) k_volume_mark(DeviceMap M, VolumeArgs v)
 		double bc[3] = {s_center[0], s_center[1], s_center[2]}, d3c[3], blkc[3];
 		child_center(bc, M.g.half_size[3], t >> 3, d3c);
 		child_center(d3c, M.g.half_size[2], t & 7u, blkc);
-		if (box_hits(v.box, d3c, M.g.half_size[3])) {
+		if (vol_hits_t<G>(v.vol, d3c, M.g.half_size[3])) {
 			if (v.min_depth == 3) {
 				mask = ~0ull;
-			} else if (box_hits(v.box, blkc, M.g.half_size[2])) {
+			} else if (vol_hits_t<G>(v.vol, blkc, M.g.half_size[2])) {
 				if (v.min_depth == 2) {
 					mask = ~0ull;
 				} else {
 					for (uint32_t o = 0; o < 8; ++o) {
 						double oc[3];
 						child_center(blkc, M.g.half_size[1], o, oc);
-						if (!box_hits(v.box, oc, M.g.half_size[1])) continue;
+						if (!vol_hits_t<G>(v.vol, oc, M.g.half_size[1])) continue;
 						const uint32_t x0 = (o & 1u) << 1, y0 = o & 2u, z0 = (o & 4u) >> 1;
 						if (v.min_depth == 1) {
 							mask |= octet_mask_of(x0, y0, z0);
@@ -474,7 +549,7 @@ __global__ void __launch_bounds__(64) k_volume_mark(DeviceMap M, VolumeArgs v)
 						for (uint32_t j = 0; j < 8; ++j) {
 							double vc[3];
 							child_center(oc, M.g.half_size[0], j, vc);
-							if (box_hits(v.box, vc, M.g.half_size[0]))
+							if (vol_hits_t<G>(v.vol, vc, M.g.half_size[0]))
 								mask |= 1ull << linear2(x0 + (j & 1u), y0 + ((j >> 1) & 1u), z0 + (j >> 2));
 						}
 					}
@@ -484,5 +559,30 @@ __global__ void __launch_bounds__(64) k_volume_mark(DeviceMap M, VolumeArgs v)
 	}
 	// the masks of a block belong to one thread here, and no scan is in flight
 	if (mask) M.miss_mask[(size_t)slot * 64 + t] |= mask;
+}
+
+// One level of the device descent of setValueVolume for a general volume: one thread per (frontier
+// node, child); the children whose cube passes go to the next frontier (keys in units of the child
+// depth, centres accumulated like getChildCenter).  *out_n counts every passing child, also those
+// beyond cap, so that the host can tell an overflow.
+__global__ void __launch_bounds__(256) k_volume_descend(Volume vol, const unsigned long long* in_key, const double* in_c, uint32_t n_in,
+                                                        double chs, unsigned long long* out_key, double* out_c, uint32_t cap,
+                                                        unsigned int* out_n)
+{
+	const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (t >= (size_t)n_in * 8) return;
+	const uint32_t node = (uint32_t)(t >> 3), i = (uint32_t)(t & 7);
+	const double pc[3] = {in_c[3 * (size_t)node], in_c[3 * (size_t)node + 1], in_c[3 * (size_t)node + 2]};
+	double c[3];
+	child_center(pc, chs, i, c);
+	if (!vol_hits(vol, c, chs)) return;
+	const uint32_t at = atomicAdd(out_n, 1u);
+	if (at >= cap) return;
+	uint32_t x, y, z;
+	unpack_key(in_key[node], x, y, z);
+	out_key[at] = pack_key((x << 1) | (i & 1u), (y << 1) | ((i >> 1) & 1u), (z << 1) | (i >> 2));
+	out_c[3 * (size_t)at] = c[0];
+	out_c[3 * (size_t)at + 1] = c[1];
+	out_c[3 * (size_t)at + 2] = c[2];
 }
 }  // namespace ufo_b200

@@ -860,7 +860,8 @@ void enqueue_scan(Map* m, PendingScan& p)
 	}
 	if (p.has_vol) {
 		// setValueVolume: the marks come from the box instead of a scan
-		k_volume_mark<<<p.vol.nx * p.vol.ny * p.vol.nz, 64, 0, s>>>(M, p.vol);
+		if (p.vol.general) k_volume_mark<true><<<p.vol.nx * p.vol.ny * p.vol.nz, 64, 0, s>>>(M, p.vol);
+		else k_volume_mark<false><<<p.vol.nx * p.vol.ny * p.vol.nz, 64, 0, s>>>(M, p.vol);
 		++m->launches;
 		if (m->profiling) CK(cudaEventRecord(m->ev[2], s));
 	} else if (a.n) {
@@ -1903,6 +1904,59 @@ int ufo_b200_export_leaves(ufo_b200_map* m, uint64_t* codes, float* logodds, uin
 
 namespace
 {
+static_assert(sizeof(VolRec) == sizeof(ufo_b200_volume) && offsetof(ufo_b200_volume, v) == offsetof(VolRec, v),
+              "ufo_b200_volume and VolRec must share their layout");
+
+const VolRec* as_records(const ufo_b200_volume* bv) { return reinterpret_cast<const VolRec*>(bv); }
+
+// the AABB record of a box6 (centre xyz, half size xyz)
+VolRec aabb_record(const double* box6)
+{
+	VolRec r{};
+	r.type = kVolAABB;
+	for (int k = 0; k < 6; ++k) r.v[k] = box6[k];
+	return r;
+}
+
+// a volume handed in through the C ABI: NULL only when empty, known shape types only
+bool volume_ok(Map* m, const ufo_b200_volume* bv, size_t n_bv)
+{
+	if (n_bv && !bv) return false;
+	if (n_bv > 0xffffffffull) {
+		if (m) m->set_error("a bounding volume of %zu shapes is not supported (at most 2^32 - 1)", n_bv);
+		return false;
+	}
+	for (size_t i = 0; i < n_bv; ++i) {
+		if (bv[i].type >= kVolTypes) {
+			if (m) m->set_error("bounding volume record %zu has the unknown type %u", i, bv[i].type);
+			return false;
+		}
+	}
+	return true;
+}
+
+// the records of a volume in device memory for the duration of one call
+struct DeviceVolume {
+	VolRec* d = nullptr;
+	DeviceVolume() = default;
+	DeviceVolume(const DeviceVolume&) = delete;
+	DeviceVolume& operator=(const DeviceVolume&) = delete;
+	~DeviceVolume()
+	{
+		if (d) cudaFree(d);
+	}
+	Volume upload(const Volume& host, cudaStream_t s)
+	{
+		Volume out = host;  // lo / hi travel as they are
+		out.rec = nullptr;
+		if (!host.n) return out;
+		CK(cudaMalloc(&d, sizeof(VolRec) * host.n));
+		CK(cudaMemcpyAsync(d, host.rec, sizeof(VolRec) * host.n, cudaMemcpyHostToDevice, s));
+		out.rec = d;
+		return out;
+	}
+};
+
 // ---- file image (ufo_export.cuh): the levels above the bricks, on the host ----
 struct UpNode {
 	int32_t child[8];  // -1: absent; >= 0: index into nodes (depth > 5) or into the sorted brick list (depth 5)
@@ -1923,7 +1977,7 @@ struct ExportPlan {
 	uint32_t levels = 16;
 	uint32_t min_depth = 0;
 	bool pruned = false;
-	ExportBox box{};
+	Volume vol{nullptr, 0, {}, {}};  // host records
 	const Geometry* g = nullptr;
 };
 
@@ -1953,7 +2007,7 @@ int32_t build_upper(ExportPlan& plan, uint32_t d, size_t lo, size_t hi, const do
 		while (end < hi && ((plan.codes[end] >> shift) & 7ull) == i) ++end;
 		double cc[3];
 		child_center(c, chs, i, cc);
-		const bool hit = box_hits(plan.box, cc, chs);
+		const bool hit = vol_hits(plan.vol, cc, chs);
 		if (hit) n.hit |= (uint8_t)(1u << i);
 		n.child[i] = -1;
 		occ[i] = 0.0f;
@@ -2036,7 +2090,7 @@ void emit_upper(const ExportPlan& plan, const std::vector<unsigned long long>& o
 // Produces the node stream (optionally behind the file header) through sink(ptr, len) calls, in
 // order.  *total = bytes produced.
 template <class Sink>
-int export_image(Map* m, int pruned, uint32_t min_depth, const double* box6, bool with_header, Sink&& sink,
+int export_image(Map* m, int pruned, uint32_t min_depth, const Volume& vol, bool with_header, Sink&& sink,
                  unsigned long long* total)
 {
 	if (m->device == -2) return UFO_B200_E_CUDA;
@@ -2059,14 +2113,7 @@ int export_image(Map* m, int pruned, uint32_t min_depth, const double* box6, boo
 	plan.min_depth = min_depth;
 	plan.pruned = pruned != 0;
 	plan.g = &m->M.g;
-	if (box6) {
-		// the reference's AABB stores centre and half size (geometry/aabb.h:49-70); getMin/getMax
-		plan.box.on = 1;
-		for (int k = 0; k < 3; ++k) {
-			plan.box.lo[k] = box6[k] - box6[3 + k];
-			plan.box.hi[k] = box6[k] + box6[3 + k];
-		}
-	}
+	plan.vol = vol;
 	*total = 0;
 	const double c0[3] = {0.0, 0.0, 0.0};
 	auto header = [&](char* head, size_t cap, unsigned long long data_size) {
@@ -2077,7 +2124,7 @@ int export_image(Map* m, int pruned, uint32_t min_depth, const double* box6, boo
 		                "uncompressed_data_size %d\ndata\n",
 		                color ? "occupancy_map_color" : "occupancy_map", m->M.g.resolution, plan.levels, (int)data_size);
 	};
-	if (!box_hits(plan.box, c0, plan.g->half_size[plan.levels])) {
+	if (!vol_hits(plan.vol, c0, plan.g->half_size[plan.levels])) {
 		// "No node intersects": the reference writes no node data at all (OMB:1462-1468)
 		if (with_header) {
 			char head[512];
@@ -2092,16 +2139,26 @@ int export_image(Map* m, int pruned, uint32_t min_depth, const double* box6, boo
 	BrickInfo* d_info = nullptr;
 	unsigned long long* d_offs = nullptr;
 	uint8_t* d_out = nullptr;
+	DeviceVolume dvol;
 	auto cleanup = [&]() {
 		if (d_info) cudaFree(d_info);
 		if (d_offs) cudaFree(d_offs);
 		if (d_out) cudaFree(d_out);
 	};
 	try {
+		// an empty or single-box volume takes the instantiation with the inline box test
+		Volume hv = plan.vol;
+		const bool general = volume_is_general(hv);
+		const Volume dv = dvol.upload(hv, s);
+		auto brick_stream = [&](uint32_t n, size_t smem, const unsigned long long* offs, uint8_t* out) {
+			if (color && general) k_brick_stream<true, true><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
+			else if (color) k_brick_stream<true, false><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
+			else if (general) k_brick_stream<false, true><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
+			else k_brick_stream<false, false><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
+		};
 		if (nb) {
 			CK(cudaMalloc(&d_info, sizeof(BrickInfo) * nb));
-			if (color) k_brick_stream<true><<<nb, 64, 0, s>>>(m->M, nb, pruned, min_depth, plan.box, d_info, nullptr, nullptr);
-			else k_brick_stream<false><<<nb, 64, 0, s>>>(m->M, nb, pruned, min_depth, plan.box, d_info, nullptr, nullptr);
+			brick_stream(nb, 0, nullptr, nullptr);
 			CK(cudaGetLastError());
 			CK(cudaMemcpyAsync(plan.info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
 			CK(cudaMemcpyAsync(keys.data(), m->M.brick_key, 8ull * nb, cudaMemcpyDeviceToHost, s));
@@ -2145,8 +2202,7 @@ int export_image(Map* m, int pruned, uint32_t min_depth, const double* box6, boo
 			CK(cudaMalloc(&d_offs, 8ull * nb));
 			CK(cudaMalloc(&d_out, packed_bytes));
 			CK(cudaMemcpyAsync(d_offs, offs.data(), 8ull * nb, cudaMemcpyHostToDevice, s));
-			if (color) k_brick_stream<true><<<nb, 64, kBrickStreamMax, s>>>(m->M, nb, pruned, min_depth, plan.box, d_info, d_offs, d_out);
-			else k_brick_stream<false><<<nb, 64, kBrickStreamMax, s>>>(m->M, nb, pruned, min_depth, plan.box, d_info, d_offs, d_out);
+			brick_stream(nb, kBrickStreamMax, d_offs, d_out);
 			CK(cudaGetLastError());
 			CK(cudaMemcpyAsync(packed.data(), d_out, packed_bytes, cudaMemcpyDeviceToHost, s));
 			CK(cudaStreamSynchronize(s));
@@ -2225,34 +2281,53 @@ bool lz4_compress(const std::vector<uint8_t>& in, int acceleration, int level, s
 }
 }  // namespace
 
+namespace
+{
+// the rejections shared by the two setValueVolume entry points
+int set_value_volume_allowed(Map* m, uint32_t min_depth)
+{
+	if (min_depth > 4 || m->M.g.depth_levels < 5) {
+		m->set_error("setValueVolume: min_depth %u > 4 (or depth_levels < 5) is not supported", min_depth);
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (m->M.color && min_depth > 0) {
+		m->set_error("setValueVolume on a colour map is supported at min_depth 0 only");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (m->M.shard_world > 1) {
+		m->set_error("setValueVolume on a sharded map is not supported");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	return UFO_B200_OK;
+}
+
+// marks the volume's voxels (k_volume_mark over the candidate bricks of v) and sets them to
+// clamp(float(logit(occupancy))): setOccupancy(LogitType&, LogitType const&), OMB:1151-1157
+int set_value_volume_run(Map* m, const VolumeArgs& v, double occupancy)
+{
+	const float lo = (float)m->cmin_log, hi = (float)m->cmax_log;
+	float value = (float)to_logit(occupancy);
+	value = value < lo ? lo : (hi < value ? hi : value);
+	const double origin[3] = {0.0, 0.0, 0.0};
+	return do_insert(m, origin, nullptr, false, 0, nullptr, UFO_B200_XYZ_F64, -1.0, 0, 0, 0, 0, 0, nullptr, &v, value);
+}
+
+constexpr uint32_t kVolumeBrickLimit = 1u << 22;
+}  // namespace
+
 extern "C" {
 
 int ufo_b200_set_value_volume(ufo_b200_map* m, const double box6[6], double occupancy, uint32_t min_depth)
 {
 	if (!m || !box6) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
-		if (min_depth > 4 || m->M.g.depth_levels < 5) {
-			m->set_error("setValueVolume: min_depth %u > 4 (or depth_levels < 5) is not supported", min_depth);
-			return (int)UFO_B200_E_UNSUPPORTED;
-		}
-		if (m->M.color && min_depth > 0) {
-			m->set_error("setValueVolume on a colour map is supported at min_depth 0 only");
-			return (int)UFO_B200_E_UNSUPPORTED;
-		}
-		if (m->M.shard_world > 1) {
-			m->set_error("setValueVolume on a sharded map is not supported");
-			return (int)UFO_B200_E_UNSUPPORTED;
-		}
+		const int allowed = set_value_volume_allowed(m, min_depth);
+		if (allowed != UFO_B200_OK) return allowed;
 		const Geometry& g = m->M.g;
-		VolumeArgs v{};
-		v.min_depth = min_depth;
-		v.box.on = 1;
-		for (int k = 0; k < 3; ++k) {
-			v.box.lo[k] = box6[k] - box6[3 + k];
-			v.box.hi[k] = box6[k] + box6[3 + k];
-		}
+		const VolRec rec = aabb_record(box6);
+		const Volume hv{&rec, 1, {}, {}};
 		const double c0[3] = {0.0, 0.0, 0.0};
-		if (!box_hits(v.box, c0, g.half_size[g.depth_levels])) return (int)UFO_B200_OK;  // no node intersects
+		if (!vol_hits(hv, c0, g.half_size[g.depth_levels])) return (int)UFO_B200_OK;  // no node intersects
 		// candidate bricks: the key range of the box, one brick of slack on every side (the kernel
 		// decides with the reference's own cube tests)
 		const double ext = g.half_size[g.depth_levels];
@@ -2260,7 +2335,8 @@ int ufo_b200_set_value_volume(ufo_b200_map* m, const double box6[6], double occu
 		uint32_t first[3], count[3];
 		unsigned long long total = 1;
 		for (int k = 0; k < 3; ++k) {
-			const double lo = std::max(v.box.lo[k], -ext), hi = std::min(v.box.hi[k], ext);
+			const double blo = box6[k] - box6[3 + k], bhi = box6[k] + box6[3 + k];
+			const double lo = std::max(blo, -ext), hi = std::min(bhi, ext);
 			long long a = ((long long)std::floor(lo * g.resolution_factor) + (long long)g.max_value) >> 4;
 			long long b = ((long long)std::floor(hi * g.resolution_factor) + (long long)g.max_value) >> 4;
 			a = std::min(std::max(a - 1, 0ll), top);
@@ -2269,37 +2345,161 @@ int ufo_b200_set_value_volume(ufo_b200_map* m, const double box6[6], double occu
 			count[k] = (uint32_t)(b - a + 1);
 			total *= count[k];
 		}
-		if (total > (1ull << 22)) {
+		if (total > kVolumeBrickLimit) {
 			m->set_error("setValueVolume: the box covers %llu bricks (limit 4194304)", total);
 			return (int)UFO_B200_E_UNSUPPORTED;
 		}
+		CK(cudaSetDevice(m->device));
+		DeviceVolume dvol;
+		VolumeArgs v{};
+		Volume box = hv;
+		volume_is_general(box);  // one AABB: lo / hi for the inline test
+		v.vol = dvol.upload(box, m->stream);
+		v.min_depth = min_depth;
 		v.bx0 = first[0];
 		v.by0 = first[1];
 		v.bz0 = first[2];
 		v.nx = count[0];
 		v.ny = count[1];
 		v.nz = count[2];
-		// setOccupancy(LogitType&, LogitType const&): float clamp of the float logit (OMB:1151-1157)
-		const float lo = (float)m->cmin_log, hi = (float)m->cmax_log;
-		float value = (float)to_logit(occupancy);
-		value = value < lo ? lo : (hi < value ? hi : value);
-		const double origin[3] = {0.0, 0.0, 0.0};
-		return do_insert(m, origin, nullptr, false, 0, nullptr, UFO_B200_XYZ_F64, -1.0, 0, 0, 0, 0, 0, nullptr, &v, value);
+		return set_value_volume_run(m, v, occupancy);
+	});
+}
+
+int ufo_b200_set_value_volume_bv(ufo_b200_map* m, const ufo_b200_volume* bv, double occupancy, uint32_t min_depth)
+{
+	if (!m || !bv) return UFO_B200_E_INVALID;
+	// argument checks that need no device
+	if (!volume_ok(m, bv, 1)) return UFO_B200_E_INVALID;
+	const int allowed = set_value_volume_allowed(m, min_depth);
+	if (allowed != UFO_B200_OK) return allowed;
+	if (m->M.route_world > 1) {
+		m->set_error("setValueVolume on a routed map is not supported");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	return guarded(m, [&]() {
+		const Geometry& g = m->M.g;
+		const Volume hv{as_records(bv), 1, {}, {}};
+		const double c0[3] = {0.0, 0.0, 0.0};
+		if (!vol_hits(hv, c0, g.half_size[g.depth_levels])) return (int)UFO_B200_OK;  // no node intersects
+		CK(cudaSetDevice(m->device));
+		sync_map(m);
+		cudaStream_t s = m->stream;
+		DeviceVolume dvol;
+		Volume hvk = hv;
+		const int general = volume_is_general(hvk) ? 1 : 0;
+		const Volume dv = dvol.upload(hvk, s);
+		// descent from the root to the bricks, one level per launch; frontier = (key, centre)
+		unsigned long long *d_key[2] = {nullptr, nullptr};
+		double* d_c[2] = {nullptr, nullptr};
+		unsigned int* d_n = nullptr;
+		auto cleanup = [&]() {
+			for (int i = 0; i < 2; ++i) {
+				if (d_key[i]) cudaFree(d_key[i]);
+				if (d_c[i]) cudaFree(d_c[i]);
+				d_key[i] = nullptr;
+				d_c[i] = nullptr;
+			}
+			if (d_n) cudaFree(d_n);
+			d_n = nullptr;
+		};
+		int rc = UFO_B200_OK;
+		try {
+			CK(cudaMalloc(&d_n, sizeof(unsigned int)));
+			CK(cudaMalloc(&d_key[0], 8));
+			CK(cudaMalloc(&d_c[0], 24));
+			CK(cudaMemsetAsync(d_key[0], 0, 8, s));
+			CK(cudaMemsetAsync(d_c[0], 0, 24, s));
+			uint32_t n_in = 1, cur = 0;
+			for (uint32_t d = g.depth_levels; d > 4 && n_in; --d) {
+				// children of depth d - 1
+				const uint32_t cap = (uint32_t)std::min<unsigned long long>(8ull * n_in, kVolumeBrickLimit);
+				const uint32_t nxt = cur ^ 1u;
+				CK(cudaMalloc(&d_key[nxt], 8ull * cap));
+				CK(cudaMalloc(&d_c[nxt], 24ull * cap));
+				CK(cudaMemsetAsync(d_n, 0, sizeof(unsigned int), s));
+				const unsigned long long threads = 8ull * n_in;
+				k_volume_descend<<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(dv, d_key[cur], d_c[cur], n_in, g.half_size[d - 1],
+				                                                                    d_key[nxt], d_c[nxt], cap, d_n);
+				CK(cudaGetLastError());
+				unsigned int got = 0;
+				CK(cudaMemcpyAsync(&got, d_n, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+				CK(cudaStreamSynchronize(s));
+				CK(cudaFree(d_key[cur]));
+				CK(cudaFree(d_c[cur]));
+				d_key[cur] = nullptr;
+				d_c[cur] = nullptr;
+				if (got > kVolumeBrickLimit) {
+					m->set_error("setValueVolume: %u nodes of depth %u pass the volume (limit 4194304)", got, d - 1);
+					cleanup();
+					return (int)UFO_B200_E_UNSUPPORTED;
+				}
+				n_in = got;
+				cur = nxt;
+			}
+			if (n_in) {
+				VolumeArgs v{};
+				v.vol = dv;
+				v.min_depth = min_depth;
+				v.nx = n_in;
+				v.ny = 1;
+				v.nz = 1;
+				v.cand = d_key[cur];
+				v.general = general;
+				rc = set_value_volume_run(m, v, occupancy);
+				sync_map(m);
+			}
+		} catch (...) {
+			cleanup();
+			throw;
+		}
+		cleanup();
+		return rc;
+	});
+}
+
+int ufo_b200_write_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, uint32_t min_depth, int expanded,
+                      void* buf, size_t cap, size_t* size)
+{
+	if (!m || !size) return UFO_B200_E_INVALID;
+	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() {
+		uint8_t* out = static_cast<uint8_t*>(buf);
+		size_t at = 0;
+		unsigned long long total = 0;
+		int rc = export_image(m, expanded ? 0 : 1, min_depth, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, true,
+		                      [&](const void* p, size_t len) {
+			                      if (out && at + len <= cap) std::memcpy(out + at, p, len);
+			                      at += len;
+		                      },
+		                      &total);
+		*size = (size_t)total;
+		return rc;
 	});
 }
 
 int ufo_b200_write(ufo_b200_map* m, const double* box6, uint32_t min_depth, int expanded, void* buf, size_t cap,
                    size_t* size)
 {
+	const VolRec r = box6 ? aabb_record(box6) : VolRec{};
+	return ufo_b200_write_bv(m, reinterpret_cast<const ufo_b200_volume*>(&r), box6 ? 1 : 0, min_depth, expanded, buf, cap, size);
+}
+
+int ufo_b200_write_data_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, uint32_t min_depth, void* buf,
+                           size_t cap, size_t* size)
+{
 	if (!m || !size) return UFO_B200_E_INVALID;
+	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
 		uint8_t* out = static_cast<uint8_t*>(buf);
 		size_t at = 0;
 		unsigned long long total = 0;
-		int rc = export_image(m, expanded ? 0 : 1, min_depth, box6, true, [&](const void* p, size_t len) {
-			if (out && at + len <= cap) std::memcpy(out + at, p, len);
-			at += len;
-		}, &total);
+		int rc = export_image(m, 1, min_depth, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, false,
+		                      [&](const void* p, size_t len) {
+			                      if (out && at + len <= cap) std::memcpy(out + at, p, len);
+			                      at += len;
+		                      },
+		                      &total);
 		*size = (size_t)total;
 		return rc;
 	});
@@ -2308,18 +2508,8 @@ int ufo_b200_write(ufo_b200_map* m, const double* box6, uint32_t min_depth, int 
 int ufo_b200_write_data(ufo_b200_map* m, const double* box6, uint32_t min_depth, void* buf, size_t cap,
                         size_t* size)
 {
-	if (!m || !size) return UFO_B200_E_INVALID;
-	return guarded(m, [&]() {
-		uint8_t* out = static_cast<uint8_t*>(buf);
-		size_t at = 0;
-		unsigned long long total = 0;
-		int rc = export_image(m, 1, min_depth, box6, false, [&](const void* p, size_t len) {
-			if (out && at + len <= cap) std::memcpy(out + at, p, len);
-			at += len;
-		}, &total);
-		*size = (size_t)total;
-		return rc;
-	});
+	const VolRec r = box6 ? aabb_record(box6) : VolRec{};
+	return ufo_b200_write_data_bv(m, reinterpret_cast<const ufo_b200_volume*>(&r), box6 ? 1 : 0, min_depth, buf, cap, size);
 }
 
 int ufo_b200_write_file(ufo_b200_map* m, const char* filename, const double* box6, uint32_t min_depth,
@@ -2332,9 +2522,10 @@ int ufo_b200_write_file(ufo_b200_map* m, const char* filename, const double* box
 			m->set_error("cannot open %s", filename);
 			return (int)UFO_B200_E_INVALID;
 		}
+		const VolRec r = box6 ? aabb_record(box6) : VolRec{};
 		unsigned long long total = 0;
 		bool ok = true;
-		int rc = export_image(m, expanded ? 0 : 1, min_depth, box6, true,
+		int rc = export_image(m, expanded ? 0 : 1, min_depth, Volume{&r, box6 ? 1u : 0u, {}, {}}, true,
 		                      [&](const void* p, size_t len) { ok = ok && fwrite(p, 1, len, f) == len; }, &total);
 		ok = fclose(f) == 0 && ok;
 		if (rc == UFO_B200_OK && !ok) {
@@ -2737,11 +2928,12 @@ int ufo_b200_changed_codes(ufo_b200_map* m, uint32_t depth, uint64_t* codes, siz
 	});
 }
 
-int ufo_b200_write_compressed(ufo_b200_map* m, const double* box6, uint32_t min_depth, int data_only,
-                              int acceleration_level, int compression_level, void* buf, size_t cap, size_t* size,
-                              size_t* uncompressed_size)
+int ufo_b200_write_compressed_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, uint32_t min_depth,
+                                 int data_only, int acceleration_level, int compression_level, void* buf, size_t cap,
+                                 size_t* size, size_t* uncompressed_size)
 {
 	if (!m || !size) return UFO_B200_E_INVALID;
+	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
 		if (!lz4().ok) {
 			m->set_error("liblz4.so.1 not found: compressed output is unavailable");
@@ -2749,7 +2941,7 @@ int ufo_b200_write_compressed(ufo_b200_map* m, const double* box6, uint32_t min_
 		}
 		std::vector<uint8_t> raw;
 		unsigned long long total = 0;
-		int rc = export_image(m, 1, min_depth, box6, false, [&](const void* p, size_t len) {
+		int rc = export_image(m, 1, min_depth, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, false, [&](const void* p, size_t len) {
 			const uint8_t* b = static_cast<const uint8_t*>(p);
 			raw.insert(raw.end(), b, b + len);
 		}, &total);
@@ -2780,6 +2972,15 @@ int ufo_b200_write_compressed(ufo_b200_map* m, const double* box6, uint32_t min_
 		}
 		return (int)UFO_B200_OK;
 	});
+}
+
+int ufo_b200_write_compressed(ufo_b200_map* m, const double* box6, uint32_t min_depth, int data_only,
+                              int acceleration_level, int compression_level, void* buf, size_t cap, size_t* size,
+                              size_t* uncompressed_size)
+{
+	const VolRec r = box6 ? aabb_record(box6) : VolRec{};
+	return ufo_b200_write_compressed_bv(m, reinterpret_cast<const ufo_b200_volume*>(&r), box6 ? 1 : 0, min_depth, data_only,
+	                                    acceleration_level, compression_level, buf, cap, size, uncompressed_size);
 }
 
 int ufo_b200_cast_rays(ufo_b200_map* m, const double* origins, const double* directions, size_t n,
@@ -2826,36 +3027,52 @@ int ufo_b200_cast_rays(ufo_b200_map* m, const double* origins, const double* dir
 	});
 }
 
-int ufo_b200_export_nodes(ufo_b200_map* m, uint32_t depth, int occupied, int free_space, int unknown, const double* box6,
-                          uint64_t* codes, float* logodds, uint8_t* rgb, size_t cap, size_t* n)
+}  // extern "C"
+
+namespace
 {
-	if (!m || !n) return UFO_B200_E_INVALID;
-	return guarded(m, [&]() {
-		CK(cudaSetDevice(m->device));
-		sync_map(m);
-		*n = 0;
-		if (depth > m->M.g.depth_levels) return (int)UFO_B200_E_INVALID;
-		NodeFilter f{};
-		f.depth = depth;
-		f.occupied = occupied;
-		f.free_ = free_space;
-		f.unknown = unknown;
-		if (box6) {
-			f.box.on = 1;
-			for (int k = 0; k < 3; ++k) {
-				f.box.lo[k] = box6[k] - box6[3 + k];
-				f.box.hi[k] = box6[k] + box6[3 + k];
-			}
-		}
+// Filtered leaf iteration (ufo_export.cuh, k_export_nodes / k_export_upper).  chain == false: the
+// node's own cube is tested against the volume; chain == true: every cube on its path from the root.
+int export_nodes(Map* m, uint32_t depth, int occupied, int free_space, int unknown, const Volume& vol, bool chain,
+                 uint64_t* codes, float* logodds, uint8_t* rgb, size_t cap, size_t* n)
+{
+	CK(cudaSetDevice(m->device));
+	sync_map(m);
+	*n = 0;
+	if (depth > m->M.g.depth_levels) return (int)UFO_B200_E_INVALID;
+	NodeFilter f{};
+	f.depth = depth;
+	f.occupied = occupied;
+	f.free_ = free_space;
+	f.unknown = unknown;
+	f.chain = chain && vol.n ? 1 : 0;
+	if (f.chain) {
+		const double c0[3] = {0.0, 0.0, 0.0};
+		if (!vol_hits(vol, c0, m->M.g.half_size[m->M.g.depth_levels])) return (int)UFO_B200_OK;  // the root misses
+	}
+	{
 		cudaStream_t s = m->stream;
 		unsigned long long *d_count = nullptr, *d_codes = nullptr;
 		float* d_occ = nullptr;
 		uint32_t* d_rgb = nullptr;
+		uint8_t* d_ok = nullptr;
+		double* d_bc = nullptr;
+		DeviceVolume dvol;
 		auto cleanup = [&]() {
-			for (void* p : {(void*)d_count, (void*)d_codes, (void*)d_occ, (void*)d_rgb})
+			for (void* p : {(void*)d_count, (void*)d_codes, (void*)d_occ, (void*)d_rgb, (void*)d_ok, (void*)d_bc})
 				if (p) cudaFree(p);
 		};
 		try {
+			Volume hv = vol;
+			volume_is_general(hv);  // lo / hi of a single box, tested inline without the chain
+			f.vol = dvol.upload(hv, s);
+			if (f.chain && depth <= 4 && m->n_bricks) {
+				CK(cudaMalloc(&d_ok, m->n_bricks));
+				CK(cudaMalloc(&d_bc, 24ull * m->n_bricks));
+				k_brick_chain<<<(m->n_bricks + 255) / 256, 256, 0, s>>>(m->M, m->n_bricks, f.vol, d_ok, d_bc);
+				f.brick_ok = d_ok;
+				f.brick_c = d_bc;
+			}
 			CK(cudaMalloc(&d_count, 8));
 			const bool fill = codes != nullptr && cap > 0;
 			if (fill) {
@@ -2866,9 +3083,13 @@ int ufo_b200_export_nodes(ufo_b200_map* m, uint32_t depth, int occupied, int fre
 			CK(cudaMemsetAsync(d_count, 0, 8, s));
 			if (depth <= 4) {
 				const size_t threads = (size_t)m->n_bricks * 64;
-				if (threads) k_export_nodes<<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(m->M, m->n_bricks, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
+				if (threads && f.chain)
+					k_export_nodes<true><<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(m->M, m->n_bricks, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
+				else if (threads)
+					k_export_nodes<false><<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(m->M, m->n_bricks, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
 			} else if (m->n_upper) {
-				k_export_upper<<<(m->n_upper + 255) / 256, 256, 0, s>>>(m->M, m->n_upper, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
+				if (f.chain) k_export_upper<true><<<(m->n_upper + 255) / 256, 256, 0, s>>>(m->M, m->n_upper, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
+				else k_export_upper<false><<<(m->n_upper + 255) / 256, 256, 0, s>>>(m->M, m->n_upper, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
 			}
 			CK(cudaGetLastError());
 			unsigned long long cnt = 0;
@@ -2894,8 +3115,119 @@ int ufo_b200_export_nodes(ufo_b200_map* m, uint32_t depth, int occupied, int fre
 			throw;
 		}
 		cleanup();
-		return (int)UFO_B200_OK;
+	}
+	return (int)UFO_B200_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int ufo_b200_export_nodes(ufo_b200_map* m, uint32_t depth, int occupied, int free_space, int unknown, const double* box6,
+                          uint64_t* codes, float* logodds, uint8_t* rgb, size_t cap, size_t* n)
+{
+	if (!m || !n) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() {
+		const VolRec r = box6 ? aabb_record(box6) : VolRec{};
+		return export_nodes(m, depth, occupied, free_space, unknown, Volume{&r, box6 ? 1u : 0u, {}, {}}, false, codes, logodds, rgb, cap, n);
 	});
+}
+
+int ufo_b200_export_nodes_bv(ufo_b200_map* m, uint32_t depth, int occupied, int free_space, int unknown,
+                             const ufo_b200_volume* bv, size_t n_bv, uint64_t* codes, float* logodds, uint8_t* rgb,
+                             size_t cap, size_t* n)
+{
+	if (!m || !n) return UFO_B200_E_INVALID;
+	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() {
+		return export_nodes(m, depth, occupied, free_space, unknown, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, true, codes, logodds,
+		                    rgb, cap, n);
+	});
+}
+
+}  // extern "C"
+
+namespace
+{
+Vec3 vec_of(const double* p) { return Vec3{p[0], p[1], p[2]}; }
+Vec3 vcross(Vec3 a, Vec3 b)
+{
+	return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
+}
+double vdot(Vec3 a, Vec3 b) { return (a.x * b.x + a.y * b.y) + a.z * b.z; }
+Vec3 vnormalized(Vec3 a) { return vdiv(a, vnorm(a)); }
+
+// Plane(v1, v2, v3): normal = normalised (v3 - v2) x (v1 - v2), distance = -normal . v2
+void plane_of(Vec3 v1, Vec3 v2, Vec3 v3, double* out)
+{
+	const Vec3 n = vnormalized(vcross(vsub(v3, v2), vsub(v1, v2)));
+	out[0] = n.x;
+	out[1] = n.y;
+	out[2] = n.z;
+	out[3] = -vdot(n, v2);
+}
+}  // namespace
+
+extern "C" {
+
+int ufo_b200_geometry_frustum(const double pos_in[3], const double target[3], const double up[3], double vertical_angle,
+                              double horizontal_angle, double near_distance, double far_distance, double planes[24])
+{
+	if (!pos_in || !target || !up || !planes) return UFO_B200_E_INVALID;
+	const double ratio = horizontal_angle / vertical_angle;
+	const double tang = std::tan(vertical_angle * 0.5);
+	const double near_h = near_distance * tang, near_w = near_h * ratio;
+	const double far_h = far_distance * tang, far_w = far_h * ratio;
+	const Vec3 pos = vec_of(pos_in);
+	const Vec3 Z = vnormalized(vsub(pos, vec_of(target)));
+	const Vec3 X = vnormalized(vcross(vec_of(up), Z));
+	const Vec3 Y = vcross(Z, X);
+	const Vec3 nc = vsub(pos, vscale(Z, near_distance)), fc = vsub(pos, vscale(Z, far_distance));
+	// corner = centre (+/-) Y * height (+/-) X * width, summed left to right
+	auto corner = [&](Vec3 c, double ys, double h, double xs, double w) {
+		const Vec3 a = ys > 0 ? vadd(c, vscale(Y, h)) : vsub(c, vscale(Y, h));
+		return xs > 0 ? vadd(a, vscale(X, w)) : vsub(a, vscale(X, w));
+	};
+	const Vec3 ntl = corner(nc, 1, near_h, -1, near_w), ntr = corner(nc, 1, near_h, 1, near_w);
+	const Vec3 nbl = corner(nc, -1, near_h, -1, near_w), nbr = corner(nc, -1, near_h, 1, near_w);
+	const Vec3 ftl = corner(fc, 1, far_h, -1, far_w), ftr = corner(fc, 1, far_h, 1, far_w);
+	const Vec3 fbl = corner(fc, -1, far_h, -1, far_w), fbr = corner(fc, -1, far_h, 1, far_w);
+	plane_of(ntr, ntl, ftl, planes);       // top
+	plane_of(nbl, nbr, fbr, planes + 4);   // bottom
+	plane_of(ntl, nbl, fbl, planes + 8);   // left
+	plane_of(nbr, ntr, fbr, planes + 12);  // right
+	plane_of(ntl, ntr, nbr, planes + 16);  // near
+	plane_of(ftr, ftl, fbl, planes + 20);  // far
+	return UFO_B200_OK;
+}
+
+int ufo_b200_geometry_plane(const double v1[3], const double v2[3], const double v3[3], double plane[4])
+{
+	if (!v1 || !v2 || !v3 || !plane) return UFO_B200_E_INVALID;
+	plane_of(vec_of(v1), vec_of(v2), vec_of(v3), plane);
+	return UFO_B200_OK;
+}
+
+int ufo_b200_geometry_ray(const double origin[3], const double direction[3], double ray[6])
+{
+	if (!origin || !direction || !ray) return UFO_B200_E_INVALID;
+	const Vec3 d = vnormalized(vec_of(direction));
+	ray[0] = origin[0];
+	ray[1] = origin[1];
+	ray[2] = origin[2];
+	ray[3] = d.x;
+	ray[4] = d.y;
+	ray[5] = d.z;
+	return UFO_B200_OK;
+}
+
+int ufo_b200_volume_intersects(const ufo_b200_volume* bv, size_t n_bv, const double* centres, const double* half_sizes,
+                               size_t n, uint8_t* out)
+{
+	if ((n && (!centres || !half_sizes || !out)) || !volume_ok(nullptr, bv, n_bv)) return UFO_B200_E_INVALID;
+	const VolRec* r = as_records(bv);
+	for (size_t i = 0; i < n; ++i)
+		out[i] = (n_bv == 0 || volume_hits_any(r, (uint32_t)n_bv, centres + 3 * i, half_sizes + 3 * i)) ? 1 : 0;
+	return UFO_B200_OK;
 }
 
 }  // extern "C"
@@ -2923,7 +3255,7 @@ struct StreamReader {
 struct ImportPlan {
 	std::vector<ImportRec> small, bricks, wipe;  // depth <= 2, depth 4, depth >= 5
 	const Geometry* g = nullptr;
-	ExportBox box{};
+	Volume vol{nullptr, 0, {}, {}};  // host records
 	uint32_t P = 4;
 	uint64_t budget = 1ull << 20;  // bricks a stream may create through collapsed nodes above the brick level
 	bool too_big = false;
@@ -2972,14 +3304,14 @@ void import_rec(ImportPlan& plan, StreamReader& in, uint64_t code, uint32_t dept
 	for (uint32_t i = 0; i < 8 && in.ok; ++i) {
 		double cc[3];
 		child_center(c, chs, i, cc);
-		if (!box_hits(plan.box, cc, chs)) continue;
+		if (!vol_hits(plan.vol, cc, chs)) continue;
 		const uint64_t ccode = code + ((uint64_t)i << (3 * cd));
 		if ((children >> i) & 1u) {
 			if (1 == cd) {
 				for (uint32_t j = 0; j < 8; ++j) {
 					double gc[3];
 					child_center(cc, plan.g->half_size[0], j, gc);
-					if (!box_hits(plan.box, gc, plan.g->half_size[0])) continue;
+					if (!vol_hits(plan.vol, gc, plan.g->half_size[0])) continue;
 					float occ;
 					uint32_t rgb;
 					read_payload(in, plan.P, occ, rgb);
@@ -2997,7 +3329,7 @@ void import_rec(ImportPlan& plan, StreamReader& in, uint64_t code, uint32_t dept
 	}
 }
 
-int import_stream(Map* m, const uint8_t* data, size_t size, const double* box6)
+int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
 {
 	DeviceMap& M = m->M;
 	if (M.g.depth_levels < 5) {
@@ -3013,15 +3345,9 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const double* box6)
 	ImportPlan plan;
 	plan.g = &M.g;
 	plan.P = M.color ? 7 : 4;
-	if (box6) {
-		plan.box.on = 1;
-		for (int k = 0; k < 3; ++k) {
-			plan.box.lo[k] = box6[k] - box6[3 + k];
-			plan.box.hi[k] = box6[k] + box6[3 + k];
-		}
-	}
+	plan.vol = vol;
 	const double c0[3] = {0.0, 0.0, 0.0};
-	if (!box_hits(plan.box, c0, M.g.half_size[M.g.depth_levels])) return UFO_B200_OK;  // no node intersects
+	if (!vol_hits(plan.vol, c0, M.g.half_size[M.g.depth_levels])) return UFO_B200_OK;  // no node intersects
 	StreamReader in{data, size};
 	uint8_t children = 0;
 	in.get(&children, 1);
@@ -3104,12 +3430,14 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const double* box6)
 
 extern "C" {
 
-int ufo_b200_read_data(ufo_b200_map* m, const double* box6, const void* data, size_t size, int compressed,
-                       size_t uncompressed_size)
+int ufo_b200_read_data_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, const void* data, size_t size,
+                          int compressed, size_t uncompressed_size)
 {
 	if (!m || (!data && size)) return UFO_B200_E_INVALID;
+	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
-		if (!compressed) return import_stream(m, static_cast<const uint8_t*>(data), size, box6);
+		const Volume vol{as_records(bv), (uint32_t)n_bv};
+		if (!compressed) return import_stream(m, static_cast<const uint8_t*>(data), size, vol);
 		if (!lz4().ok) {
 			m->set_error("liblz4.so.1 not found: compressed input is unavailable");
 			return (int)UFO_B200_E_UNSUPPORTED;
@@ -3120,8 +3448,16 @@ int ufo_b200_read_data(ufo_b200_map* m, const double* box6, const void* data, si
 			m->set_error("readData: LZ4 decompression failed");
 			return (int)UFO_B200_E_INVALID;
 		}
-		return import_stream(m, raw.data(), (size_t)n, box6);
+		return import_stream(m, raw.data(), (size_t)n, vol);
 	});
+}
+
+int ufo_b200_read_data(ufo_b200_map* m, const double* box6, const void* data, size_t size, int compressed,
+                       size_t uncompressed_size)
+{
+	const VolRec r = box6 ? aabb_record(box6) : VolRec{};
+	return ufo_b200_read_data_bv(m, reinterpret_cast<const ufo_b200_volume*>(&r), box6 ? 1 : 0, data, size, compressed,
+	                             uncompressed_size);
 }
 
 }  // extern "C"
