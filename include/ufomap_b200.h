@@ -80,8 +80,10 @@ int ufo_b200_set_stream(ufo_b200_map* m, void* cuda_stream);
  * unlimited.  depth = insert depth of the free-space rays.  async != 0 returns
  * after the work is enqueued; ufo_b200_wait / ufo_b200_done mirror
  * insertPointCloudWait / insertPointCloudDone (occupancy_map_base.h:430-443).
- * early_stopping != 0 is order-dependent in the reference and is rejected with
- * UFO_B200_E_UNSUPPORTED. */
+ * early_stopping != 0 is order-dependent in the reference: it is rejected with
+ * UFO_B200_E_UNSUPPORTED unless the map opted in with ufo_b200_set_early_stopping(m, 1),
+ * which computes the reference's sequential result exactly (at the cost of extra device
+ * work and memory; see ufo_b200_last_early_stats). */
 int ufo_b200_insert_pointcloud(ufo_b200_map* m, const double origin[3], const void* points,
                                size_t n, int layout, double max_range, uint32_t depth,
                                int simple_ray_casting, uint32_t early_stopping, int discrete,
@@ -411,6 +413,31 @@ typedef struct {
 	uint64_t dirty_reductions; /* reductions on the bitmap of touched bricks */
 } ufo_b200_walk_stats;
 int ufo_b200_last_walk_stats(ufo_b200_map* m, ufo_b200_walk_stats* out);
+
+/* Early stopping.  On the CPU, early_stopping = E > 0 makes a scan cheaper: a ray stops after E
+ * nodes in a row that earlier rays (or its own earlier samples) already put into the scan's free
+ * set.  The result depends on the order of the rays.  Here it costs more than a plain scan: every
+ * ray's walk is stored and the prefixes are solved in parallel rounds until they reach the
+ * reference's sequential answer.  So a map rejects early_stopping != 0 (UFO_B200_E_UNSUPPORTED)
+ * until the caller opts in with exact = 1; exact = 0 restores the rejection.  Any other value:
+ * UFO_B200_E_INVALID.  Needs no device.  Routed passes keep rejecting early_stopping. */
+int ufo_b200_set_early_stopping(ufo_b200_map* m, int exact);
+
+/* The most recent insert's early-stopping work (waits for it to finish); all zero when that
+ * insert did not use early stopping.  The times are CUDA events at profiling level >= 1. */
+typedef struct {
+	uint64_t rounds;      /* rounds of the prefix solver, the last one without a change included */
+	uint64_t converged;   /* 1: the rounds reached their fixed point                    */
+	uint64_t visits;      /* node visits of all walks                                  */
+	uint64_t nodes;       /* distinct nodes the walks visit                            */
+	uint64_t free_nodes;  /* nodes in the scan's free set                              */
+	uint64_t table_bytes; /* device memory of the scan-local node table                */
+	uint64_t id_bytes;    /* device memory of the visit ids and per-ray arrays         */
+	float ms_walk;        /* E1: walks, node ids                                       */
+	float ms_rounds;      /* E2: prefix rounds                                         */
+	float ms_mark;        /* E3: free set -> miss masks                                */
+} ufo_b200_early_stats;
+int ufo_b200_last_early_stats(ufo_b200_map* m, ufo_b200_early_stats* out);
 
 /* Octree::clear(resolution, depth_levels)  octree.h:541-560 -- the server's reset service
  * (server.cpp:364-378): empties the map and changes its geometry. */

@@ -18,7 +18,7 @@
 //
 // Differences, all documented in DESIGN.md: state getters use the INTENDED node semantics
 // (the reference's getNode is off by one level, octree.h:974-985); early_stopping != 0 is
-// rejected (order-dependent in the reference); errors of the void insert functions are
+// rejected (order-dependent in the reference) unless setEarlyStoppingExact(true); errors of the void insert functions are
 // kept in lastError().
 #pragma once
 
@@ -956,6 +956,10 @@ class MapFacade
 	int lastStatus() const noexcept { return last_status_; }
 	std::string lastError() const { return ufo_b200_last_error(map_); }
 	ufo_b200_map* handle() noexcept { return map_; }
+	// early_stopping != 0 is rejected (lastStatus() == UFO_B200_E_UNSUPPORTED) unless the map opts in:
+	// then the reference's sequential result is computed on the device, at extra cost
+	// (ufo_b200_set_early_stopping)
+	void setEarlyStoppingExact(bool exact) { last_status_ = ufo_b200_set_early_stopping(map_, exact ? 1 : 0); }
 
  protected:
 	struct NodeValue {

@@ -55,6 +55,15 @@ class WalkStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class EarlyStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in (
+        "rounds", "converged", "visits", "nodes", "free_nodes", "table_bytes", "id_bytes")] + [
+            (n, C.c_float) for n in ("ms_walk", "ms_rounds", "ms_mark")]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 # every symbol include/ufomap_b200.h declares
 SYMBOLS = [
     "ufo_b200_default_params", "ufo_b200_create", "ufo_b200_destroy", "ufo_b200_last_error",
@@ -77,6 +86,7 @@ SYMBOLS = [
     "ufo_b200_write_bv", "ufo_b200_write_data_bv", "ufo_b200_write_compressed_bv", "ufo_b200_read_data_bv",
     "ufo_b200_export_nodes_bv", "ufo_b200_set_value_volume_bv", "ufo_b200_volume_intersects",
     "ufo_b200_geometry_frustum", "ufo_b200_geometry_plane", "ufo_b200_geometry_ray",
+    "ufo_b200_set_early_stopping", "ufo_b200_last_early_stats",
 ]
 
 # ufo_b200_volume: one shape of a bounding volume (type in BoundingVar order, members in v)
@@ -273,6 +283,8 @@ def load():
     lib.ufo_b200_geometry_ray.argtypes = [vp, vp, vp]
     lib.ufo_b200_clear.argtypes = [vp]
     lib.ufo_b200_set_shard.argtypes = [vp, u32, u32]
+    lib.ufo_b200_set_early_stopping.argtypes = [vp, i32]
+    lib.ufo_b200_last_early_stats.argtypes = [vp, C.POINTER(EarlyStats)]
     lib.ufo_b200_version.restype = C.c_char_p
     _lib = lib
     return lib
@@ -356,7 +368,7 @@ class Map:
             int(simple), int(early_stopping), int(discrete), int(async_)))
 
     def insert_frame(self, origin, xyz, frame_pose, rgb=None, max_range=-1.0, depth=0, simple=False,
-                     discrete=False, async_=False, dtype=np.float64):
+                     discrete=False, async_=False, dtype=np.float64, early_stopping=0):
         """insertPointCloud(sensor_origin, cloud, frame_origin, ...): the cloud is moved into the
         map frame on the device.  frame_pose = (tx, ty, tz, qw, qx, qy, qz)."""
         buf, layout = pack_points(xyz, rgb, dtype)
@@ -366,11 +378,11 @@ class Map:
         self._keep = (buf, o, f)
         self._check(self.lib.ufo_b200_insert_pointcloud_frame(
             self.h, o.ctypes.data, buf.ctypes.data, len(buf), layout, f.ctypes.data,
-            float(max_range), int(depth), int(simple), 0, int(discrete), int(async_)))
+            float(max_range), int(depth), int(simple), int(early_stopping), int(discrete), int(async_)))
 
     def insert_pointcloud2(self, origin, data, point_step, off_xyz=(0, 4, 8), off_rgb=None,
                            frame_pose=None, max_range=-1.0, depth=0, simple=False, discrete=False,
-                           async_=False):
+                           async_=False, early_stopping=0):
         """Insert a raw sensor_msgs/PointCloud2 data buffer (numpy uint8 array); NaN points are
         skipped on the device like rosToUfo does."""
         buf = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
@@ -383,16 +395,16 @@ class Map:
         self._keep = (buf, o, f, c)
         self._check(self.lib.ufo_b200_insert_pointcloud2(
             self.h, o.ctypes.data, C.byref(c), None if f is None else f.ctypes.data, float(max_range),
-            int(depth), int(simple), 0, int(discrete), int(async_)))
+            int(depth), int(simple), int(early_stopping), int(discrete), int(async_)))
 
     def insert_packed(self, origin, buf_ptr, n, layout, max_range=-1.0, depth=0, simple=False,
-                      discrete=False, async_=False, on_device=False):
+                      discrete=False, async_=False, on_device=False, early_stopping=0):
         """Insert from an already packed buffer (host pointer, or device pointer when
         on_device=True)."""
         o = np.ascontiguousarray(origin, dtype=np.float64)
         f = self.lib.ufo_b200_insert_device if on_device else self.lib.ufo_b200_insert_pointcloud
         self._check(f(self.h, o.ctypes.data, buf_ptr, int(n), int(layout), float(max_range),
-                      int(depth), int(simple), 0, int(discrete), int(async_)))
+                      int(depth), int(simple), int(early_stopping), int(discrete), int(async_)))
 
     def wait(self):
         self._check(self.lib.ufo_b200_wait(self.h))
@@ -424,6 +436,19 @@ class Map:
         records pushed, mask reductions issued, words they found empty, dirty-bit reductions."""
         st = WalkStats()
         self._check(self.lib.ufo_b200_last_walk_stats(self.h, C.byref(st)))
+        return st.as_dict()
+
+    def set_early_stopping(self, exact):
+        """exact=True: inserts with early_stopping != 0 compute the reference's sequential result on
+        the device (extra work and memory); False: they are rejected with E_UNSUPPORTED (the
+        default)."""
+        self._check(self.lib.ufo_b200_set_early_stopping(self.h, int(exact)))
+
+    def early_stats(self):
+        """The last insert's early-stopping work: rounds, converged, visits, nodes, free_nodes,
+        table_bytes, id_bytes and, at profiling level >= 1, ms_walk / ms_rounds / ms_mark."""
+        st = EarlyStats()
+        self._check(self.lib.ufo_b200_last_early_stats(self.h, C.byref(st)))
         return st.as_dict()
 
     def set_sensor_model_field(self, index, probability):

@@ -41,7 +41,7 @@ struct Counters {
 	uint32_t n_blocks;   // blocks that ever received an update (statistics only)
 	uint32_t n_bricks;   // next free brick slot
 	uint32_t n_upper;    // next free upper-node slot
-	uint32_t overflow;   // bit1 bricks/brick hash, bit2 upper nodes, bit3 ray-record buffer, bit4 ray bound violated (bug), bit5 alias arrays needed
+	uint32_t overflow;   // bit1 bricks/brick hash, bit2 upper nodes, bit3 ray-record buffer, bit4 ray bound violated (bug), bit5 alias arrays needed, bit8 early-stopping buffers
 	uint32_t n_touched;    // bricks stamped by this scan = length of DeviceMap::touched
 	uint32_t item_cursor;  // next work unit of the fused walk (k_walk_mark)
 	uint32_t max_span;     // longest ray of the scan in dominant-axis steps (sets the shell thickness)
@@ -65,6 +65,11 @@ struct Counters {
 	// dense fused walk, profiling level 2 only (k_walk_mark<COUNT = true>): block records pushed,
 	// global mask reductions issued, of those the ones that found the word empty, dirty-bit reductions
 	unsigned long long walk_records, walk_mask_reds, walk_words, walk_dirty_reds;
+	// early stopping (ufo_early.cuh): visits and distinct nodes of the walks, nodes in the free set,
+	// rounds run, 1 when the rounds reached their fixed point; the lowest ray whose prefix changed
+	// (two slots, alternating by round)
+	unsigned long long e_visits, e_nodes, e_free;
+	uint32_t e_rounds, e_converged, e_low[2];
 	// k_update statistics spread over slots: [slot][0 voxels, 1 hit voxels, 2 octets, 3 blocks,
 	// 4 first-touched blocks, 5 bricks, 6 depth-3 nodes, 7 touched 128 B leaf lines]
 	unsigned long long stat[64][8];

@@ -9,6 +9,7 @@
 // out-of-tree keys and the fixed-step walk use k_rays -> k_scatter instead of the fused walk,
 // which mirrors insertPointCloud + insertPointCloudHelper
 // (/root/reference/ufomap/include/ufo/map/occupancy_map_base.h:270-327, :1345-1373).
+// early_stopping on a map that opted in replaces the walk by E1-E3 (ufo_early.cuh).
 // There is no CPU fallback anywhere in this file.
 
 #include <cuda_runtime.h>
@@ -32,8 +33,10 @@
 #include "ufo_route.cuh"
 #include "ufo_import.cuh"
 #include "ufo_write.cuh"
+#include "ufo_early.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 using namespace ufo_b200;
 
@@ -102,6 +105,7 @@ struct PendingScan {
 	bool dense = false;   // marks go to the dense scan volume
 	VolumeArgs vol{};
 	float set_value = 0.0f;
+	uint32_t early = 0;  // early_stopping of a scan on a map that opted in (ufo_early.cuh); 0: off
 	uint32_t regrows = 0;
 	// write batch (ufo_write.cuh): ordered node updates or rays instead of a scan
 	bool write = false;
@@ -153,6 +157,22 @@ struct ufo_b200_map {
 	void* d_w_tmp = nullptr;
 	size_t w_tmp_cap = 0;
 	bool write_pass = false;  // the last pass was a write batch (its stats carry ms_update)
+	// early stopping (ufo_early.cuh), allocated on the first such scan: node table, per-ray visit
+	// counts / offsets / prefix lengths, visit ids, scan scratch
+	int early_exact = 0;  // ufo_b200_set_early_stopping: early_stopping != 0 is computed, not rejected
+	bool early_pass = false;  // the last pass was such a scan
+	unsigned long long* d_e_keys = nullptr;
+	uint32_t* d_e_first = nullptr;
+	size_t e_tab_cap = 0;
+	unsigned long long *d_e_cnt = nullptr, *d_e_off = nullptr;
+	uint32_t *d_e_plen = nullptr, *d_e_pnext = nullptr;
+	size_t e_ray_cap = 0;
+	uint32_t* d_e_ids = nullptr;
+	unsigned long long e_id_cap = 0;
+	void* d_e_tmp = nullptr;
+	size_t e_tmp_cap = 0;
+	int early_blocks_per_sm = 1;
+	ufo_b200_early_stats early_stats{};
 	// bookkeeping
 	uint32_t n_blocks = 0, n_bricks = 0, n_upper = 0;  // host view after the last completed scan
 	size_t device_bytes = 0;
@@ -293,7 +313,8 @@ void free_pools(Map* m)
 	                m->d_list[1], m->d_points[0], m->d_points[1], m->d_ray_end, m->d_hit_tab, m->d_tab_keys, m->d_tab_min,
 	                m->d_seg, m->d_seg_base, m->d_seg_count, m->d_order, m->d_nodes, m->d_items, m->d_vmask, m->d_rc,
 	                m->d_w_in, m->d_w_keys[0], m->d_w_keys[1], m->d_w_idx[0], m->d_w_idx[1], m->d_w_recs, m->d_w_seg,
-	                m->d_w_tmp, m->d_route_tab_keys, m->d_route_tab_min};
+	                m->d_w_tmp, m->d_route_tab_keys, m->d_route_tab_min, m->d_e_keys, m->d_e_first, m->d_e_cnt, m->d_e_off,
+	                m->d_e_plen, m->d_e_pnext, m->d_e_ids, m->d_e_tmp};
 	for (void* p : ptrs)
 		if (p) cudaFree(p);
 }
@@ -470,6 +491,22 @@ void finish_stats(Map* m)
 	st.rays = c.n_rays;
 	st.visits = c.visits;
 	m->walk_stats = ufo_b200_walk_stats{c.walk_records, c.walk_mask_reds, c.walk_words, c.walk_dirty_reds};
+	m->early_stats = ufo_b200_early_stats{};
+	if (m->early_pass) {
+		ufo_b200_early_stats& es = m->early_stats;
+		es.rounds = c.e_rounds;
+		es.converged = c.e_converged;
+		es.visits = c.e_visits;
+		es.nodes = c.e_nodes;
+		es.free_nodes = c.e_free;
+		es.table_bytes = m->e_tab_cap * (sizeof(unsigned long long) + sizeof(uint32_t));
+		es.id_bytes = m->e_id_cap * sizeof(uint32_t) + m->e_ray_cap * (2 * sizeof(unsigned long long) + 2 * sizeof(uint32_t));
+		if (m->ev_valid && m->profiling) {
+			cudaEventElapsedTime(&es.ms_walk, m->ev[2], m->ev[1]);
+			cudaEventElapsedTime(&es.ms_rounds, m->ev[1], m->ev[4]);
+			cudaEventElapsedTime(&es.ms_mark, m->ev[4], m->ev[3]);
+		}
+	}
 	st.touched_voxels = sum[0];
 	st.hit_voxels = sum[1];
 	st.touched_octets = sum[2];
@@ -644,7 +681,7 @@ void launch_rays_fused(Map* m, const ScanArgs& a)
 
 bool use_fused(const Map* m, const PendingScan& p)
 {
-	return !p.has_vol && !p.simple && p.a.depth <= 2 && !m->M.alias_miss && !m->force_records;
+	return !p.has_vol && !p.simple && !p.early && p.a.depth <= 2 && !m->M.alias_miss && !m->force_records;
 }
 
 // Dense scan volume: bricks per axis a scan of this range needs around the sensor (0: no volume)
@@ -743,6 +780,103 @@ void ensure_dev(Map* m, T*& p, size_t& cap_bytes, size_t bytes)
 	m->device_bytes += nb;
 }
 
+// Early-stopping buffers (ufo_early.cuh) for n rays and `visits` walk visits; called with the stream
+// idle.  The node table stays below 80 % load (distinct nodes <= visits, plus one end node per ray of
+// a discrete scan) and every scan leaves it empty (E3 clears the slots it reads), so it is only
+// cleared when it is allocated.
+void ensure_early(Map* m, size_t n, unsigned long long visits)
+{
+	size_t& tot = m->device_bytes;
+	cudaStream_t s = m->stream;
+	if (n + 1 > m->e_ray_cap) {
+		for (void* q : {(void*)m->d_e_cnt, (void*)m->d_e_off, (void*)m->d_e_plen, (void*)m->d_e_pnext})
+			if (q) CK(cudaFree(q));
+		tot -= m->e_ray_cap * (2 * sizeof(unsigned long long) + 2 * sizeof(uint32_t));
+		const size_t cap = std::max<size_t>(n + 1, 1024);
+		dev_alloc(m->d_e_cnt, cap, 0, s, tot);
+		dev_alloc(m->d_e_off, cap, 0, s, tot);
+		dev_alloc(m->d_e_plen, cap, 0, s, tot);
+		dev_alloc(m->d_e_pnext, cap, 0, s, tot);
+		m->e_ray_cap = cap;
+	}
+	if (visits > m->e_id_cap) {
+		if (m->d_e_ids) {
+			CK(cudaFree(m->d_e_ids));
+			tot -= m->e_id_cap * sizeof(uint32_t);
+		}
+		m->d_e_ids = nullptr;
+		m->e_id_cap = visits + visits / 8;
+		CK(cudaMalloc(reinterpret_cast<void**>(&m->d_e_ids), m->e_id_cap * sizeof(uint32_t)));  // written before read
+		tot += m->e_id_cap * sizeof(uint32_t);
+	}
+	const unsigned long long need = std::max<unsigned long long>(visits + visits / 4 + n + 1, 2ull * (n + 1));
+	if (need > m->e_tab_cap) {
+		if (need > (1ull << 31)) throw std::bad_alloc();
+		if (m->d_e_keys) {
+			CK(cudaFree(m->d_e_keys));
+			CK(cudaFree(m->d_e_first));
+			tot -= m->e_tab_cap * (sizeof(unsigned long long) + sizeof(uint32_t));
+		}
+		const size_t cap = next_pow2(need);
+		dev_alloc(m->d_e_keys, cap, 0xff, s, tot);
+		dev_alloc(m->d_e_first, cap, 0xff, s, tot);
+		m->e_tab_cap = cap;
+	}
+	size_t tmp = 0;
+	CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, m->d_e_cnt, m->d_e_off, (int)(n + 1), s));
+	ensure_dev(m, m->d_e_tmp, m->e_tmp_cap, tmp);
+}
+
+// E1-E3 (ufo_early.cuh): the scan's free set under early stopping, marked like the record path
+// marks it.  The rounds run in one cooperative kernel, so nothing here waits for the device.
+void launch_early(Map* m, const PendingScan& p)
+{
+	const ScanArgs& a = p.a;
+	cudaStream_t s = m->stream;
+	EarlyArgs e{};
+	e.stop = p.early;
+	e.simple = p.simple ? 1 : 0;
+	e.keys = m->d_e_keys;
+	e.first = m->d_e_first;
+	e.tab_mask = (uint32_t)(m->e_tab_cap - 1);
+	e.cnt = m->d_e_cnt;
+	e.off = m->d_e_off;
+	e.ids = m->d_e_ids;
+	e.id_cap = m->e_id_cap;
+	e.plen = m->d_e_plen;
+	e.pnext = m->d_e_pnext;
+	uint32_t n = a.n;
+	if (a.discrete) {
+		k_early_rank<<<(n + kEarlyThreads - 1) / kEarlyThreads, kEarlyThreads, 0, s>>>(m->M, a, e);
+		k_early_place<<<(n + kEarlyThreads - 1) / kEarlyThreads, kEarlyThreads, 0, s>>>(m->M, a, e);
+		m->launches += 2;
+	}
+	k_early_count<<<(n + kEarlyThreads) / kEarlyThreads, kEarlyThreads, 0, s>>>(m->M, a, e);  // n + 1 threads
+	size_t tmp = m->e_tmp_cap;
+	CK(cub::DeviceScan::ExclusiveSum(m->d_e_tmp, tmp, m->d_e_cnt, m->d_e_off, (int)(n + 1), s));
+	k_early_check<<<1, 1, 0, s>>>(m->M, e, n);
+	k_early_fill<<<(n + kEarlyThreads - 1) / kEarlyThreads, kEarlyThreads, 0, s>>>(m->M, a, e);
+	if (m->profiling) CK(cudaEventRecord(m->ev[1], s));
+	{
+		DeviceMap M = m->M;
+		void* args[] = {&M, &e, &n};
+		CK(cudaLaunchCooperativeKernel((const void*)k_early_rounds, dim3((unsigned)(m->sm_count * m->early_blocks_per_sm)),
+		                               dim3(kEarlyThreads), args, 0, s));
+	}
+	if (m->profiling) CK(cudaEventRecord(m->ev[4], s));
+	const uint32_t grid = (uint32_t)m->sm_count * 8;
+	if (a.depth == 0) k_early_mark<0><<<grid, kEarlyThreads, 0, s>>>(m->M, a, e);
+	else if (a.depth == 1) k_early_mark<1><<<grid, kEarlyThreads, 0, s>>>(m->M, a, e);
+	else if (a.depth == 2) k_early_mark<2><<<grid, kEarlyThreads, 0, s>>>(m->M, a, e);
+	else if (a.depth <= 4) k_early_mark<3><<<grid, kEarlyThreads, 0, s>>>(m->M, a, e);
+	else k_early_mark<5><<<grid, kEarlyThreads, 0, s>>>(m->M, a, e);
+	m->launches += 5;  // the scan's own launches not counted
+	if (a.depth >= 5) {
+		k_expand_nodes<<<m->sm_count * 8, 256, 0, s>>>(m->M, a);
+		++m->launches;
+	}
+}
+
 // Enqueues one write batch (ufo_write.cuh): expand -> sort -> segments -> apply -> aggregates.
 // Called with the stream idle.  If a pool overflows while expanding, every later kernel backs off
 // and finalize_scan() grows the pool and enqueues the whole batch again: no leaf was written, and
@@ -819,7 +953,7 @@ void bind_scan_buffers(Map* m, PendingScan& p, bool fused)
 		a.item_stride = m->item_cap;
 		a.vmask = m->d_vmask;
 		a.rc = m->d_rc;
-	} else if (!p.simple && !p.has_vol) {
+	} else if (!p.simple && !p.has_vol && !p.early) {
 		a.seg = m->d_seg;
 		a.seg_cap = m->seg_cap;
 		a.seg_base = m->d_seg_base;
@@ -841,6 +975,7 @@ void enqueue_scan(Map* m, PendingScan& p)
 		return;
 	}
 	m->write_pass = false;
+	m->early_pass = p.early != 0;
 	DeviceMap& M = m->M;
 	cudaStream_t s = m->stream;
 	ScanArgs& a = p.a;
@@ -874,6 +1009,7 @@ void enqueue_scan(Map* m, PendingScan& p)
 		}
 		if (m->profiling) CK(cudaEventRecord(m->ev[2], s));
 		if (fused) launch_rays_fused(m, a);
+		else if (p.early) launch_early(m, p);
 		else launch_rays_records(m, a, p.simple);
 	} else if (m->profiling) {
 		CK(cudaEventRecord(m->ev[2], s));
@@ -988,7 +1124,8 @@ void finalize_scan(Map* m)
 					}
 				}
 				const bool fused = use_fused(m, p);
-				if (!fused && !p.simple && !p.has_vol) {
+				if (ov & 256u) ensure_early(m, p.a.n, m->h_ctr->e_visits);  // the walks need more ids / table slots
+				if (!fused && !p.simple && !p.has_vol && !p.early) {
 					ensure_scan_buffers(m, p.a.n, false, true, false);
 					unsigned long long want = std::max<unsigned long long>(m->h_ctr->seg_total + m->h_ctr->seg_total / 4 + 1024,
 					                                                        std::max<unsigned long long>(p.a.n, 1024) * 48ull);
@@ -1100,8 +1237,9 @@ int do_insert(Map* m, const double origin[3], const void* points, bool on_device
 			return UFO_B200_E_INVALID;
 		}
 	}
-	if (early_stopping != 0) {
-		m->set_error("early_stopping is order-dependent in the reference (occupancy_map_base.h:1289-1298) and is not supported");
+	if (early_stopping != 0 && !m->early_exact) {
+		m->set_error("early_stopping is order-dependent in the reference (occupancy_map_base.h:1289-1298) and is not supported "
+		             "unless the map opted in with ufo_b200_set_early_stopping(map, 1)");
 		return UFO_B200_E_UNSUPPORTED;
 	}
 	if (depth > 6) {
@@ -1149,6 +1287,7 @@ int do_insert(Map* m, const double origin[3], const void* points, bool on_device
 	p.has_vol = vol != nullptr;
 	if (vol) p.vol = *vol;
 	p.set_value = set_value;
+	p.early = vol ? 0u : early_stopping;
 
 	ScanArgs& a = p.a;
 	a.origin = {origin[0], origin[1], origin[2]};
@@ -1175,8 +1314,10 @@ int do_insert(Map* m, const double origin[3], const void* points, bool on_device
 		                frame_pose[0], frame_pose[1], frame_pose[2]};
 	}
 	const bool fused = use_fused(m, p);
-	const bool records = !fused && !p.simple && !p.has_vol;
+	const bool records = !fused && !p.simple && !p.has_vol && !p.early;
 	ensure_scan_buffers(m, n, p.need_table, records, fused);
+	// first guess for the walks: 64 visits per ray; grown to the exact count on demand
+	if (p.early) ensure_early(m, n, m->e_id_cap ? 0ull : std::max<size_t>(n, 1024) * 64ull);
 	if (fused) {
 		const uint32_t db = volume_bricks(m, p);
 		p.dense = db != 0;
@@ -1523,6 +1664,9 @@ int ufo_b200_create(const ufo_b200_params* p, ufo_b200_map** out)
 		if (m->ray_blocks_per_sm < 1) m->ray_blocks_per_sm = 1;
 		CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m->walk_blocks_per_sm, k_walk_mark<0, false, false, true>, kWalkThreads, 0));
 		if (m->walk_blocks_per_sm < 1) m->walk_blocks_per_sm = 1;
+		// the rounds kernel is cooperative: every CTA of its grid must be resident
+		CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m->early_blocks_per_sm, k_early_rounds, kEarlyThreads, 0));
+		if (m->early_blocks_per_sm < 1) m->early_blocks_per_sm = 1;
 		{
 			const char* e = getenv("UFO_B200_MARK");
 			m->force_records = e && !strcmp(e, "records");
@@ -2623,6 +2767,27 @@ int ufo_b200_completed_scan_stats(ufo_b200_map* m, ufo_b200_scan_stats* out)
 {
 	if (!m || !out) return UFO_B200_E_INVALID;
 	*out = m->done_stats;
+	return UFO_B200_OK;
+}
+
+int ufo_b200_last_early_stats(ufo_b200_map* m, ufo_b200_early_stats* out)
+{
+	if (!m || !out) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() {
+		sync_map(m);
+		*out = m->early_stats;
+		return (int)UFO_B200_OK;
+	});
+}
+
+int ufo_b200_set_early_stopping(ufo_b200_map* m, int exact)
+{
+	if (!m) return UFO_B200_E_INVALID;
+	if (exact != 0 && exact != 1) {
+		m->set_error("ufo_b200_set_early_stopping: exact must be 0 or 1, got %d", exact);
+		return UFO_B200_E_INVALID;
+	}
+	m->early_exact = exact;  // read when a scan is enqueued: the scan in flight keeps its own setting
 	return UFO_B200_OK;
 }
 
