@@ -1,6 +1,7 @@
 """Shared comparison helpers for the parity tests."""
 import numpy as np
 
+from color_lib import inner_colors
 from oracle_lib import aggregate_level
 
 
@@ -14,27 +15,39 @@ def assert_value_fields_equal(a, b, color_tol=0, what=""):
     assert len(bad) == 0, "%s: %d log-odds differ, first code %x: %r vs %r" % (
         what, len(bad), int(ca[bad[0]]), va[bad[0]], vb[bad[0]])
     if color_tol == 0:
-        assert np.array_equal(ga, gb), "%s: colours differ" % what
+        bad = np.nonzero((ga != gb).any(axis=1))[0]
+        assert len(bad) == 0, "%s: %d colours differ, first code %x: %r vs %r" % (
+            what, len(bad), int(ca[bad[0]]), tuple(int(x) for x in ga[bad[0]]), tuple(int(x) for x in gb[bad[0]]))
     else:
         d = np.abs(ga.astype(np.int32) - gb.astype(np.int32))
         assert d.max(initial=0) <= color_tol, "%s: colour error %d" % (what, d.max())
 
 
 def check_inner_against_field(gpu_map, field, model, levels=(1, 2, 3, 4, 5, 6, 9), max_nodes=200000):
-    """Inner aggregates of the CUDA map == pure function of the value field."""
+    """Inner aggregates of the CUDA map == pure function of the value field (max, flags and, on
+    colour maps, the restated inner colour)."""
     codes, occ, rgb = field
+    levels = [lvl for lvl in levels if lvl <= gpu_map.depth_levels]
+    colors = inner_colors(codes, rgb, max(levels)) if gpu_map.color and levels else None
     for lvl in levels:
-        if lvl > gpu_map.depth_levels:
-            continue
         parents, mx, free, unk = aggregate_level(codes, occ, rgb, lvl, model)
+        col = None
+        if colors is not None:
+            assert np.array_equal(colors[lvl][0], parents)
+            col = colors[lvl][1]
         if len(parents) > max_nodes:
             sel = np.linspace(0, len(parents) - 1, max_nodes).astype(np.int64)
             parents, mx, free, unk = parents[sel], mx[sel], free[sel], unk[sel]
+            col = None if col is None else col[sel]
         q = parents << np.uint64(3 * lvl)
-        o, f, _ = gpu_map.query(q, lvl)
+        o, f, g = gpu_map.query(q, lvl)
         assert np.array_equal(o.view(np.uint32), mx.view(np.uint32)), "level %d max mismatch" % lvl
         assert np.array_equal((f & 1).astype(bool), free), "level %d contains_free mismatch" % lvl
         assert np.array_equal(((f >> 1) & 1).astype(bool), unk), "level %d contains_unknown mismatch" % lvl
+        if col is not None:
+            bad = np.nonzero((g != col).any(axis=1))[0]
+            assert len(bad) == 0, "level %d: %d inner colours differ, first node %x: %r vs %r" % (
+                lvl, len(bad), int(q[bad[0]]), tuple(g[bad[0]]), tuple(col[bad[0]]))
 
 
 def sorted_field_large(gpu_map):

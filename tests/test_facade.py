@@ -6,24 +6,25 @@ import subprocess
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "tests", "cpp", "facade_smoke")
 
 
-def _build():
+@pytest.fixture(scope="module")
+def exe(tmp_path_factory):
+    """The facade program, built once per module outside the source tree (which may be read-only)."""
+    path = str(tmp_path_factory.mktemp("facade") / "facade_smoke")
     lib_dir = os.path.join(ROOT, "ufomap_b200")
     subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "facade_smoke.cpp"), "-o", EXE,
+                           os.path.join(ROOT, "tests", "cpp", "facade_smoke.cpp"), "-o", path,
                            "-L" + lib_dir, "-lufomap_b200", "-Wl,-rpath," + lib_dir])
+    return path
 
 
-def test_facade_compiles_and_validates_arguments():
-    _build()
-    out = subprocess.run([EXE, "--no-device"], capture_output=True, text=True)
+def test_facade_compiles_and_validates_arguments(exe):
+    out = subprocess.run([exe, "--no-device"], capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr
 
 
 @pytest.mark.gpu
-def test_facade_on_device():
-    _build()
-    out = subprocess.run([EXE], capture_output=True, text=True)
+def test_facade_on_device(exe):
+    out = subprocess.run([exe], capture_output=True, text=True)
     assert out.returncode == 0 and "facade ok" in out.stdout, (out.returncode, out.stdout, out.stderr)

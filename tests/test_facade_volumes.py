@@ -11,23 +11,25 @@ import pytest
 import volumes_lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "tests", "cpp", "facade_volumes")
 
 
-def _build():
+@pytest.fixture(scope="module")
+def exe(tmp_path_factory):
+    """The facade program, built once per module outside the source tree (which may be read-only)."""
+    path = str(tmp_path_factory.mktemp("facade") / "facade_volumes")
     lib_dir = os.path.join(ROOT, "ufomap_b200")
     subprocess.check_call(["g++", "-std=c++17", "-O1", "-Wall", "-I" + os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "cpp", "facade_volumes.cpp"), "-o", EXE,
+                           os.path.join(ROOT, "tests", "cpp", "facade_volumes.cpp"), "-o", path,
                            "-L" + lib_dir, "-lufomap_b200", "-Wl,-rpath," + lib_dir])
+    return path
 
 
 def _doubles(line):
     return np.array([struct.unpack("<d", struct.pack("<Q", int(h, 16)))[0] for h in line.split()[1:]])
 
 
-def test_facade_volumes_compile_and_reject():
-    _build()
-    out = subprocess.run([EXE, "--no-device"], capture_output=True, text=True)
+def test_facade_volumes_compile_and_reject(exe):
+    out = subprocess.run([exe, "--no-device"], capture_output=True, text=True)
     assert out.returncode == 0 and "facade volumes ok (no device)" in out.stdout, (out.returncode, out.stdout, out.stderr)
     if not volumes_lib.have_ref():
         pytest.skip("reference volume checker not built: constructors not compared")
@@ -43,7 +45,6 @@ def test_facade_volumes_compile_and_reject():
 
 
 @pytest.mark.gpu
-def test_facade_volumes_on_device(tmp_path):
-    _build()
-    out = subprocess.run([EXE, str(tmp_path / "saved.ufo")], capture_output=True, text=True)
+def test_facade_volumes_on_device(exe, tmp_path):
+    out = subprocess.run([exe, str(tmp_path / "saved.ufo")], capture_output=True, text=True)
     assert out.returncode == 0 and "facade volumes ok" in out.stdout, (out.returncode, out.stdout, out.stderr)

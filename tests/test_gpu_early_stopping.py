@@ -33,7 +33,7 @@ def _run(map_kw, inserts, color=False, oracle=True, levels=(1, 2, 3, 4, 5, 6, 9)
             c.insert(**ins)
     field = gpu.value_field()
     for c in cpus:
-        assert_value_fields_equal(field, c.value_field(), color_tol=1 if color else 0, what=type(c).__name__)
+        assert_value_fields_equal(field, c.value_field(), color_tol=0, what=type(c).__name__)
     check_inner_against_field(gpu, cpus[0].value_field(), cpus[0].sensor_model(), levels=levels)
     st = gpu.early_stats()
     gpu.close()

@@ -1,5 +1,5 @@
 """GPU parity: the CUDA path (through the C ABI) against the CPU oracle on the same
-seeded inputs.  Log-odds are compared bit-for-bit, codes/keys exactly, colours +-1.
+seeded inputs.  Log-odds and colours are compared bit-for-bit, codes/keys exactly.
 
 The oracle is oracle/libufo_oracle.so (plain-C restatement, pinned to the real
 reference by tests/test_oracle_vs_reference.py and tests/golden/); when the
@@ -17,7 +17,7 @@ from ufomap_b200.capi import Map, UfoError, E_UNSUPPORTED
 pytestmark = pytest.mark.gpu
 
 
-def _run_case(map_kw, inserts, color=False, color_tol=1, with_ref=True, levels=(1, 2, 3, 4, 5, 6, 9, 16)):
+def _run_case(map_kw, inserts, color=False, color_tol=0, with_ref=True, levels=(1, 2, 3, 4, 5, 6, 9, 16)):
     gpu = Map(color=color, initial_blocks=1 << 14, **map_kw)
     cpus = [OracleMap(color=color, **map_kw)]
     if with_ref and have_ref():
@@ -28,7 +28,7 @@ def _run_case(map_kw, inserts, color=False, color_tol=1, with_ref=True, levels=(
             c.insert(**ins)
     field = gpu.value_field()
     for c in cpus:
-        assert_value_fields_equal(field, c.value_field(), color_tol=color_tol if color else 0,
+        assert_value_fields_equal(field, c.value_field(), color_tol=color_tol,
                                   what=type(c).__name__)
     check_inner_against_field(gpu, cpus[0].value_field(), cpus[0].sensor_model(), levels=levels)
     mn, mx = gpu.change_bbox()
@@ -313,7 +313,7 @@ def test_frame_insert(color, discrete, dtype):
         rgb = c if color else None
         gpu.insert_frame(pose[:3], local, pose, rgb=rgb, max_range=4.0, discrete=discrete, dtype=dtype)
         cpu.insert(origin=pose[:3], xyz=world, rgb=rgb, max_range=4.0, discrete=discrete)
-    assert_value_fields_equal(gpu.value_field(), cpu.value_field(), color_tol=1 if color else 0, what="frame")
+    assert_value_fields_equal(gpu.value_field(), cpu.value_field(), color_tol=0, what="frame")
     mn, mx = gpu.change_bbox()
     rmn, rmx = cpu.change_bbox()
     assert np.array_equal(mn, rmn) and np.array_equal(mx, rmx)
@@ -356,7 +356,7 @@ def test_pointcloud2_ingestion(color, discrete):
         cpu.insert(origin=pose[:3], xyz=world, rgb=c[keep] if color else None, max_range=4.0,
                    discrete=discrete)
         assert gpu.stats()["points"] == n
-    assert_value_fields_equal(gpu.value_field(), cpu.value_field(), color_tol=1 if color else 0, what="pc2")
+    assert_value_fields_equal(gpu.value_field(), cpu.value_field(), color_tol=0, what="pc2")
     mn, mx = gpu.change_bbox()
     rmn, rmx = cpu.change_bbox()
     assert np.array_equal(mn, rmn) and np.array_equal(mx, rmx)
@@ -394,7 +394,7 @@ def test_set_value_volume(color):
                 m.set_value_volume((lo, hi), val, md)
             field = gpu.value_field()
             for m in cpus:
-                assert_value_fields_equal(field, m.value_field(), color_tol=1 if color else 0,
+                assert_value_fields_equal(field, m.value_field(), color_tol=0,
                                           what="%s after volume %d (depth %d)" % (type(m).__name__, i, md))
     check_inner_against_field(gpu, cpus[0].value_field(), cpus[0].sensor_model(), levels=(1, 2, 3, 4, 5, 6, 9, 16))
     # outside the map / unsupported depth

@@ -1,6 +1,6 @@
 """GPU parity at the BASELINE configs' REAL sizes against the compiled, unmodified reference
 (oracle/_ref/libufo_ref.so; falls back to the C restatement when the prebuilt harness did not
-travel).  The whole value field is compared bit for bit (log-odds) / +-1 (colour), inner
+travel).  The whole value field is compared bit for bit (log-odds and colour), inner
 aggregates on random samples of every level, and the change box.
 
 The reference needs minutes per case on one core (BASELINE.md section 4: ~1 k points/s), so
@@ -118,13 +118,13 @@ def test_config4_two_full_scans_100m(cpu_results):
 
 
 def test_config3_reduced_2mm_color(cpu_results):
-    _compare("c3r", cpu_results, color_tol=1)
+    _compare("c3r", cpu_results)
 
 
 @pytest.mark.parametrize("name", ["c3d4", "c3d6"])
 def test_config3_full_size_coarse_insert_color(cpu_results, name):
     """Full-size #3 at insert depth 4 / 6: number of non-default voxels, and occupancy (bit-exact) +
-    colour (+-1) of 2 M voxels sampled along the rays (free space) and at the end points (hits)."""
+    colour (both bit-exact) of 2 M voxels sampled along the rays (free space) and at the end points (hits)."""
     cases, futures = cpu_results
     if not have_ref():
         pytest.skip("needs the compiled reference (batched node lookup)")
@@ -148,7 +148,7 @@ def test_config3_full_size_coarse_insert_color(cpu_results, name):
     ref = futures[name].result()
     rocc, rrgb, _, _ = ref["map"].node_batch(codes, 0)
     assert np.array_equal(occ.view(np.uint32), rocc.view(np.uint32))
-    assert np.abs(rgb.astype(np.int32) - rrgb.astype(np.int32)).max() <= 1
+    assert np.array_equal(rgb, rrgb)
     assert (occ > 0).sum() > 100000 and (occ < 0).sum() > 100000
     st = gpu.stats()
     print("%s: gpu %.3f ms/scan vs %.3f s/scan on the CPU" % (name, st["ms_total"], ref["secs"] / len(case["inserts"])))

@@ -204,7 +204,7 @@ def test_colour_sensors_merged_in_sensor_order():
     field = _union(maps)
     assert_value_fields_equal(field, single.value_field(), what="merged colour sensors vs single GPU")
     if ref is not None:
-        assert_value_fields_equal(field, ref.value_field(), color_tol=1, what="merged colour sensors vs reference")
+        assert_value_fields_equal(field, ref.value_field(), color_tol=0, what="merged colour sensors vs reference")
 
 
 @pytest.mark.parametrize("color", [False, True])

@@ -161,7 +161,7 @@ def test_set_value_volume_every_shape(color):
             gpu.set_value_volume_bv(shape, val, md)
             ref.set_value_volume_bv(shape, val, md)
             field = gpu.value_field()
-            assert_value_fields_equal(field, ref.value_field(), color_tol=1 if color else 0,
+            assert_value_fields_equal(field, ref.value_field(), color_tol=0,
                                       what="shape %d, scan %d, depth %d" % (kind, k, md))
             i += 1
     check_inner_against_field(gpu, ref.value_field(), ref.sensor_model(), levels=(1, 2, 3, 4, 5, 6, 9, 16))

@@ -150,7 +150,7 @@ def test_colour_map():
     for m in (gpu, cpu):
         m.update_nodes(codes, depths, ops, vals)
     field = gpu.value_field()
-    assert_value_fields_equal(field, cpu.value_field(), color_tol=1, what="OracleMap")
+    assert_value_fields_equal(field, cpu.value_field(), color_tol=0, what="OracleMap")
     check_inner_against_field(gpu, cpu.value_field(), cpu.sensor_model(), levels=LEVELS)
     keep = np.isin(field[0], before[0])
     assert np.array_equal(field[2][keep], before[2][np.isin(before[0], field[0])])

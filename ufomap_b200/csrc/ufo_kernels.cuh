@@ -19,6 +19,7 @@
 //   k_brick_agg    depth-3/4 aggregates per brick (updateNode :1179-1224) when alias marks exist
 //   k_split / k_walk_mark / k_gather* (ufo_walk.cuh): the fused marking path
 //   k_alias_*      marks of keys outside the tree (octree.h:321), launched only when present
+//   k_wrapped_colors  colour hits of keys outside the tree, in cloud order, on maps that met them
 //   k_upper_*  K4  aggregates of the dirty nodes of depth >= 5 (seed, levels 5-6, one-CTA tail)
 #pragma once
 
@@ -498,18 +499,14 @@ __global__ void __launch_bounds__(256) k_points(DeviceMap M, ScanArgs a)
 	}
 }
 
-// updateNodeColor (occupancy_map_color.cpp:142-171): blends `upd` into leaf li, weighted by the
-// leaf's occupancy before this scan's update
-__device__ __forceinline__ void blend_color(const DeviceMap& M, size_t li, uint32_t upd)
+// updateNodeColor (occupancy_map_color.cpp:142-171): the colour of a leaf of colour `cur` and
+// log-odds `occ` after a hit of colour `upd`
+__device__ __forceinline__ uint32_t blended_color(const DeviceMap& M, uint32_t cur, uint32_t upd, float occ)
 {
-	uint32_t cur = M.leaf_rgb[li];
-	if (cur == upd) return;
-	if (cur == 0) {
-		M.leaf_rgb[li] = upd;
-		return;
-	}
+	if (cur == upd) return cur;
+	if (cur == 0) return upd;
 	double prob = M.prob_hit;
-	double total = prob + to_prob(M.leaf[li]);
+	double total = prob + to_prob(occ);
 	prob = prob / total;
 	double inv = 1.0 - prob;
 	uint32_t out = 0;
@@ -518,7 +515,49 @@ __device__ __forceinline__ void blend_color(const DeviceMap& M, size_t li, uint3
 		double r = dop::sqrt(dop::add(dop::mul(dop::mul(cc, cc), inv), dop::mul(dop::mul(uu, uu), prob)));
 		out |= ((uint32_t)(int)r & 0xffu) << (8 * c);
 	}
-	M.leaf_rgb[li] = out;
+	return out;
+}
+
+// blends `upd` into leaf li, weighted by the leaf's occupancy before this scan's update
+__device__ __forceinline__ void blend_color(const DeviceMap& M, size_t li, uint32_t upd)
+{
+	uint32_t cur = M.leaf_rgb[li];
+	if (cur == upd) return;
+	M.leaf_rgb[li] = blended_color(M, cur, upd, M.leaf[li]);
+}
+
+// slot of `key` in the scan-local table, kNone when absent
+__device__ __forceinline__ uint32_t table_find(const ScanArgs& a, uint64_t key)
+{
+	for (uint32_t i = hash_u64(key) & a.tab_mask;; i = (i + 1) & a.tab_mask) {
+		const unsigned long long k = a.tab_keys[i];
+		if (k == key) return i;
+		if (k == kEmptyKey) return kNone;
+	}
+}
+
+// Out-of-tree hit keys: a point on a + face is inside the map (isInside is inclusive,
+// octree.h:1297-1304) and toKey gives 2^L there; a ray end clipped onto a - face can give -1
+// (2^21 - 1 in the 21-bit code).  The tree's code walk only reads L bits, so 2^L wraps onto
+// key 0 and -1 onto key 2^L - 1 of that axis.  The wrapped key of an in-tree key (itself if none):
+__device__ __forceinline__ uint32_t wrapped_alt(const DeviceMap& M, uint32_t c)
+{
+	if (M.g.key_mask == 0x1fffffu) return c;  // 21 levels: every 21-bit key is in the tree
+	return c == 0u ? M.g.key_mask + 1u : (c == M.g.key_mask ? 0x1fffffu : c);
+}
+
+// Visits the table slots of the hits of in-tree voxel v (with_self) and of every out-of-tree key
+// that wraps onto it (bit s of `sel` puts axis s at its wrapped key); f returns false to stop.
+template <class F>
+__device__ __forceinline__ void for_wrapped_hits(const DeviceMap& M, const ScanArgs& a, Key3 v, bool with_self, F f)
+{
+	const Key3 w = {wrapped_alt(M, v.x), wrapped_alt(M, v.y), wrapped_alt(M, v.z)};
+	for (uint32_t sel = with_self ? 0u : 1u; sel < 8u; ++sel) {
+		if (((sel & 1u) && w.x == v.x) || ((sel & 2u) && w.y == v.y) || ((sel & 4u) && w.z == v.z)) continue;
+		const Key3 c = {(sel & 1u) ? w.x : v.x, (sel & 2u) ? w.y : v.y, (sel & 4u) ? w.z : v.z};
+		const uint32_t ts = table_find(a, key_to_code(c));
+		if (ts != kNone && !f(sel, a.tab_min[ts])) return;
+	}
 }
 
 // K1b: colour maps.  The first point (lowest cloud index) of every hit voxel blends
@@ -532,19 +571,9 @@ __global__ void __launch_bounds__(256) k_hits(DeviceMap M, ScanArgs a)
 	if (t == kNone || a.tab_min[t] != i) return;
 	Key3 k = code_to_key(a.tab_keys[t]);
 	if ((k.x | k.y | k.z) & ~M.g.key_mask) {
-		// out-of-tree hit voxel: occupancy goes through the alias path; its colour is blended
-		// into the wrapped voxel below with the occupancy the voxel has at this point
+		// out-of-tree hit voxel: occupancy goes through the alias path, colour through
+		// k_wrapped_colors
 		mark_alias(M, k.x >> 2, k.y >> 2, k.z >> 2, 1ull << linear2(k.x, k.y, k.z), true);
-		k.x &= M.g.key_mask;
-		k.y &= M.g.key_mask;
-		k.z &= M.g.key_mask;
-		uint32_t tb = brick_find(M, pack_key(k.x >> 4, k.y >> 4, k.z >> 4));
-		if (tb == kNone) return;
-		const size_t tl = ((size_t)tb * 64 + morton2(k.x >> 2, k.y >> 2, k.z >> 2)) * 64 + morton2(k.x, k.y, k.z);
-		Vec3 tp;
-		uint32_t tu;
-		load_point(a, i, tp, tu);
-		if (M.leaf_rgb[tl] == 0) M.leaf_rgb[tl] = tu;
 		return;
 	}
 	if (M.shard_world > 1 && brick_owner(pack_key(k.x >> 4, k.y >> 4, k.z >> 4), M.shard_world) != M.shard_rank) return;
@@ -556,10 +585,68 @@ __global__ void __launch_bounds__(256) k_hits(DeviceMap M, ScanArgs a)
 	const unsigned long long hbit = 1ull << linear2(k.x, k.y, k.z);
 	unsigned long long old = atomicOr(&M.hit_mask[slot], hbit);
 	if (old & hbit) return;  // re-run after a pool regrow: colour already blended
+	if (wrapped_alt(M, k.x) != k.x || wrapped_alt(M, k.y) != k.y || wrapped_alt(M, k.z) != k.z) {
+		// a voxel on the map's boundary may also receive out-of-tree hits: k_wrapped_colors blends
+		// all of them in cloud order
+		bool wrapped = false;
+		for_wrapped_hits(M, a, k, false, [&](uint32_t, uint32_t) {
+			wrapped = true;
+			return false;
+		});
+		if (wrapped) return;
+	}
 	Vec3 p;
 	uint32_t upd;
 	load_point(a, i, p, upd);
 	blend_color(M, slot * 64 + v, upd);
+}
+
+// The colour hits of a voxel that out-of-tree keys wrap onto, applied like the reference does: one
+// at a time in cloud order, each blend with the occupancy the earlier hits of this scan left
+// (occupancy_map_color.h:269-287).  One thread per such voxel: the lowest-index out-of-tree winner.
+// Runs after marking and before any occupancy update of the scan, only in the scan's final run.
+__global__ void __launch_bounds__(256) k_wrapped_colors(DeviceMap M, ScanArgs a)
+{
+	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= a.n || (__ldg(&M.ctr->overflow) & ~4u)) return;
+	uint32_t t = a.hit_tab[i];
+	if (t == kNone || a.tab_min[t] != i) return;
+	Key3 k = code_to_key(a.tab_keys[t]);
+	if (!((k.x | k.y | k.z) & ~M.g.key_mask)) return;
+	k.x &= M.g.key_mask;
+	k.y &= M.g.key_mask;
+	k.z &= M.g.key_mask;
+	if (M.shard_world > 1 && brick_owner(pack_key(k.x >> 4, k.y >> 4, k.z >> 4), M.shard_world) != M.shard_rank) return;
+	uint32_t idx[8], n = 0;
+	bool lead = true;
+	for_wrapped_hits(M, a, k, true, [&](uint32_t sel, uint32_t j) {
+		if (sel && j < i) {
+			lead = false;
+			return false;
+		}
+		idx[n++] = j;
+		return true;
+	});
+	if (!lead) return;
+	const uint32_t tb = brick_find(M, pack_key(k.x >> 4, k.y >> 4, k.z >> 4));
+	if (tb == kNone) return;
+	for (uint32_t x = 1; x < n; ++x)
+		for (uint32_t y = x; y > 0 && idx[y - 1] > idx[y]; --y) {
+			const uint32_t s = idx[y];
+			idx[y] = idx[y - 1];
+			idx[y - 1] = s;
+		}
+	const size_t tl = ((size_t)tb * 64 + morton2(k.x >> 2, k.y >> 2, k.z >> 2)) * 64 + morton2(k.x, k.y, k.z);
+	float occ = M.leaf[tl];
+	uint32_t rgb = M.leaf_rgb[tl];
+	for (uint32_t x = 0; x < n; ++x) {
+		Vec3 p;
+		uint32_t upd;
+		load_point(a, idx[x], p, upd);
+		rgb = blended_color(M, rgb, upd, occ);
+		occ = apply_update(M, occ, M.hit);
+	}
+	M.leaf_rgb[tl] = rgb;
 }
 
 // ---------------------------------------------------------------------------
@@ -1077,6 +1164,18 @@ __global__ void __launch_bounds__(256) k_alias_refresh(DeviceMap M)
 		// every octet now holds real values; several sources refreshing one target write the same
 		M.agg2[tb] = {bmax, bfl};
 		M.meta[tb] = meta | 0xff0000u | (M.scan_id << 24);
+		if (M.color) {
+			// the wrapped leaves' colours changed too (k_wrapped_colors): depth 1 and 2 colours
+			const volatile uint32_t* lrgb = M.leaf_rgb + tb * 64;
+			uint32_t oc[8];
+			for (int o = 0; o < 8; ++o) {
+				uint32_t c[8];
+				for (int j = 0; j < 8; ++j) c[j] = lrgb[8 * o + j];
+				oc[o] = rms_rgb(c, 8);
+				M.sum1_rgb[tb * 8 + o] = oc[o];
+			}
+			M.rgb2[tb] = rms_rgb(oc, 8);
+		}
 	}
 }
 

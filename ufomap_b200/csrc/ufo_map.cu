@@ -1011,6 +1011,11 @@ void enqueue_scan(Map* m, PendingScan& p)
 		if (fused) launch_rays_fused(m, a);
 		else if (p.early) launch_early(m, p);
 		else launch_rays_records(m, a, p.simple);
+		if (p.use_color && M.alias_miss) {
+			// only maps that have met out-of-tree keys; after marking, before the occupancy update
+			k_wrapped_colors<<<grid, 256, 0, s>>>(M, a);
+			++m->launches;
+		}
 	} else if (m->profiling) {
 		CK(cudaEventRecord(m->ev[2], s));
 	}
