@@ -318,6 +318,24 @@ int ufo_b200_read_data_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_b
 int ufo_b200_export_nodes_bv(ufo_b200_map* m, uint32_t depth, int occupied, int free_space, int unknown,
                              const ufo_b200_volume* bv, size_t n_bv, uint64_t* codes, float* logodds, uint8_t* rgb,
                              size_t cap, size_t* n);
+/* Iteration: beginLeaves (leaves_only != 0) / beginTree (occupancy_map_base.h:93-163) with the
+ * filters occupied / free_space / unknown / contains and min_depth, over the bounding volume bv[n_bv]
+ * (n_bv == 0: the whole map).  The nodes come in the reference iterator's order (pre-order, children
+ * 0..7) over the canonical tree of the file writer (a node whose eight children are leaves with equal
+ * payload is a leaf; untouched space is a default leaf):
+ *   codes[i]   the node's Code as the iterator builds it (Code::getChild from the root: the bits
+ *              below 3 * depth are zero)
+ *   depths[i]  its depth, 0..depth_levels
+ *   logodds[i] a leaf's value, an inner node's aggregate (max over the subtree) -- ufo_b200_query's
+ *   flags[i]   bit0 contains_free, bit1 contains_unknown (as ufo_b200_query), bit2 isLeaf
+ *   rgb        3 bytes per node or NULL
+ * *n is always the number of nodes; the arrays (host memory) are filled when it is <= cap.
+ * min_depth > depth_levels, or a volume that misses the root: no nodes.  Waits for a pending scan.
+ * depth_levels < 5 is UFO_B200_E_UNSUPPORTED; an unknown volume type UFO_B200_E_INVALID.  A sharded
+ * or routed map iterates the part its own rank holds. */
+int ufo_b200_iterate(ufo_b200_map* m, int leaves_only, int occupied, int free_space, int unknown, int contains,
+                     uint32_t min_depth, const ufo_b200_volume* bv, size_t n_bv, uint64_t* codes, uint8_t* depths,
+                     float* logodds, uint8_t* flags, uint8_t* rgb, size_t cap, size_t* n);
 /* setValueVolume(BoundingVar, occupancy, min_depth) for one shape (the mapping server loops over the
  * shapes of a volume, server.cpp:345-354).  The bricks whose path passes are found by a descent on
  * the device, one level per kernel; more than 2^22 nodes at any level of it is UFO_B200_E_UNSUPPORTED

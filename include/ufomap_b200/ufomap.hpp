@@ -30,6 +30,7 @@
 #include <fstream>
 #include <istream>
 #include <iterator>
+#include <memory>
 #include <optional>
 #include <ostream>
 #include <string>
@@ -506,6 +507,15 @@ using CodeRay = std::vector<Code>;
 
 enum class OccupancyState { unknown, free, occupied };
 
+// what an iterator dereferences to (map/occupancy_map_node.h: OccupancyNode / ColorOccupancyNode value)
+struct OccupancyValue {
+	float occupancy = 0.0f;  // log-odds
+};
+struct ColorOccupancyValue {
+	float occupancy = 0.0f;  // log-odds
+	Color color;
+};
+
 namespace detail
 {
 // Common implementation of OccupancyMap / OccupancyMapColor over the C ABI.
@@ -545,6 +555,152 @@ class MapFacade
 	virtual ~MapFacade() { ufo_b200_destroy(map_); }
 
 	virtual std::string getTreeType() const noexcept { return COLOR ? "occupancy_map_color" : "occupancy_map"; }
+
+	//
+	// Iteration (occupancy_map_base.h:93-163, iterator/octree.h, iterator/occupancy_map.h): the nodes
+	// come from one ufo_b200_iterate call -- computed on the device, in the reference iterator's order --
+	// and the iterator walks that snapshot, so a map changed after begin*() does not change an
+	// iteration in progress.  Forward iterator; copies share the snapshot.
+	//
+	class Iterator
+	{
+	 public:
+		using value_type = std::conditional_t<COLOR, ColorOccupancyValue, OccupancyValue>;
+		using difference_type = std::ptrdiff_t;
+		using pointer = value_type const*;
+		using reference = value_type const&;
+		using iterator_category = std::forward_iterator_tag;
+
+		Iterator() {}  // the end iterator
+
+		// Equal when both are exhausted, or when both walk the same snapshot and are at the same node.
+		// (The reference's operator== compares the tree pointers only, so two live iterators of one map
+		// compare equal there whatever node they are at; that is not reproduced.)
+		bool operator==(Iterator const& o) const
+		{
+			return (atEnd() && o.atEnd()) || (!atEnd() && !o.atEnd() && s_ == o.s_ && i_ == o.i_);
+		}
+		bool operator!=(Iterator const& o) const { return !(*this == o); }
+		Iterator& operator++()
+		{
+			++i_;
+			load();
+			return *this;
+		}
+		Iterator operator++(int)
+		{
+			Iterator r = *this;
+			++(*this);
+			return r;
+		}
+		reference operator*() const { return value_; }
+		pointer operator->() const { return &value_; }
+
+		// Code::getChild from the root: Code(code, max(getDepth(), depth)) with the bits below zero
+		Code getCode(DepthType depth = 0) const
+		{
+			DepthType d = std::min(std::max(getDepth(), depth), s_->levels);
+			CodeType s = CodeType(3) * d;
+			return Code((s_->codes[i_] >> s) << s, d);
+		}
+		DepthType getDepth() const { return s_->depths[i_]; }
+		Point3 getCenter() const { return center_; }
+		double getX() const { return center_.x(); }
+		double getY() const { return center_.y(); }
+		double getZ() const { return center_.z(); }
+		double getSize() const { return 2.0 * getHalfSize(); }
+		double getHalfSize() const { return s_->half_size[getDepth()]; }
+		ufo::geometry::AABB getBoundingVolume() const { return ufo::geometry::AABB(center_, getHalfSize()); }
+		bool isLeaf() const { return s_->flags[i_] & 4u; }
+		bool isPureLeaf() const { return 0 == getDepth(); }
+		bool hasChildren() const { return !isLeaf(); }
+		// occupancy_map_base.h:926-980 on the node's value and flags
+		bool isOccupied() const { return s_->occupied_thres_log < value_.occupancy; }
+		bool isFree() const { return s_->free_thres_log > value_.occupancy; }
+		bool isUnknown() const { return !isOccupied() && !isFree(); }
+		bool containsOccupied() const { return isOccupied(); }
+		bool containsFree() const { return s_->flags[i_] & 1u; }
+		bool containsUnknown() const { return s_->flags[i_] & 2u; }
+		double getOccupancy() const { return toProb(value_.occupancy); }
+
+	 private:
+		friend class MapFacade;
+		struct Snapshot {
+			std::vector<std::uint64_t> codes;
+			std::vector<std::uint8_t> depths, flags, rgb;
+			std::vector<float> logodds;
+			double half_size[22];
+			DepthType levels;
+			double occupied_thres_log, free_thres_log;
+		};
+		explicit Iterator(std::shared_ptr<Snapshot const> s) : s_(std::move(s)) { load(); }
+		bool atEnd() const { return !s_ || i_ >= s_->codes.size(); }
+		void load()
+		{
+			if (atEnd()) return;
+			value_.occupancy = s_->logodds[i_];
+			if constexpr (COLOR) value_.color = Color(s_->rgb[3 * i_], s_->rgb[3 * i_ + 1], s_->rgb[3 * i_ + 2]);
+			// getChildCenter from the root down (octree.h:625-633), as the reference iterator accumulates it
+			Point3 c(0.0, 0.0, 0.0);
+			for (DepthType d = s_->levels; d > getDepth(); --d) {
+				unsigned idx = unsigned(s_->codes[i_] >> (3 * (d - 1))) & 7u;
+				double hs = s_->half_size[d - 1];
+				c[0] += (idx & 1u) ? hs : -hs;
+				c[1] += (idx & 2u) ? hs : -hs;
+				c[2] += (idx & 4u) ? hs : -hs;
+			}
+			center_ = c;
+		}
+		std::shared_ptr<Snapshot const> s_;
+		std::size_t i_ = 0;
+		value_type value_{};
+		Point3 center_;
+	};
+	using TreeIterator = Iterator;
+	using LeafIterator = Iterator;
+
+	// beginTree / beginLeaves with the reference's overloads and defaults.  A call that fails (no
+	// device, depth_levels < 5) gives an empty sequence; lastError() says why.
+	Iterator beginTree(bool occupied_space = true, bool free_space = true, bool unknown_space = false,
+	                   bool contains = false, DepthType min_depth = 0) const
+	{
+		return iterate(false, {}, occupied_space, free_space, unknown_space, contains, min_depth);
+	}
+	Iterator beginTree(ufo::geometry::BoundingVar const& bounding_volume, bool occupied_space = true,
+	                   bool free_space = true, bool unknown_space = false, bool contains = false,
+	                   DepthType min_depth = 0) const
+	{
+		return iterate(false, {ufo::geometry::toRecord(bounding_volume)}, occupied_space, free_space, unknown_space, contains,
+		               min_depth);
+	}
+	Iterator beginTree(ufo::geometry::BoundingVolume const& bounding_volume, bool occupied_space = true,
+	                   bool free_space = true, bool unknown_space = false, bool contains = false,
+	                   DepthType min_depth = 0) const
+	{
+		return iterate(false, ufo::geometry::toRecords(bounding_volume), occupied_space, free_space, unknown_space, contains,
+		               min_depth);
+	}
+	Iterator endTree() const noexcept { return Iterator(); }
+	Iterator beginLeaves(bool occupied_space = true, bool free_space = true, bool unknown_space = false,
+	                     bool contains = false, DepthType min_depth = 0) const
+	{
+		return iterate(true, {}, occupied_space, free_space, unknown_space, contains, min_depth);
+	}
+	Iterator beginLeaves(ufo::geometry::BoundingVar const& bounding_volume, bool occupied_space = true,
+	                     bool free_space = true, bool unknown_space = false, bool contains = false,
+	                     DepthType min_depth = 0) const
+	{
+		return iterate(true, {ufo::geometry::toRecord(bounding_volume)}, occupied_space, free_space, unknown_space, contains,
+		               min_depth);
+	}
+	Iterator beginLeaves(ufo::geometry::BoundingVolume const& bounding_volume, bool occupied_space = true,
+	                     bool free_space = true, bool unknown_space = false, bool contains = false,
+	                     DepthType min_depth = 0) const
+	{
+		return iterate(true, ufo::geometry::toRecords(bounding_volume), occupied_space, free_space, unknown_space, contains,
+		               min_depth);
+	}
+	Iterator endLeaves() const noexcept { return Iterator(); }
 
 	//
 	// File / wire format (octree.h:776-864): whole map or the part inside an AABB, truncated at
@@ -974,6 +1130,30 @@ class MapFacade
 		std::uint32_t d = code.getDepth();
 		ufo_b200_query(map_, &c, &d, 1, &v.logodds, &v.flags, COLOR ? v.rgb : nullptr);
 		return v;
+	}
+	Iterator iterate(bool leaves, std::vector<ufo_b200_volume> const& bv, bool occupied, bool free_space, bool unknown,
+	                 bool contains, DepthType min_depth) const
+	{
+		auto s = std::make_shared<typename Iterator::Snapshot>();
+		auto call = [&](std::size_t cap, std::size_t* n) {
+			return ufo_b200_iterate(map_, leaves, occupied, free_space, unknown, contains, min_depth, bv.data(), bv.size(),
+			                        cap ? s->codes.data() : nullptr, cap ? s->depths.data() : nullptr,
+			                        cap ? s->logodds.data() : nullptr, cap ? s->flags.data() : nullptr,
+			                        cap && COLOR ? s->rgb.data() : nullptr, cap, n);
+		};
+		std::size_t n = 0;
+		if (UFO_B200_OK != call(0, &n) || 0 == n) return Iterator();
+		s->codes.resize(n);
+		s->depths.resize(n);
+		s->logodds.resize(n);
+		s->flags.resize(n);
+		if (COLOR) s->rgb.resize(3 * n);
+		if (UFO_B200_OK != call(n, &n) || n != s->codes.size()) return Iterator();
+		s->levels = getTreeDepthLevels();
+		for (DepthType d = 0; d < 22; ++d) s->half_size[d] = getNodeHalfSize(d);
+		s->occupied_thres_log = model()[0];
+		s->free_thres_log = model()[1];
+		return Iterator(std::move(s));
 	}
 	// occupancy_map_base.h:911 -- LogitType is float there: the argument narrows to float and the
 	// exponential is the float one, for the sensor-model getters as well as for getOccupancy

@@ -87,6 +87,7 @@ SYMBOLS = [
     "ufo_b200_export_nodes_bv", "ufo_b200_set_value_volume_bv", "ufo_b200_volume_intersects",
     "ufo_b200_geometry_frustum", "ufo_b200_geometry_plane", "ufo_b200_geometry_ray",
     "ufo_b200_set_early_stopping", "ufo_b200_last_early_stats",
+    "ufo_b200_iterate",
 ]
 
 # ufo_b200_volume: one shape of a bounding volume (type in BoundingVar order, members in v)
@@ -276,6 +277,7 @@ def load():
     lib.ufo_b200_write_compressed_bv.argtypes = [vp, vp, sz, u32, i32, i32, i32, vp, sz, C.POINTER(sz), C.POINTER(sz)]
     lib.ufo_b200_read_data_bv.argtypes = [vp, vp, sz, vp, sz, i32, sz]
     lib.ufo_b200_export_nodes_bv.argtypes = [vp, u32, i32, i32, i32, vp, sz, vp, vp, vp, sz, C.POINTER(sz)]
+    lib.ufo_b200_iterate.argtypes = [vp, i32, i32, i32, i32, i32, u32, vp, sz, vp, vp, vp, vp, vp, sz, C.POINTER(sz)]
     lib.ufo_b200_set_value_volume_bv.argtypes = [vp, vp, dbl, u32]
     lib.ufo_b200_volume_intersects.argtypes = [vp, sz, vp, vp, sz, vp]
     lib.ufo_b200_geometry_frustum.argtypes = [vp, vp, vp, dbl, dbl, dbl, dbl, vp]
@@ -652,6 +654,28 @@ class Map:
                                                           rgb.ctypes.data if self.color else None, cnt, C.byref(n)))
         order = np.argsort(codes, kind="stable")
         return codes[order], occ[order], rgb[order]
+
+    def iterate(self, volume=None, leaves=True, occupied=True, free=True, unknown=False, contains=False, min_depth=0):
+        """beginLeaves (leaves=True) / beginTree (occupancy_map_base.h:93-163) over a bounding volume
+        (None: the whole map): (codes, depths u8, logodds f32, flags u8, rgb u8[n,3]) in the
+        reference iterator's order.  flags: bit0 contains_free, bit1 contains_unknown, bit2 isLeaf."""
+        bv, bp, nb = self._bv(volume)
+        args = (int(bool(leaves)), int(bool(occupied)), int(bool(free)), int(bool(unknown)), int(bool(contains)),
+                int(min_depth), bp, nb)
+        n = C.c_size_t()
+        self._check(self.lib.ufo_b200_iterate(self.h, *args, None, None, None, None, None, 0, C.byref(n)))
+        cnt = n.value
+        codes = np.empty(cnt, np.uint64)
+        depths = np.empty(cnt, np.uint8)
+        occ = np.empty(cnt, np.float32)
+        flags = np.empty(cnt, np.uint8)
+        rgb = np.zeros((cnt, 3), np.uint8)
+        if cnt:
+            self._check(self.lib.ufo_b200_iterate(self.h, *args, codes.ctypes.data, depths.ctypes.data, occ.ctypes.data,
+                                                  flags.ctypes.data, rgb.ctypes.data if self.color else None, cnt,
+                                                  C.byref(n)))
+            assert n.value == cnt
+        return codes, depths, occ, flags, rgb
 
     def set_value_volume_bv(self, shape, occupancy, min_depth=0):
         """setValueVolume(BoundingVar, occupancy probability, min_depth) for one shape record."""

@@ -41,8 +41,34 @@ UFO_HD void child_center(const double c[3], double hs, uint32_t i, double out[3]
 	out[2] = dop::add(c[2], (i & 4u) ? hs : -hs);
 }
 
+// The canonical-leaf rule, the one place that decides the tree shape of the file writer and of the
+// iteration (k_brick_stream, k_brick_iter, build_upper): a node keeps its children unless none of
+// them has children and all eight carry the same payload, colour included.  rgb == nullptr: no colour.
+UFO_HD bool keeps_children(bool a_child_has_children, const float* occ, const uint32_t* rgb)
+{
+	if (a_child_has_children) return true;
+	for (int i = 1; i < 8; ++i)
+		if (occ[i] != occ[0] || (rgb && rgb[i] != rgb[0])) return true;
+	return false;
+}
+
+// centre of the brick's cube, accumulated from the root like the reference's recursion
+UFO_HD void brick_center(const Geometry& g, uint32_t kx, uint32_t ky, uint32_t kz, double c[3])
+{
+	c[0] = c[1] = c[2] = 0.0;
+	for (uint32_t d = g.depth_levels; d > 4; --d) {
+		const uint32_t bit = d - 5;  // brick-key bit that selects the child of the depth-d node
+		const uint32_t i = ((kx >> bit) & 1u) | (((ky >> bit) & 1u) << 1) | (((kz >> bit) & 1u) << 2);
+		double n[3];
+		child_center(c, g.half_size[d - 1], i, n);
+		c[0] = n[0];
+		c[1] = n[1];
+		c[2] = n[2];
+	}
+}
+
 struct BrickInfo {
-	uint32_t size;   // bytes the brick contributes to the stream (0: skipped by the box)
+	uint32_t size;   // bytes the brick contributes to the stream (0: skipped by the box); k_brick_iter: records
 	uint32_t flags;  // bit 0: has children (in the map); bit 1: not part of the map (alias collector);
 	                 // bit 2: written as a record (size bytes at its offset), else as a payload
 	float occ;       // payload when bit 2 is clear: the leaf value, or the depth-4 aggregate
@@ -113,17 +139,8 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 		return;
 	}
 	if (t == 0) {
-		// centre of the brick, accumulated from the root like the reference's recursion
-		double c[3] = {0.0, 0.0, 0.0};
-		for (uint32_t d = M.g.depth_levels; d > 4; --d) {
-			const uint32_t bit = d - 5;  // brick-key bit that selects the child of the depth-d node
-			const uint32_t i = ((kx >> bit) & 1u) | (((ky >> bit) & 1u) << 1) | (((kz >> bit) & 1u) << 2);
-			double n[3];
-			child_center(c, M.g.half_size[d - 1], i, n);
-			c[0] = n[0];
-			c[1] = n[1];
-			c[2] = n[2];
-		}
+		double c[3];
+		brick_center(M.g, kx, ky, kz, c);
 		s_center[0] = c[0];
 		s_center[1] = c[1];
 		s_center[2] = c[2];
@@ -157,22 +174,14 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 		}
 		const float* lp = M.leaf + b * 64 + 8 * o;
 		const uint32_t* cp = COLOR ? M.leaf_rgb + b * 64 + 8 * o : nullptr;
-		const float v0 = lp[0];
-		const uint32_t c0 = COLOR ? cp[0] : 0u;
-		bool same = true;
-		for (int j = 1; j < 8; ++j) same = same && lp[j] == v0 && (!COLOR || cp[j] == c0);
-		if (same) {
-			oocc[o] = v0;
-			orgb[o] = c0;
-		} else {
+		if (keeps_children(false, lp, cp)) {
 			oct_has |= 1u << o;
+		} else {
+			oocc[o] = lp[0];
+			orgb[o] = COLOR ? cp[0] : 0u;
 		}
 	}
-	bool blk_has = oct_has != 0;
-	if (pruned && !blk_has) {
-#pragma unroll
-		for (int o = 1; o < 8; ++o) blk_has = blk_has || oocc[o] != oocc[0] || orgb[o] != orgb[0];
-	}
+	const bool blk_has = pruned ? keeps_children(oct_has != 0, oocc, orgb) : oct_has != 0;
 	// the block's contribution to the stream
 	uint32_t blk_size = 0;
 	if (blk_hit && d3_hit && brick_hit) {
@@ -206,10 +215,8 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 			if (min_depth < 2) mask |= (uint32_t)s_blk_has[c] << k;
 			size += s_blk_size[c];
 		}
-		if (pruned && !has) {
-			// leaf blocks only: s_blk_occ / s_blk_rgb hold their leaf payloads
-			for (int k = 1; k < 8; ++k) has = has || s_blk_occ[8 * t + k] != s_blk_occ[8 * t] || s_blk_rgb[8 * t + k] != s_blk_rgb[8 * t];
-		}
+		// leaf blocks only reach the payload test: s_blk_occ / s_blk_rgb hold their leaf payloads
+		if (pruned) has = keeps_children(has, s_blk_occ + 8 * t, s_blk_rgb + 8 * t);
 		s_d3_has[t] = has ? 1 : 0;
 		s_d3_hit[t] = hit ? 1 : 0;
 		s_d3_mask[t] = (uint8_t)mask;
@@ -226,9 +233,7 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 			s_d3_off[j] = size;
 			size += s_d3_size[j];
 		}
-		if (pruned && !has) {
-			for (int j = 1; j < 8; ++j) has = has || s_d3_occ[j] != s_d3_occ[0] || s_d3_rgb[j] != s_d3_rgb[0];
-		}
+		if (pruned) has = keeps_children(has, s_d3_occ, s_d3_rgb);
 		const bool record = has && min_depth < 4 && brick_hit;
 		s_brick_record = record ? 1u : 0u;
 		s_brick_size = !brick_hit ? 0u : (record ? size : P);
@@ -274,6 +279,239 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 	__syncthreads();
 	uint8_t* dst = out + offsets[brick];
 	for (uint32_t i = t; i < s_brick_size; i += 64) dst[i] = s_buf[i];
+}
+
+// ---------------------------------------------------------------------------
+// Iteration: beginTree / beginLeaves (occupancy_map_base.h:93-163) over the canonical tree of the
+// file writer, in the reference's order -- pre-order, children 0..7 (iterator/octree.h:181-316) --
+// with its filters (iterator/occupancy_map.h:168-208).  A node is visited when its parent is
+// descended into and validNode holds: its cube passes the volume (centres accumulated like
+// getChildCenter) and, when contains or depth != min_depth, one of the contains tests passes
+// (containsOccupied: max > occupied threshold; containsFree / containsUnknown: the node's flags, its
+// own state at depth 0), else one of the own-state tests.  A visited node is descended into when
+// depth > min_depth and it is not a leaf.  It is returned when validReturnNode holds: leaves
+// iterator -- depth == min_depth or a leaf, and the own state; tree iterator -- the contains tests
+// when contains, else the own state.  Values are the file writer's: a leaf carries its payload, an
+// inner node its aggregate; flags are those ufo_b200_query reports.
+//
+// k_brick_iter produces the records of one brick's subtree (depth 4 down) assuming its parent is
+// descended into; the host walks the levels above and splices the bricks it reaches in Morton
+// order (ufo_map.cu, iterate).  Size pass (offsets == nullptr): info[brick] = records, shape and
+// payload of the brick node.  Emit pass: the records of every brick with offsets[brick] != ~0 go
+// to out + offsets[brick].  One CTA per brick, one thread per 4^3 block; only the octets whose
+// "initialised" bit is set are read below depth 2.
+struct IterArgs {
+	Volume vol;
+	double occ_thr, free_thr;
+	uint32_t min_depth;
+	int leaves_only, occupied, free_, unknown, contains;
+};
+
+// One returned node.  meta: rgb in bits 0..23, depth in 24..28, bit 29 contains_free, bit 30
+// contains_unknown, bit 31 leaf.
+struct IterRec {
+	unsigned long long code;
+	float occ;
+	uint32_t meta;
+};
+
+UFO_HD IterRec iter_rec(unsigned long long code, float v, uint32_t rgb, uint32_t d, uint32_t fl, bool leaf)
+{
+	return {code, v, (rgb & 0xffffffu) | (d << 24) | ((fl & 3u) << 29) | (leaf ? 1u << 31 : 0u)};
+}
+
+UFO_HD bool iter_own(const IterArgs& a, float v)
+{
+	const bool occ = a.occ_thr < (double)v, fre = a.free_thr > (double)v;
+	return (a.occupied && occ) || (a.free_ && fre) || (a.unknown && !occ && !fre);
+}
+
+// flags: bit 0 contains_free, bit 1 contains_unknown (at depth 0: the node's own free / unknown state)
+UFO_HD bool iter_contains(const IterArgs& a, float v, uint32_t fl)
+{
+	return (a.occupied && a.occ_thr < (double)v) || (a.unknown && (fl & 2u)) || (a.free_ && (fl & 1u));
+}
+
+// validNode without the cube test
+UFO_HD bool iter_valid(const IterArgs& a, uint32_t d, float v, uint32_t fl)
+{
+	return (a.contains || d != a.min_depth) ? iter_contains(a, v, fl) : iter_own(a, v);
+}
+
+UFO_HD bool iter_returns(const IterArgs& a, uint32_t d, bool leaf, float v, uint32_t fl)
+{
+	if (a.leaves_only) return (d == a.min_depth || leaf) && iter_own(a, v);
+	return a.contains ? iter_contains(a, v, fl) : iter_own(a, v);
+}
+
+// validNode of a node whose parent is descended into; *ret = validReturnNode
+template <bool G>
+__device__ __forceinline__ bool iter_visit(const IterArgs& a, const double c[3], double hs, uint32_t d, float v, uint32_t fl,
+                                           bool leaf, bool* ret)
+{
+	*ret = false;
+	if (!vol_hits_t<G>(a.vol, c, hs) || !iter_valid(a, d, v, fl)) return false;
+	*ret = iter_returns(a, d, leaf, v, fl);
+	return true;
+}
+
+// The records of one depth-2 node (block b) and its subtree, its parent being descended into;
+// written to dst when dst != nullptr.  oct_has / oocc / orgb: the block's octets as the canonical
+// shape sees them.
+template <bool COLOR, bool G>
+__device__ __forceinline__ uint32_t block_records(const DeviceMap& M, const IterArgs& a, size_t b, uint32_t meta,
+                                                  uint32_t oct_has, const float oocc[8], const uint32_t orgb[8],
+                                                  bool blk_has, float blk_v, uint32_t blk_rgb, const double blkc[3],
+                                                  unsigned long long code, IterRec* dst)
+{
+	const uint32_t blk_fl = (meta >> 16) ? M.agg2[b].flags : M.default_flags;
+	uint32_t n = 0;
+	bool ret;
+	if (!iter_visit<G>(a, blkc, M.g.half_size[2], 2, blk_v, blk_fl, !blk_has, &ret)) return 0;
+	if (ret) {
+		if (dst) dst[n] = iter_rec(code, blk_v, blk_rgb, 2, blk_fl, !blk_has);
+		++n;
+	}
+	if (a.min_depth >= 2 || !blk_has) return n;
+	for (uint32_t o = 0; o < 8; ++o) {
+		const bool oi = (meta >> (16 + o)) & 1u, oh = (oct_has >> o) & 1u;
+		const float ov = oh ? M.sum1[b * 8 + o] : oocc[o];
+		const uint32_t orv = oh ? (COLOR ? M.sum1_rgb[b * 8 + o] : 0u) : orgb[o];
+		const uint32_t ofl = oi ? (meta >> (2 * o)) & 3u : M.default_flags;
+		const unsigned long long ocode = code | ((unsigned long long)o << 3);
+		double oc[3];
+		child_center(blkc, M.g.half_size[1], o, oc);
+		if (!iter_visit<G>(a, oc, M.g.half_size[1], 1, ov, ofl, !oh, &ret)) continue;
+		if (ret) {
+			if (dst) dst[n] = iter_rec(ocode, ov, orv, 1, ofl, !oh);
+			++n;
+		}
+		if (a.min_depth >= 1 || !oh) continue;
+		for (uint32_t j = 0; j < 8; ++j) {
+			const float v = M.leaf[b * 64 + 8 * o + j];
+			const uint32_t fl = leaf_flags(M, v);
+			double vc[3];
+			child_center(oc, M.g.half_size[0], j, vc);
+			if (!iter_visit<G>(a, vc, M.g.half_size[0], 0, v, fl, true, &ret) || !ret) continue;
+			if (dst) dst[n] = iter_rec(ocode | j, v, COLOR ? M.leaf_rgb[b * 64 + 8 * o + j] : 0u, 0, fl, true);
+			++n;
+		}
+	}
+	return n;
+}
+
+template <bool COLOR, bool G>
+__global__ void __launch_bounds__(64) k_brick_iter(DeviceMap M, uint32_t n_bricks, IterArgs a, BrickInfo* info,
+                                                   const unsigned long long* offsets, IterRec* out)
+{
+	__shared__ float s_blk_occ[64], s_d3_occ[8];
+	__shared__ uint32_t s_blk_rgb[64], s_d3_rgb[8], s_warp[2];
+	__shared__ uint8_t s_blk_has[64], s_d3_has[8], s_desc3[8], s_ret3[8];
+	__shared__ IterRec s_rec4, s_rec3[8];
+	__shared__ uint8_t s_desc4, s_ret4;
+	__shared__ double s_center[3];
+	const uint32_t brick = blockIdx.x, t = threadIdx.x;
+	if (brick >= n_bricks) return;
+	if (offsets && offsets[brick] == ~0ull) return;  // not reached by the walk above the bricks
+	uint32_t kx, ky, kz;
+	unpack_key(M.brick_key[brick], kx, ky, kz);
+	if ((kx | ky | kz) & ~(M.g.key_mask >> 4)) {  // collects out-of-tree marks, owns no voxels
+		if (!offsets && t == 0) info[brick] = {0u, 2u, 0.0f, 0u};
+		return;
+	}
+	const unsigned long long code4 = key_to_code({kx << 4, ky << 4, kz << 4});
+	if (t == 0) brick_center(M.g, kx, ky, kz, s_center);
+	// canonical shape of the block (as k_brick_stream, pruned)
+	const size_t b = (size_t)brick * 64 + t;
+	const uint32_t meta = M.meta[b];
+	uint32_t oct_has = 0;
+	float oocc[8];
+	uint32_t orgb[8];
+#pragma unroll
+	for (uint32_t o = 0; o < 8; ++o) {
+		oocc[o] = 0.0f;
+		orgb[o] = 0u;
+		if (!((meta >> (16 + o)) & 1u)) continue;
+		const float* lp = M.leaf + b * 64 + 8 * o;
+		const uint32_t* cp = COLOR ? M.leaf_rgb + b * 64 + 8 * o : nullptr;
+		if (keeps_children(false, lp, cp)) {
+			oct_has |= 1u << o;
+		} else {
+			oocc[o] = lp[0];
+			orgb[o] = COLOR ? cp[0] : 0u;
+		}
+	}
+	const bool blk_has = keeps_children(oct_has != 0, oocc, orgb);
+	const float blk_v = blk_has ? M.agg2[b].occ : oocc[0];
+	const uint32_t blk_rgb = blk_has ? (COLOR ? M.rgb2[b] : 0u) : orgb[0];
+	s_blk_has[t] = blk_has ? 1 : 0;
+	s_blk_occ[t] = blk_v;
+	s_blk_rgb[t] = blk_rgb;
+	__syncthreads();
+	const uint32_t j3 = t >> 3, k3 = t & 7u;
+	const double bc[3] = {s_center[0], s_center[1], s_center[2]};
+	double d3c[3], blkc[3];
+	child_center(bc, M.g.half_size[3], j3, d3c);
+	child_center(d3c, M.g.half_size[2], k3, blkc);
+	if (t < 8) {
+		bool any = false;
+		for (int k = 0; k < 8; ++k) any = any || s_blk_has[8 * t + k];
+		const bool has = keeps_children(any, s_blk_occ + 8 * t, s_blk_rgb + 8 * t);
+		s_d3_has[t] = has ? 1 : 0;
+		s_d3_occ[t] = has ? M.brick_sum3[(size_t)brick * 8 + t].occ : s_blk_occ[8 * t];
+		s_d3_rgb[t] = has ? (COLOR ? M.brick_rgb3[(size_t)brick * 8 + t] : 0u) : s_blk_rgb[8 * t];
+	}
+	__syncthreads();
+	if (t == 0) {
+		bool any = false;
+		for (int j = 0; j < 8; ++j) any = any || s_d3_has[j];
+		const bool has = keeps_children(any, s_d3_occ, s_d3_rgb);
+		const float v = has ? M.brick_sum4[brick].occ : s_d3_occ[0];
+		const uint32_t rgb = has ? (COLOR ? M.brick_rgb4[brick] : 0u) : s_d3_rgb[0];
+		const uint32_t fl = M.brick_sum4[brick].flags;
+		bool ret;
+		const bool vis = a.min_depth <= 4 && iter_visit<G>(a, bc, M.g.half_size[4], 4, v, fl, !has, &ret);
+		s_desc4 = (vis && a.min_depth < 4 && has) ? 1 : 0;
+		s_ret4 = (vis && ret) ? 1 : 0;
+		s_rec4 = iter_rec(code4, v, rgb, 4, fl, !has);
+		if (!offsets) info[brick] = {0u, has ? 1u : 0u, v, rgb};  // size: below
+	}
+	__syncthreads();
+	if (t < 8) {
+		const bool has = s_d3_has[t];
+		const float v = s_d3_occ[t];
+		const uint32_t fl = M.brick_sum3[(size_t)brick * 8 + t].flags;
+		double c3[3];
+		child_center(bc, M.g.half_size[3], t, c3);
+		bool ret = false;
+		const bool vis = s_desc4 && iter_visit<G>(a, c3, M.g.half_size[3], 3, v, fl, !has, &ret);
+		s_desc3[t] = (vis && a.min_depth < 3 && has) ? 1 : 0;
+		s_ret3[t] = (vis && ret) ? 1 : 0;
+		s_rec3[t] = iter_rec(code4 | ((unsigned long long)t << 9), v, s_d3_rgb[t], 3, fl, !has);
+	}
+	__syncthreads();
+	// this thread's records, in pre-order: the brick node (t == 0), the depth-3 node (k3 == 0), the block
+	const unsigned long long blk_code = code4 | ((unsigned long long)t << 6);
+	const uint32_t head = (t == 0 ? s_ret4 : 0u) + (k3 == 0 ? s_ret3[j3] : 0u);
+	const uint32_t mine =
+	    head + (s_desc3[j3] ? block_records<COLOR, G>(M, a, b, meta, oct_has, oocc, orgb, blk_has, blk_v, blk_rgb, blkc, blk_code, nullptr) : 0u);
+	const uint32_t lane = t & 31u, warp = t >> 5;
+	uint32_t incl = mine;
+#pragma unroll
+	for (uint32_t off = 1; off < 32; off <<= 1) {
+		const uint32_t y = __shfl_up_sync(0xffffffffu, incl, off);
+		if (lane >= off) incl += y;
+	}
+	if (lane == 31) s_warp[warp] = incl;
+	__syncthreads();
+	if (!offsets) {
+		if (t == 0) info[brick].size = s_warp[0] + s_warp[1];
+		return;
+	}
+	IterRec* dst = out + offsets[brick] + (incl - mine) + (warp ? s_warp[0] : 0u);
+	if (t == 0 && s_ret4) *dst++ = s_rec4;
+	if (k3 == 0 && s_ret3[j3]) *dst++ = s_rec3[j3];
+	if (mine > head) block_records<COLOR, G>(M, a, b, meta, oct_has, oocc, orgb, blk_has, blk_v, blk_rgb, blkc, blk_code, dst);
 }
 
 // ---------------------------------------------------------------------------

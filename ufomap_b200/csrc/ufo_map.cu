@@ -2189,11 +2189,7 @@ int32_t build_upper(ExportPlan& plan, uint32_t d, size_t lo, size_t hi, const do
 		if (hit) n.size += bytes;
 		pos = end;
 	}
-	if (plan.pruned && !any_children) {
-		bool same = true;
-		for (int i = 1; i < 8; ++i) same = same && occ[i] == occ[0] && rgb[i] == rgb[0];
-		if (same) n.has = false;
-	}
+	if (plan.pruned) n.has = keeps_children(any_children, occ, rgb);
 	n.occ = occ[0];  // payload if collapsed
 	n.rgb = rgb[0];
 	plan.nodes[self] = n;
@@ -3311,6 +3307,244 @@ int ufo_b200_export_nodes_bv(ufo_b200_map* m, uint32_t depth, int occupied, int 
 	return guarded(m, [&]() {
 		return export_nodes(m, depth, occupied, free_space, unknown, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, true, codes, logodds,
 		                    rgb, cap, n);
+	});
+}
+
+}  // extern "C"
+
+namespace
+{
+// ---- iteration (ufo_export.cuh, k_brick_iter): the levels above the bricks on the host ----
+struct IterWalk {
+	const ExportPlan* plan = nullptr;  // tree shape above the bricks (build_upper)
+	IterArgs a{};                      // host volume records
+	std::vector<float> occ;            // ufo_b200_query values of plan->nodes
+	std::vector<uint8_t> flags;
+	std::vector<uint32_t> rgb;
+	uint32_t default_flags = 0;
+	// the sequence: a record of a node above the bricks (brick == kNone), or the records of a brick
+	std::vector<std::pair<IterRec, uint32_t>> pieces;
+	std::vector<unsigned long long> offs;  // per brick slot: first record in the packed brick records, ~0 = not reached
+	unsigned long long packed = 0, total = 0;
+};
+
+// code and depth of every node of the shape, for the value query
+void upper_codes(const ExportPlan& plan, int32_t idx, uint32_t d, unsigned long long code, std::vector<unsigned long long>& codes,
+                 std::vector<uint32_t>& depths)
+{
+	codes[idx] = code;
+	depths[idx] = d;
+	if (d == 5) return;
+	for (uint32_t i = 0; i < 8; ++i)
+		if (plan.nodes[idx].child[i] >= 0)
+			upper_codes(plan, plan.nodes[idx].child[i], d - 1, code | ((unsigned long long)i << (3 * (d - 1))), codes, depths);
+}
+
+// node (idx into plan->nodes, -1: a default leaf) of depth d >= 4 whose parent is descended into
+void iter_walk(IterWalk& w, int32_t idx, uint32_t d, unsigned long long code, const double c[3], float v, uint32_t fl, uint32_t rgb,
+               bool leaf)
+{
+	const Geometry& g = *w.plan->g;
+	if (!vol_hits(w.a.vol, c, g.half_size[d]) || !iter_valid(w.a, d, v, fl)) return;
+	if (iter_returns(w.a, d, leaf, v, fl)) {
+		w.pieces.emplace_back(iter_rec(code, v, rgb, d, fl, leaf), kNone);
+		++w.total;
+	}
+	if (d <= w.a.min_depth || leaf) return;
+	const UpNode& n = w.plan->nodes[idx];
+	for (uint32_t i = 0; i < 8; ++i) {
+		double cc[3];
+		child_center(c, g.half_size[d - 1], i, cc);
+		const unsigned long long ccode = code | ((unsigned long long)i << (3 * (d - 1)));
+		const int32_t ch = n.child[i];
+		if (ch < 0) {
+			iter_walk(w, -1, d - 1, ccode, cc, 0.0f, w.default_flags, 0u, true);
+		} else if (d == 5) {
+			// the brick node and its subtree: validNode and the rest were evaluated by the size pass
+			const uint32_t slot = w.plan->order[ch];
+			const uint32_t k = w.plan->info[slot].size;
+			if (!k) continue;
+			w.offs[slot] = w.packed;
+			w.packed += k;
+			w.total += k;
+			w.pieces.emplace_back(IterRec{}, slot);
+		} else {
+			const UpNode& cn = w.plan->nodes[ch];
+			iter_walk(w, ch, d - 1, ccode, cc, cn.has ? w.occ[ch] : cn.occ, w.flags[ch], cn.has ? w.rgb[ch] : cn.rgb, !cn.has);
+		}
+	}
+}
+
+int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, float* logodds, uint8_t* flags, uint8_t* rgb, size_t cap,
+            size_t* n)
+{
+	*n = 0;
+	if (m->M.g.depth_levels < 5) {
+		m->set_error("iteration needs depth_levels >= 5");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	CK(cudaSetDevice(m->device));
+	sync_map(m);
+	const uint32_t L = m->M.g.depth_levels;
+	const double c0[3] = {0.0, 0.0, 0.0};
+	if (args.min_depth > L || !vol_hits(args.vol, c0, m->M.g.half_size[L])) return UFO_B200_OK;  // octree.h:200-208
+	cudaStream_t s = m->stream;
+	const uint32_t nb = m->n_bricks;
+	const bool color = m->M.color != 0;
+	ExportPlan plan;
+	plan.levels = L;
+	plan.pruned = true;
+	plan.g = &m->M.g;
+	plan.info.resize(nb);
+	IterWalk w;
+	w.plan = &plan;
+	w.a = args;
+	w.a.occ_thr = m->M.occ_thr;
+	w.a.free_thr = m->M.free_thr;
+	w.default_flags = m->M.default_flags;
+	w.offs.assign(nb, ~0ull);
+	BrickInfo* d_info = nullptr;
+	unsigned long long* d_offs = nullptr;
+	IterRec* d_out = nullptr;
+	unsigned long long* d_qcodes = nullptr;
+	uint32_t *d_qdepths = nullptr, *d_qrgb = nullptr;
+	float* d_qocc = nullptr;
+	uint8_t* d_qflags = nullptr;
+	DeviceVolume dvol;
+	auto cleanup = [&]() {
+		for (void* p : {(void*)d_info, (void*)d_offs, (void*)d_out, (void*)d_qcodes, (void*)d_qdepths, (void*)d_qrgb, (void*)d_qocc,
+		                (void*)d_qflags})
+			if (p) cudaFree(p);
+	};
+	try {
+		Volume hv = args.vol;
+		const bool general = volume_is_general(hv);
+		IterArgs da = w.a;
+		da.vol = dvol.upload(hv, s);
+		auto brick_iter = [&](const unsigned long long* offs, IterRec* out) {
+			if (color && general) k_brick_iter<true, true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+			else if (color) k_brick_iter<true, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+			else if (general) k_brick_iter<false, true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+			else k_brick_iter<false, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+		};
+		std::vector<unsigned long long> keys(nb);
+		if (nb) {
+			CK(cudaMalloc(&d_info, sizeof(BrickInfo) * nb));
+			brick_iter(nullptr, nullptr);
+			CK(cudaGetLastError());
+			CK(cudaMemcpyAsync(plan.info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
+			CK(cudaMemcpyAsync(keys.data(), m->M.brick_key, 8ull * nb, cudaMemcpyDeviceToHost, s));
+			CK(cudaStreamSynchronize(s));
+		}
+		// bricks in the tree, in Morton order (as export_image: a default leaf brick is untouched space)
+		std::vector<std::pair<unsigned long long, uint32_t>> sorted;
+		sorted.reserve(nb);
+		for (uint32_t b = 0; b < nb; ++b) {
+			const BrickInfo& bi = plan.info[b];
+			if (bi.flags & 2u) continue;
+			if (!(bi.flags & 1u) && bi.occ == 0.0f && bi.rgb == 0u) continue;
+			uint32_t x, y, z;
+			unpack_key(keys[b], x, y, z);
+			sorted.emplace_back(spread3_host(x) | (spread3_host(y) << 1) | (spread3_host(z) << 2), b);
+		}
+		std::sort(sorted.begin(), sorted.end());
+		plan.order.resize(sorted.size());
+		plan.codes.resize(sorted.size());
+		for (size_t i = 0; i < sorted.size(); ++i) {
+			plan.codes[i] = sorted[i].first;
+			plan.order[i] = sorted[i].second;
+		}
+		if (sorted.empty()) {
+			iter_walk(w, -1, L, 0ull, c0, 0.0f, w.default_flags, 0u, true);
+		} else {
+			build_upper(plan, L, 0, sorted.size(), c0);
+			// values of the nodes above the bricks: ufo_b200_query's, one batch
+			const size_t nu = plan.nodes.size();
+			std::vector<unsigned long long> qc(nu);
+			std::vector<uint32_t> qd(nu), qrgb(nu, 0u);
+			upper_codes(plan, 0, L, 0ull, qc, qd);
+			w.occ.resize(nu);
+			w.flags.resize(nu);
+			CK(cudaMalloc(&d_qcodes, 8 * nu));
+			CK(cudaMalloc(&d_qdepths, 4 * nu));
+			CK(cudaMalloc(&d_qocc, 4 * nu));
+			CK(cudaMalloc(&d_qflags, nu));
+			if (color) CK(cudaMalloc(&d_qrgb, 4 * nu));
+			CK(cudaMemcpyAsync(d_qcodes, qc.data(), 8 * nu, cudaMemcpyHostToDevice, s));
+			CK(cudaMemcpyAsync(d_qdepths, qd.data(), 4 * nu, cudaMemcpyHostToDevice, s));
+			k_query<<<(uint32_t)((nu + 255) / 256), 256, 0, s>>>(m->M, d_qcodes, d_qdepths, (uint32_t)nu, d_qocc, d_qflags, d_qrgb);
+			CK(cudaGetLastError());
+			CK(cudaMemcpyAsync(w.occ.data(), d_qocc, 4 * nu, cudaMemcpyDeviceToHost, s));
+			CK(cudaMemcpyAsync(w.flags.data(), d_qflags, nu, cudaMemcpyDeviceToHost, s));
+			if (color) CK(cudaMemcpyAsync(qrgb.data(), d_qrgb, 4 * nu, cudaMemcpyDeviceToHost, s));
+			CK(cudaStreamSynchronize(s));
+			w.rgb = std::move(qrgb);
+			const UpNode& r = plan.nodes[0];
+			iter_walk(w, 0, L, 0ull, c0, r.has ? w.occ[0] : r.occ, w.flags[0], r.has ? w.rgb[0] : r.rgb, !r.has);
+		}
+		*n = (size_t)w.total;
+		if (codes && w.total && w.total <= cap) {
+			std::vector<IterRec> packed(w.packed);
+			if (w.packed) {
+				CK(cudaMalloc(&d_offs, 8ull * nb));
+				CK(cudaMalloc(&d_out, sizeof(IterRec) * w.packed));
+				CK(cudaMemcpyAsync(d_offs, w.offs.data(), 8ull * nb, cudaMemcpyHostToDevice, s));
+				brick_iter(d_offs, d_out);
+				CK(cudaGetLastError());
+				CK(cudaMemcpyAsync(packed.data(), d_out, sizeof(IterRec) * w.packed, cudaMemcpyDeviceToHost, s));
+				CK(cudaStreamSynchronize(s));
+			}
+			size_t at = 0;
+			auto put = [&](const IterRec& r) {
+				codes[at] = r.code;
+				depths[at] = (uint8_t)((r.meta >> 24) & 31u);
+				logodds[at] = r.occ;
+				flags[at] = (uint8_t)(r.meta >> 29);
+				if (rgb) {
+					rgb[3 * at] = (uint8_t)r.meta;
+					rgb[3 * at + 1] = (uint8_t)(r.meta >> 8);
+					rgb[3 * at + 2] = (uint8_t)(r.meta >> 16);
+				}
+				++at;
+			};
+			for (const auto& p : w.pieces) {
+				if (p.second == kNone) {
+					put(p.first);
+				} else {
+					const IterRec* r = packed.data() + w.offs[p.second];
+					for (uint32_t i = 0; i < plan.info[p.second].size; ++i) put(r[i]);
+				}
+			}
+		}
+	} catch (...) {
+		cleanup();
+		throw;
+	}
+	cleanup();
+	return UFO_B200_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int ufo_b200_iterate(ufo_b200_map* m, int leaves_only, int occupied, int free_space, int unknown, int contains, uint32_t min_depth,
+                     const ufo_b200_volume* bv, size_t n_bv, uint64_t* codes, uint8_t* depths, float* logodds, uint8_t* flags,
+                     uint8_t* rgb, size_t cap, size_t* n)
+{
+	if (!m || !n) return UFO_B200_E_INVALID;
+	*n = 0;
+	if (cap && (!codes || !depths || !logodds || !flags)) return UFO_B200_E_INVALID;
+	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() {
+		IterArgs a{};
+		a.vol = Volume{as_records(bv), (uint32_t)n_bv, {}, {}};
+		a.min_depth = min_depth;
+		a.leaves_only = leaves_only != 0;
+		a.occupied = occupied != 0;
+		a.free_ = free_space != 0;
+		a.unknown = unknown != 0;
+		a.contains = contains != 0;
+		return iterate(m, a, codes, depths, logodds, flags, rgb, cap, n);
 	});
 }
 
