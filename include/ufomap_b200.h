@@ -190,6 +190,28 @@ int ufo_b200_set_value_volume(ufo_b200_map* m, const double box6[6], double occu
 int ufo_b200_update_nodes(ufo_b200_map* m, const uint64_t* codes, const uint32_t* depths, const uint8_t* ops,
                           const float* values, size_t n, int async);
 
+/* ufo_b200_update_nodes plus the two writers of a colour map, as one ordered batch (DESIGN.md
+ * section 8); rgb[n][3] (host array) holds the colour of entry i, read for ops 2 and 3 only:
+ *   op[i] = 0, 1  as ufo_b200_update_nodes; the colour is left as it is.
+ *   op[i] = 2     ADD_COLOR: OccupancyMapColor::updateValue(code, value, Color(rgb))
+ *                 occupancy_map_color.h:269-287 -- the voxel's colour blends towards rgb
+ *                 (updateNodeColor, occupancy_map_color.cpp:142-171) weighted by toProb(value)
+ *                 against toProb of the log-odds the batch's earlier entries left, then the
+ *                 log-odds becomes clamp(v + value).  An unset colour takes rgb; rgb (0,0,0)
+ *                 onto a set colour blends towards black.
+ *   op[i] = 3     SET_COLOR: setColor(code, Color(rgb))  occupancy_map_color.cpp:74-81 -- the
+ *                 voxel's colour becomes rgb ((0,0,0) unsets it); the log-odds is unchanged.
+ * Ops 2 and 3 create the voxel like createNode does, and the inner colours up to the root are
+ * recomputed after the batch.  Change detection records a voxel when an ADD_COLOR changed its
+ * log-odds, never for SET_COLOR; the min/max change box is not updated.  Rejected as a whole,
+ * before anything is applied: op > 3, ops 2 / 3 on a map without colour, rgb == NULL while the
+ * batch holds op 2 or 3, a code outside the map (UFO_B200_E_INVALID); ops 2 / 3 at depth > 0 (the
+ * reference's result depends on whether the node has children) and everything
+ * ufo_b200_update_nodes rejects with UFO_B200_E_UNSUPPORTED.  These checks need no device. */
+int ufo_b200_update_nodes_color(ufo_b200_map* m, const uint64_t* codes, const uint32_t* depths,
+                                const uint8_t* ops, const float* values, const uint8_t* rgb, size_t n,
+                                int async);
+
 /* insertMissOnRay (hit_end = 0) / insertRay (hit_end = 1)  occupancy_map_base.h:251-268 for n rays,
  * origins / ends [n][3] (host arrays): integrateMiss on every node computeRay (octree.h:449-496, as
  * ufo_b200_compute_ray) walks at `depth`, then with hit_end integrateHit on the depth-0 voxel of the

@@ -1303,12 +1303,33 @@ class OccupancyMapColor : public detail::MapFacade<true>
 {
  public:
 	using detail::MapFacade<true>::MapFacade;
-	// occupancy_map_color.h:304-318
+
+	// occupancy_map_color.h:269-287 and :304-314.  Each call is a batch of one on the device
+	// (ufo_b200_update_nodes_color) at depth 0 only; the status is left in lastStatus().
+	void updateValue(Code const& code, float update, Color color) { writeColorNode(code, 2, update, color); }
+	void setColor(Code const& code, Color color) { writeColorNode(code, 3, 0.0f, color); }
+	void setColor(Point3 const& coord, Color color, DepthType depth = 0) { setColor(toCode(coord, depth), color); }
+	void setColor(double x, double y, double z, Color color, DepthType depth = 0)
+	{
+		setColor(toCode(x, y, z, depth), color);
+	}
+
+	// occupancy_map_color.h:320-330
 	Color getColor(Code const& code) const
 	{
 		NodeValue v = node(code);
 		return Color(v.rgb[0], v.rgb[1], v.rgb[2]);
 	}
 	Color getColor(Point3 const& coord, DepthType depth = 0) const { return getColor(toCode(coord, depth)); }
+	Color getColor(double x, double y, double z, DepthType depth = 0) const { return getColor(toCode(x, y, z, depth)); }
+
+ private:
+	void writeColorNode(Code const& code, std::uint8_t op, float value, Color color)
+	{
+		std::uint64_t c = code.getCode();
+		std::uint32_t d = code.getDepth();
+		const std::uint8_t rgb[3] = {color.r, color.g, color.b};
+		last_status_ = ufo_b200_update_nodes_color(map_, &c, &d, &op, &value, rgb, 1, 0);
+	}
 };
 }  // namespace ufo::map

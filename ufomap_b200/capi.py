@@ -87,7 +87,7 @@ SYMBOLS = [
     "ufo_b200_export_nodes_bv", "ufo_b200_set_value_volume_bv", "ufo_b200_volume_intersects",
     "ufo_b200_geometry_frustum", "ufo_b200_geometry_plane", "ufo_b200_geometry_ray",
     "ufo_b200_set_early_stopping", "ufo_b200_last_early_stats",
-    "ufo_b200_iterate",
+    "ufo_b200_iterate", "ufo_b200_update_nodes_color",
 ]
 
 # ufo_b200_volume: one shape of a bounding volume (type in BoundingVar order, members in v)
@@ -229,6 +229,7 @@ def load():
     lib.ufo_b200_clear_resize.argtypes = [vp, dbl, u32]
     lib.ufo_b200_set_value_volume.argtypes = [vp, vp, dbl, u32]
     lib.ufo_b200_update_nodes.argtypes = [vp, vp, vp, vp, vp, sz, i32]
+    lib.ufo_b200_update_nodes_color.argtypes = [vp, vp, vp, vp, vp, vp, sz, i32]
     lib.ufo_b200_insert_rays.argtypes = [vp, vp, vp, sz, dbl, u32, i32, i32]
     lib.ufo_b200_write_data.argtypes = [vp, vp, u32, vp, sz, C.POINTER(sz)]
     lib.ufo_b200_transform_points.argtypes = [vp, vp, sz, i32, vp]
@@ -574,6 +575,25 @@ class Map:
         v = np.ascontiguousarray(np.broadcast_to(values, (n,)), dtype=np.float32)
         self._check(self.lib.ufo_b200_update_nodes(self.h, c.ctypes.data, d.ctypes.data, o.ctypes.data,
                                                    v.ctypes.data, n, int(async_)))
+
+    ADD_COLOR, SET_COLOR = 2, 3
+
+    def update_nodes_color(self, codes, depths, ops, values, rgb, async_=False):
+        """update_nodes plus the colour map's writers, one ordered batch: op 2 blends rgb[i] into the
+        voxel's colour and then adds values[i] (updateValue(code, value, Color)), op 3 sets the
+        colour (setColor); both at depth 0.  rgb: [n][3] uint8 or one colour, or None for a batch
+        without ops 2 and 3."""
+        c = np.ascontiguousarray(codes, dtype=np.uint64).reshape(-1)
+        n = len(c)
+        d = np.ascontiguousarray(np.broadcast_to(depths, (n,)), dtype=np.uint32)
+        o = np.ascontiguousarray(np.broadcast_to(ops, (n,)), dtype=np.uint8)
+        v = np.ascontiguousarray(np.broadcast_to(values, (n,)), dtype=np.float32)
+        col = None
+        if rgb is not None:
+            col = np.ascontiguousarray(np.broadcast_to(np.asarray(rgb, np.uint8).reshape(-1, 3), (n, 3)))
+        self._check(self.lib.ufo_b200_update_nodes_color(self.h, c.ctypes.data, d.ctypes.data, o.ctypes.data,
+                                                         v.ctypes.data, None if col is None else col.ctypes.data,
+                                                         n, int(async_)))
 
     def insert_rays(self, origins, ends, max_range=-1.0, depth=0, hit_end=False, async_=False):
         """insertMissOnRay (hit_end=False) / insertRay (hit_end=True) for every (origin, end)."""

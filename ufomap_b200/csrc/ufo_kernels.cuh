@@ -500,12 +500,14 @@ __global__ void __launch_bounds__(256) k_points(DeviceMap M, ScanArgs a)
 }
 
 // updateNodeColor (occupancy_map_color.cpp:142-171): the colour of a leaf of colour `cur` and
-// log-odds `occ` after a hit of colour `upd`
-__device__ __forceinline__ uint32_t blended_color(const DeviceMap& M, uint32_t cur, uint32_t upd, float occ)
+// log-odds `occ` after an update of colour `upd` with hit probability `prob` (toProb of the
+// update's log-odds; M.prob_hit for a scan's hits).  `hit` is taken by reference so that it is
+// only read past the two early returns, as the scans' blends always did.
+__device__ __forceinline__ uint32_t blended_color(uint32_t cur, uint32_t upd, const double& hit, float occ)
 {
 	if (cur == upd) return cur;
 	if (cur == 0) return upd;
-	double prob = M.prob_hit;
+	double prob = hit;
 	double total = prob + to_prob(occ);
 	prob = prob / total;
 	double inv = 1.0 - prob;
@@ -523,7 +525,7 @@ __device__ __forceinline__ void blend_color(const DeviceMap& M, size_t li, uint3
 {
 	uint32_t cur = M.leaf_rgb[li];
 	if (cur == upd) return;
-	M.leaf_rgb[li] = blended_color(M, cur, upd, M.leaf[li]);
+	M.leaf_rgb[li] = blended_color(cur, upd, M.prob_hit, M.leaf[li]);
 }
 
 // slot of `key` in the scan-local table, kNone when absent
@@ -643,7 +645,7 @@ __global__ void __launch_bounds__(256) k_wrapped_colors(DeviceMap M, ScanArgs a)
 		Vec3 p;
 		uint32_t upd;
 		load_point(a, idx[x], p, upd);
-		rgb = blended_color(M, rgb, upd, occ);
+		rgb = blended_color(rgb, upd, M.prob_hit, occ);
 		occ = apply_update(M, occ, M.hit);
 	}
 	M.leaf_rgb[tl] = rgb;

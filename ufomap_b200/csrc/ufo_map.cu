@@ -919,7 +919,8 @@ void enqueue_write(Map* m, PendingScan& p)
 	a.idx = m->d_w_idx[1];
 	k_write_segments<<<m->sm_count * 8, 256, 0, s>>>(M, a);
 	CK(cudaEventRecord(m->ev[3], s));
-	k_write_apply<<<m->sm_count * 16, 64, 0, s>>>(M, a);
+	if (a.rgb) k_write_apply<true><<<m->sm_count * 16, 64, 0, s>>>(M, a);
+	else k_write_apply<false><<<m->sm_count * 16, 64, 0, s>>>(M, a);
 	CK(cudaEventRecord(m->ev[5], s));
 	k_import_refresh<<<m->sm_count * 8, 256, 0, s>>>(M);
 	if (M.color) k_brick_agg<true><<<m->sm_count * 4, 256, 0, s>>>(M);
@@ -3958,18 +3959,18 @@ int do_write(Map* m, WriteArgs w, const std::vector<std::pair<const void*, size_
 	if (!async) return sync_map(m);
 	return UFO_B200_OK;
 }
-}  // namespace
 
-extern "C" {
-
-int ufo_b200_update_nodes(ufo_b200_map* m, const uint64_t* codes, const uint32_t* depths, const uint8_t* ops,
-                          const float* values, size_t n, int async)
+bool code_in_map(const Geometry& g, uint64_t code, uint32_t d)
 {
-	if (!m || (n && (!codes || !depths || !ops || !values)) || n > 0x7fffffffull) return UFO_B200_E_INVALID;
-	for (size_t i = 0; i < n; ++i) {
-		const int rc = write_allowed(m, depths[i]);
-		if (rc != UFO_B200_OK) return rc;
-	}
+	const Key3 k = code_to_key(code);
+	return !((((k.x >> d) << d) | ((k.y >> d) << d) | ((k.z >> d) << d)) & ~g.key_mask);
+}
+
+// The body of ufo_b200_update_nodes (rgb == NULL) and of ufo_b200_update_nodes_color for a batch
+// that holds a colour op (rgb != NULL, every entry already checked).
+int write_nodes(Map* m, const uint64_t* codes, const uint32_t* depths, const uint8_t* ops, const float* values,
+                const uint8_t* rgb, size_t n, int async)
+{
 	return guarded(m, [&]() {
 		CK(cudaSetDevice(m->device));
 		const Geometry& g = m->M.g;
@@ -3977,7 +3978,7 @@ int ufo_b200_update_nodes(ufo_b200_map* m, const uint64_t* codes, const uint32_t
 		unsigned long long tot = 0;
 		for (size_t i = 0; i < n; ++i) {
 			const uint32_t d = depths[i];
-			if (ops[i] > 1) {
+			if (ops[i] > (rgb ? 3 : 1)) {
 				m->set_error("entry %zu: op %u is neither ADD (0) nor SET (1)", i, (unsigned)ops[i]);
 				return (int)UFO_B200_E_INVALID;
 			}
@@ -3985,8 +3986,7 @@ int ufo_b200_update_nodes(ufo_b200_map* m, const uint64_t* codes, const uint32_t
 				m->set_error("SET on a colour map is supported at depth 0 only");
 				return (int)UFO_B200_E_UNSUPPORTED;
 			}
-			const Key3 k = code_to_key(codes[i]);
-			if ((((k.x >> d) << d) | ((k.y >> d) << d) | ((k.z >> d) << d)) & ~g.key_mask) {
+			if (!code_in_map(g, codes[i], d)) {
 				m->set_error("entry %zu: code %llu lies outside the map", i, (unsigned long long)codes[i]);
 				return (int)UFO_B200_E_INVALID;
 			}
@@ -4000,14 +4000,71 @@ int ufo_b200_update_nodes(ufo_b200_map* m, const uint64_t* codes, const uint32_t
 		}
 		WriteArgs w{};
 		w.n = (uint32_t)n;
-		return do_write(m, w, {{codes, n * 8}, {values, n * 4}, {depths, n * 4}, {ops, n}}, offs, async,
-		                [](WriteArgs& a, const std::vector<const void*>& p) {
-			                a.codes = static_cast<const unsigned long long*>(p[0]);
-			                a.values = static_cast<const float*>(p[1]);
-			                a.depths = static_cast<const uint32_t*>(p[2]);
-			                a.ops = static_cast<const uint8_t*>(p[3]);
-		                });
+		std::vector<std::pair<const void*, size_t>> blobs = {{codes, n * 8}, {values, n * 4}, {depths, n * 4}, {ops, n}};
+		if (rgb) blobs.push_back({rgb, n * 3});
+		return do_write(m, w, blobs, offs, async, [](WriteArgs& a, const std::vector<const void*>& p) {
+			a.codes = static_cast<const unsigned long long*>(p[0]);
+			a.values = static_cast<const float*>(p[1]);
+			a.depths = static_cast<const uint32_t*>(p[2]);
+			a.ops = static_cast<const uint8_t*>(p[3]);
+			a.rgb = p.size() > 4 ? static_cast<const uint8_t*>(p[4]) : nullptr;
+		});
 	});
+}
+}  // namespace
+
+extern "C" {
+
+int ufo_b200_update_nodes(ufo_b200_map* m, const uint64_t* codes, const uint32_t* depths, const uint8_t* ops,
+                          const float* values, size_t n, int async)
+{
+	if (!m || (n && (!codes || !depths || !ops || !values)) || n > 0x7fffffffull) return UFO_B200_E_INVALID;
+	for (size_t i = 0; i < n; ++i) {
+		const int rc = write_allowed(m, depths[i]);
+		if (rc != UFO_B200_OK) return rc;
+	}
+	return write_nodes(m, codes, depths, ops, values, nullptr, n, async);
+}
+
+int ufo_b200_update_nodes_color(ufo_b200_map* m, const uint64_t* codes, const uint32_t* depths, const uint8_t* ops,
+                                const float* values, const uint8_t* rgb, size_t n, int async)
+{
+	if (!m || (n && (!codes || !depths || !ops || !values)) || n > 0x7fffffffull) return UFO_B200_E_INVALID;
+	// every check runs on the host before any device work, so a rejected batch applies nothing
+	bool has_color = false;
+	for (size_t i = 0; i < n; ++i) {
+		const uint32_t d = depths[i];
+		if (ops[i] > 3) {
+			m->set_error("entry %zu: op %u is not ADD (0), SET (1), ADD_COLOR (2) or SET_COLOR (3)", i, (unsigned)ops[i]);
+			return UFO_B200_E_INVALID;
+		}
+		if (ops[i] >= 2 && !m->params.color) {
+			m->set_error("entry %zu: colour op %u on a map without colour", i, (unsigned)ops[i]);
+			return UFO_B200_E_INVALID;
+		}
+		const int rc = write_allowed(m, d);
+		if (rc != UFO_B200_OK) return rc;
+		if (!code_in_map(m->M.g, codes[i], d)) {
+			m->set_error("entry %zu: code %llu lies outside the map", i, (unsigned long long)codes[i]);
+			return UFO_B200_E_INVALID;
+		}
+		if (ops[i] >= 2 && d > 0) {
+			// the reference's result depends on whether the node has children, which the value
+			// field does not record (DESIGN.md section 8)
+			m->set_error("entry %zu: colour ops are supported at depth 0 only", i);
+			return UFO_B200_E_UNSUPPORTED;
+		}
+		if (ops[i] == 1 && d > 0 && m->params.color) {
+			m->set_error("SET on a colour map is supported at depth 0 only");
+			return UFO_B200_E_UNSUPPORTED;
+		}
+		has_color |= ops[i] >= 2;
+	}
+	if (has_color && !rgb) {
+		m->set_error("the batch holds a colour op but rgb is NULL");
+		return UFO_B200_E_INVALID;
+	}
+	return write_nodes(m, codes, depths, ops, values, has_color ? rgb : nullptr, n, async);
 }
 
 int ufo_b200_insert_rays(ufo_b200_map* m, const double* origins, const double* ends, size_t n, double max_range,

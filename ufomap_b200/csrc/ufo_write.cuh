@@ -15,22 +15,29 @@
 //      its block to its voxels.
 // The depth 1-4 aggregates are then rebuilt from the leaves (k_import_refresh, k_brick_agg) and the
 // usual propagation pass runs.
+//
+// Colour maps add two depth-0 ops (ufo_b200_update_nodes_color): ADD_COLOR, the colour map's
+// updateValue(code, value, Color) (occupancy_map_color.h:269-287), and SET_COLOR, setColor(code,
+// Color) (occupancy_map_color.cpp:74-81).  Their colour rides in the record's op word, and only a
+// batch holding one runs the colour variant of phase 3.
 #pragma once
 
 #include "ufo_import.cuh"
 
 namespace ufo_b200
 {
-constexpr uint32_t kWriteAdd = 0, kWriteSet = 1;
+constexpr uint32_t kWriteAdd = 0, kWriteSet = 1, kWriteAddColor = 2, kWriteSetColor = 3;
 constexpr unsigned long long kWritePad = ~0ull;  // key of an unused record slot (sorts last)
 
 // what one record does inside its brick: every voxel of vmask (Morton order, bit j = leaf[j]) in
-// every block of bmask (Morton child index of the block) takes the update
+// every block of bmask (Morton child index of the block) takes the update.  op: bits 0-7 the op,
+// bits 8-31 the colour of a colour op (r | g << 8 | b << 16, the leaf_rgb layout)
 struct WriteRec {
 	unsigned long long bmask, vmask;
 	float value;
 	uint32_t op;
 };
+static_assert(sizeof(WriteRec) == 24, "write records stay 24 bytes");
 
 struct WriteArgs {
 	uint32_t n;       // entries or rays
@@ -40,6 +47,7 @@ struct WriteArgs {
 	const uint32_t* depths;
 	const uint8_t* ops;
 	const float* values;
+	const uint8_t* rgb;  // [n][3]; set only when the batch holds a colour op
 	// rays: origins / ends [n][3]
 	const double* origins;
 	const double* ends;
@@ -126,7 +134,12 @@ __global__ void __launch_bounds__(128) k_write_expand(DeviceMap M, WriteArgs a)
 		const uint32_t d = a.depths[i];
 		const Key3 c = code_to_key(a.codes[i]);
 		const Key3 k = {(c.x >> d) << d, (c.y >> d) << d, (c.z >> d) << d};
-		at = put_node(M, a, at, i, k, d, a.values[i], a.ops[i] ? kWriteSet : kWriteAdd);
+		uint32_t op = a.ops[i];
+		if (a.rgb && op >= kWriteAddColor) {
+			const uint8_t* c3 = a.rgb + 3 * (size_t)i;
+			op |= ((uint32_t)c3[0] | ((uint32_t)c3[1] << 8) | ((uint32_t)c3[2] << 16)) << 8;
+		}
+		at = put_node(M, a, at, i, k, d, a.values[i], op);
 	} else {
 		// the walk of ufo_b200_compute_ray (Octree::computeRay, octree.h:449-496)
 		const uint32_t d = a.depth;
@@ -223,9 +236,15 @@ constexpr uint32_t kWriteChunk = 64;
 // memory the first time a record covers it, applies every covering record in sequence order
 // (float add + clamp, or clamp of the set value, one clamp per update), and writes back the block,
 // its octet "initialised" bits and the voxels whose value changed at some update.
+// COLOR (batches with a colour op): the block's 64 leaf colours are loaded into shared memory too,
+// at the first colour record that covers it, and written back at the end.  ADD_COLOR blends with
+// the log-odds the earlier records left, before its own add; SET_COLOR replaces the colour.  Both
+// initialise the voxel's octet; only a log-odds change enters the change mask.
+template <bool COLOR>
 __global__ void __launch_bounds__(64) k_write_apply(DeviceMap M, WriteArgs a)
 {
 	__shared__ float s_v[64][68];
+	__shared__ __align__(16) uint32_t s_c[COLOR ? 64 : 1][68];
 	__shared__ unsigned long long s_bm[kWriteChunk], s_vm[kWriteChunk];
 	__shared__ float s_val[kWriteChunk];
 	__shared__ uint32_t s_op[kWriteChunk];
@@ -240,6 +259,8 @@ __global__ void __launch_bounds__(64) k_write_apply(DeviceMap M, WriteArgs a)
 		const size_t b = (size_t)brick * 64 + t;
 		float* leaf = M.leaf + b * 64;
 		float* v = s_v[t];
+		uint32_t* col = s_c[COLOR ? t : 0];
+		bool col_loaded = false;
 		unsigned long long written = 0, changed = 0;
 		for (uint32_t c0 = begin; c0 < end; c0 += kWriteChunk) {
 			__syncthreads();
@@ -261,6 +282,32 @@ __global__ void __launch_bounds__(64) k_write_apply(DeviceMap M, WriteArgs a)
 				}
 				unsigned long long vm = s_vm[r];
 				const float u = s_val[r];
+				if (COLOR && (s_op[r] & 0xffu) >= kWriteAddColor) {
+					if (!col_loaded) {
+						const uint4* cp = reinterpret_cast<const uint4*>(M.leaf_rgb + b * 64);
+#pragma unroll
+						for (int q = 0; q < 16; ++q) reinterpret_cast<uint4*>(col)[q] = cp[q];
+						col_loaded = true;
+					}
+					const uint32_t rgb = s_op[r] >> 8;
+					const bool add = (s_op[r] & 0xffu) == kWriteAddColor;
+					const double prob = add ? to_prob(u) : 0.0;
+					written |= vm;
+					while (vm) {
+						const uint32_t j = __ffsll((long long)vm) - 1;
+						vm &= vm - 1;
+						if (!add) {
+							col[j] = rgb;
+							continue;
+						}
+						const float old = v[j];
+						col[j] = blended_color(col[j], rgb, prob, old);
+						const float nv = apply_update(M, old, u);
+						changed |= (unsigned long long)(__float_as_uint(nv) != __float_as_uint(old)) << j;
+						v[j] = nv;
+					}
+					continue;
+				}
 				const bool set = s_op[r] == kWriteSet;
 				written |= vm;
 				while (vm) {
@@ -277,6 +324,11 @@ __global__ void __launch_bounds__(64) k_write_apply(DeviceMap M, WriteArgs a)
 			float4* lp = reinterpret_cast<float4*>(leaf);
 #pragma unroll
 			for (int q = 0; q < 16; ++q) lp[q] = reinterpret_cast<const float4*>(v)[q];
+			if (COLOR && col_loaded) {
+				uint4* cp = reinterpret_cast<uint4*>(M.leaf_rgb + b * 64);
+#pragma unroll
+				for (int q = 0; q < 16; ++q) cp[q] = reinterpret_cast<const uint4*>(col)[q];
+			}
 			uint32_t init = 0;
 #pragma unroll
 			for (uint32_t o = 0; o < 8; ++o) init |= ((written >> (8 * o)) & 0xffull) ? (1u << (16 + o)) : 0u;
