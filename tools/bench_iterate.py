@@ -7,7 +7,8 @@ JSON line per case.
 * map:    config #2 holds one full scan, config #4 two (bench.py's scan streams).
 * cases:  beginLeaves() over the whole map at min_depth 0 (occupied + free), and the RViz plugin's
           call -- beginLeaves(AABB, occupied, free, unknown = false, contains = false, min_depth) -- over
-          a 20 m box around the sensor at min_depth 0 and 4.
+          a 20 m box around the sensor at min_depth 0, 1, 2 and 4 (depth 1 values are the max of the
+          octet's leaf sector, depth 2 values the max of the block's pair maxima).
 * times:  device time of the size pass and of the emit pass (the two k_brick_iter launches of a call)
           and of the call's device-to-host copies, from torch.profiler's CUDA activity records; medians
           over the steps.  wall_ms: the whole call on the host clock.
@@ -102,7 +103,8 @@ def main():
     name, limit = card_info()
     o = np.asarray(origins[0], np.float64)
     box = [capi.aabb(o - 10.0, o + 10.0)]
-    for label, vol, md in (("whole map", [], 0), ("RViz box 20 m", box, 0), ("RViz box 20 m", box, 4)):
+    for label, vol, md in (("whole map", [], 0), ("RViz box 20 m", box, 0), ("RViz box 20 m", box, 1),
+                          ("RViz box 20 m", box, 2), ("RViz box 20 m", box, 4)):
         cnt, t = run_case(m, vol, md, args.steps, args.warmup)
         line = {"tool": "bench_iterate", "config": args.config, "case": "beginLeaves(%s, occupied, free, min_depth=%d)" % (label, md),
                 "records": cnt, "bricks": n_bricks, **t,

@@ -15,7 +15,10 @@
 // has touched octets in ONE of its two 128 B lines with probability 0.86, in both otherwise
 // (touched_lines / D_2 = 1.14), and 81 % of the 4 octets of a touched line are touched
 // (D_1 / touched_lines = 3.2); k3_all adds, per brick, the depth-1 sector of every marked block
-// (own region), the mask / meta slab (1280 B) and the depth-2 aggregates (512 B).
+// (own region), the mask / meta slab (1280 B) and the depth-2 aggregates (512 B) -- the metadata of
+// the layout with per-octet maxima; k3_pairs is today's layout: the leaf sectors, the untouched
+// partner (2k, 2k+1) of every touched octet (read-modify-written here, only read by K3: an upper
+// bound), the mask / meta slab and the brick's pair maxima (1 KB).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -128,12 +131,13 @@ int main(int argc, char** argv)
 	{
 		const double pb = argc > 3 ? atof(argv[3]) : 0.53, p_both = argc > 4 ? atof(argv[4]) : 0.14, po = argc > 5 ? atof(argv[5]) : 0.81;
 		std::uniform_real_distribution<double> uni(0.0, 1.0);
-		// regions inside the pool, in 32 B sectors: leaves [0, T*512), depth-1 [T*512, T*576), slab + depth-2 [T*576, T*632)
-		const uint32_t T = std::min(touched, (uint32_t)((size_t)pool_bricks * 512 / 632));
+		// regions inside the pool, in 32 B sectors: leaves [0, T*512), depth-1 [T*512, T*576), slab + depth-2
+		// [T*576, T*632); k3_pairs: slab + pair maxima [T*576, T*648)
+		const uint32_t T = std::min(touched, (uint32_t)((size_t)pool_bricks * 512 / 648));
 		std::vector<uint32_t> pt(T);
 		for (uint32_t i = 0; i < T; ++i) pt[i] = i;
 		std::shuffle(pt.begin(), pt.end(), rng);
-		for (int all = 0; all < 2; ++all) {
+		for (int all = 0; all < 3; ++all) {  // k3_leaf, k3_all, k3_pairs
 			std::vector<uint32_t> list;
 			size_t leaf_sectors = 0, lines = 0;
 			for (uint32_t t = 0; t < T; ++t) {
@@ -151,14 +155,17 @@ int main(int argc, char** argv)
 						if (!l4) l4 = 1u << (blk & 3);
 						t8 |= l4 << (4 * h);
 					}
+					const uint32_t ld = all == 2 ? t8 | ((t8 & 0x55u) << 1) | ((t8 & 0xaau) >> 1) : t8;
 					for (uint32_t o = 0; o < 8; ++o)
-						if ((t8 >> o) & 1u) list.push_back(brick * 512u + blk * 8u + o);
+						if ((ld >> o) & 1u) list.push_back(brick * 512u + blk * 8u + o);
 					leaf_sectors += __builtin_popcount(t8);
 					lines += ((t8 & 0x0f) ? 1 : 0) + ((t8 & 0xf0) ? 1 : 0);
-					if (all) list.push_back(T * 512u + brick * 64u + blk);
+					if (all == 1) list.push_back(T * 512u + brick * 64u + blk);
 				}
-				if (all)
+				if (all == 1)
 					for (uint32_t q = 0; q < 56; ++q) list.push_back(T * 576u + brick * 56u + q);
+				if (all == 2)
+					for (uint32_t q = 0; q < 72; ++q) list.push_back(T * 576u + brick * 72u + q);
 			}
 			const uint32_t n = (uint32_t)list.size();
 			uint32_t* dl;
@@ -175,7 +182,7 @@ int main(int argc, char** argv)
 				if (rep >= 1) best = std::min(best, ms);
 			}
 			printf("{\"pattern\": \"%s\", \"bricks\": %u, \"p_block\": %.2f, \"p_both_lines\": %.2f, \"p_octet_in_line\": %.2f, \"sectors\": %u, \"leaf_sectors\": %zu, \"leaf_lines_128B\": %zu, \"ms\": %.4f, \"GBps\": %.1f}\n",
-			       all ? "k3_all" : "k3_leaf", T, pb, p_both, po, n, leaf_sectors, lines, best, (double)n * 64.0 / (best * 1e-3) / 1e9);
+			       all == 2 ? "k3_pairs" : all ? "k3_all" : "k3_leaf", T, pb, p_both, po, n, leaf_sectors, lines, best, (double)n * 64.0 / (best * 1e-3) / 1e9);
 			CK(cudaFree(dl));
 		}
 	}

@@ -149,9 +149,11 @@ struct DeviceMap {
 	unsigned long long* miss_mask;  // [b] per-scan free-set bits, linear order x + 4y + 16z
 	unsigned long long* hit_mask;   // [b] per-scan hit bits
 	unsigned long long* chg_mask;   // [b] voxels changed since the last reset (allocated by enableChangeDetection)
-	Agg* agg2;                      // [b] depth-2 aggregate
 	uint32_t* meta;                 // [b] bits 0..15: flags of the 8 octets, bits 16..23: octet initialised
-	float* sum1;                    // [b][8] depth-1 maxima
+	// [b] pair maxima: component k = max of the depth-1 nodes (octets) 2k and 2k+1, an uninitialised
+	// octet counting as 0.0.  The depth-2 value is their max (block_occ), the depth-2 flags follow
+	// from meta (block_flags), a depth-1 value is the max of the octet's 32 B leaf sector (octet_occ).
+	float4* pair_max;
 	uint32_t* rgb2;                 // colour maps: [b]
 	uint32_t* sum1_rgb;             // colour maps: [b][8]
 	// Keys outside [0, 2^L) (a coordinate exactly on the + face of the map, or a walk that
@@ -433,6 +435,23 @@ __device__ __forceinline__ uint32_t leaf_flags(const DeviceMap& M, float v)
 {
 	uint32_t f = (v < M.free_ceil) ? 1u : 0u;
 	if (v >= M.free_ceil && v <= M.occ_floor) f |= 2u;
+	return f;
+}
+
+// depth-1 value of an initialised octet: the max of its eight leaves (one 32 B sector)
+__device__ __forceinline__ float octet_occ(const float* lp)
+{
+	const float4 a = reinterpret_cast<const float4*>(lp)[0], c = reinterpret_cast<const float4*>(lp)[1];
+	return fmaxf(fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w)), fmaxf(fmaxf(c.x, c.y), fmaxf(c.z, c.w)));
+}
+// depth-2 value of a block from its pair maxima
+__device__ __forceinline__ float block_occ(float4 q) { return fmaxf(fmaxf(q.x, q.y), fmaxf(q.z, q.w)); }
+// depth-2 flags of a block from its meta word: an uninitialised octet is unknown space
+__device__ __forceinline__ uint32_t block_flags(const DeviceMap& M, uint32_t mt)
+{
+	uint32_t f = 0;
+#pragma unroll
+	for (uint32_t o = 0; o < 8; ++o) f |= ((mt >> (16 + o)) & 1u) ? (mt >> (2 * o)) & 3u : M.default_flags;
 	return f;
 }
 

@@ -110,7 +110,7 @@ __device__ __forceinline__ uint32_t octet_record(const DeviceMap& M, size_t b, u
 		return n;
 	}
 	if (dst) {
-		if (has) put_payload<COLOR>(dst, M.sum1[b * 8 + o], COLOR ? M.sum1_rgb[b * 8 + o] : 0u);
+		if (has) put_payload<COLOR>(dst, octet_occ(M.leaf + b * 64 + 8 * o), COLOR ? M.sum1_rgb[b * 8 + o] : 0u);
 		else put_payload<COLOR>(dst, leaf_occ, leaf_rgb);
 	}
 	return P;
@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 	s_blk_has[t] = blk_has ? 1 : 0;
 	s_blk_size[t] = blk_size;
 	// payload when the block is written as a leaf: its value, or its depth-2 aggregate
-	s_blk_occ[t] = blk_has ? M.agg2[b].occ : oocc[0];
+	s_blk_occ[t] = blk_has ? block_occ(M.pair_max[b]) : oocc[0];
 	s_blk_rgb[t] = blk_has ? (COLOR ? M.rgb2[b] : 0u) : orgb[0];
 	__syncthreads();
 	if (t < 8) {
@@ -364,7 +364,7 @@ __device__ __forceinline__ uint32_t block_records(const DeviceMap& M, const Iter
                                                   bool blk_has, float blk_v, uint32_t blk_rgb, const double blkc[3],
                                                   unsigned long long code, IterRec* dst)
 {
-	const uint32_t blk_fl = (meta >> 16) ? M.agg2[b].flags : M.default_flags;
+	const uint32_t blk_fl = (meta >> 16) ? block_flags(M, meta) : M.default_flags;
 	uint32_t n = 0;
 	bool ret;
 	if (!iter_visit<G>(a, blkc, M.g.half_size[2], 2, blk_v, blk_fl, !blk_has, &ret)) return 0;
@@ -375,7 +375,7 @@ __device__ __forceinline__ uint32_t block_records(const DeviceMap& M, const Iter
 	if (a.min_depth >= 2 || !blk_has) return n;
 	for (uint32_t o = 0; o < 8; ++o) {
 		const bool oi = (meta >> (16 + o)) & 1u, oh = (oct_has >> o) & 1u;
-		const float ov = oh ? M.sum1[b * 8 + o] : oocc[o];
+		const float ov = oh ? octet_occ(M.leaf + b * 64 + 8 * o) : oocc[o];
 		const uint32_t orv = oh ? (COLOR ? M.sum1_rgb[b * 8 + o] : 0u) : orgb[o];
 		const uint32_t ofl = oi ? (meta >> (2 * o)) & 3u : M.default_flags;
 		const unsigned long long ocode = code | ((unsigned long long)o << 3);
@@ -442,7 +442,7 @@ __global__ void __launch_bounds__(64) k_brick_iter(DeviceMap M, uint32_t n_brick
 		}
 	}
 	const bool blk_has = keeps_children(oct_has != 0, oocc, orgb);
-	const float blk_v = blk_has ? M.agg2[b].occ : oocc[0];
+	const float blk_v = blk_has ? block_occ(M.pair_max[b]) : oocc[0];
 	const uint32_t blk_rgb = blk_has ? (COLOR ? M.rgb2[b] : 0u) : orgb[0];
 	s_blk_has[t] = blk_has ? 1 : 0;
 	s_blk_occ[t] = blk_v;
@@ -640,7 +640,7 @@ __global__ void __launch_bounds__(256) k_export_nodes(DeviceMap M, uint32_t n_br
 	const uint32_t meta = M.meta[blk];
 	const bool init = (meta >> 16) != 0;
 	if (d == 2) {
-		node_emit<CHAIN>(M, f, x0, y0, z0, init ? M.agg2[blk].occ : 0.0f, (init && M.color) ? M.rgb2[blk] : 0u, codes, occ, rgbs, cap, count);
+		node_emit<CHAIN>(M, f, x0, y0, z0, init ? block_occ(M.pair_max[blk]) : 0.0f, (init && M.color) ? M.rgb2[blk] : 0u, codes, occ, rgbs, cap, count);
 		return;
 	}
 	for (uint32_t o = 0; o < 8; ++o) {
@@ -652,7 +652,7 @@ __global__ void __launch_bounds__(256) k_export_nodes(DeviceMap M, uint32_t n_br
 			if (!vol_hits_t<true>(f.vol, oc, M.g.half_size[1])) continue;
 		}
 		if (d == 1) {
-			node_emit<CHAIN>(M, f, ox, oy, oz, oi ? M.sum1[blk * 8 + o] : 0.0f, (oi && M.color) ? M.sum1_rgb[blk * 8 + o] : 0u, codes, occ, rgbs,
+			node_emit<CHAIN>(M, f, ox, oy, oz, oi ? octet_occ(M.leaf + blk * 64 + 8 * o) : 0.0f, (oi && M.color) ? M.sum1_rgb[blk * 8 + o] : 0u, codes, occ, rgbs,
 			          cap, count);
 			continue;
 		}

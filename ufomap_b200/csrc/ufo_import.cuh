@@ -111,8 +111,8 @@ __global__ void __launch_bounds__(256) k_import_wipe(DeviceMap M, uint32_t n_bri
 	}
 }
 
-// depth-1 / depth-2 aggregates of every block of the touched bricks from the leaves (initialised
-// octets only), colours included; one thread per (touched brick, block)
+// pair maxima, octet flags and depth-1 / depth-2 colours of every block of the touched bricks from
+// the leaves (initialised octets only); one thread per (touched brick, block)
 __global__ void __launch_bounds__(256) k_import_refresh(DeviceMap M)
 {
 	if (__ldg(&M.ctr->overflow) & ~4u) return;
@@ -122,32 +122,24 @@ __global__ void __launch_bounds__(256) k_import_refresh(DeviceMap M)
 		const uint32_t mt = M.meta[b];
 		if (!(mt & 0xff0000u)) continue;
 		const float* leaf = M.leaf + b * 64;
-		float bmax = -3.402823466e+38f;
-		uint32_t bfl = 0, fl16 = 0;
+		float om[8];
+		uint32_t fl16 = 0;
 		uint32_t oc[8];
 		for (uint32_t o = 0; o < 8; ++o) {
-			float om = 0.0f;
-			uint32_t ofl = M.default_flags;
+			om[o] = 0.0f;
 			oc[o] = 0;
 			if ((mt >> (16 + o)) & 1u) {
-				om = -3.402823466e+38f;
-				ofl = 0;
-				for (int j = 0; j < 8; ++j) {
-					const float v = leaf[8 * o + j];
-					om = fmaxf(om, v);
-					ofl |= leaf_flags(M, v);
-				}
-				M.sum1[b * 8 + o] = om;
+				om[o] = octet_occ(leaf + 8 * o);
+				uint32_t ofl = 0;
+				for (int j = 0; j < 8; ++j) ofl |= leaf_flags(M, leaf[8 * o + j]);
 				fl16 |= ofl << (2 * o);
 				if (M.color) {
 					oc[o] = rms_rgb(M.leaf_rgb + b * 64 + 8 * o, 8);
 					M.sum1_rgb[b * 8 + o] = oc[o];
 				}
 			}
-			bmax = fmaxf(bmax, om);
-			bfl |= ofl;
 		}
-		M.agg2[b] = {bmax, bfl};
+		M.pair_max[b] = make_float4(fmaxf(om[0], om[1]), fmaxf(om[2], om[3]), fmaxf(om[4], om[5]), fmaxf(om[6], om[7]));
 		if (M.color) M.rgb2[b] = rms_rgb(oc, 8);
 		M.meta[b] = (mt & 0xff0000u) | fl16 | (M.scan_id << 24);
 	}

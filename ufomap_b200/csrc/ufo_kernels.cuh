@@ -1148,8 +1148,8 @@ __global__ void __launch_bounds__(256) k_alias_refresh(DeviceMap M)
 		if (dst == kNone) continue;
 		const size_t tb = (size_t)dst * 64 + (b & 63);
 		const float* leaf = M.leaf + tb * 64;
-		float bmax = -3.402823466e+38f;
-		uint32_t bfl = 0, meta = 0;
+		float om[8];
+		uint32_t meta = 0;
 		for (int o = 0; o < 8; ++o) {
 			float omax = -3.402823466e+38f;
 			uint32_t ofl = 0;
@@ -1158,13 +1158,11 @@ __global__ void __launch_bounds__(256) k_alias_refresh(DeviceMap M)
 				omax = fmaxf(omax, v);
 				ofl |= leaf_flags(M, v);
 			}
-			M.sum1[tb * 8 + o] = omax;
-			bmax = fmaxf(bmax, omax);
-			bfl |= ofl;
+			om[o] = omax;
 			meta |= ofl << (2 * o);
 		}
 		// every octet now holds real values; several sources refreshing one target write the same
-		M.agg2[tb] = {bmax, bfl};
+		M.pair_max[tb] = make_float4(fmaxf(om[0], om[1]), fmaxf(om[2], om[3]), fmaxf(om[4], om[5]), fmaxf(om[6], om[7]));
 		M.meta[tb] = meta | 0xff0000u | (M.scan_id << 24);
 		if (M.color) {
 			// the wrapped leaves' colours changed too (k_wrapped_colors): depth 1 and 2 colours
@@ -1486,13 +1484,13 @@ __device__ __forceinline__ void node_value(const DeviceMap& M, Key3 k, uint32_t 
 		const uint32_t meta = M.meta[slot];
 		if (!(meta >> 16)) return;
 		if (d == 2) {
-			o = M.agg2[slot].occ;
-			f = M.agg2[slot].flags;
+			o = block_occ(M.pair_max[slot]);
+			f = block_flags(M, meta);
 			if (M.color) c = M.rgb2[slot];
 		} else if (d == 1) {
 			uint32_t j = ((k.x >> 1) & 1u) | (((k.y >> 1) & 1u) << 1) | (((k.z >> 1) & 1u) << 2);
 			if ((meta >> (16 + j)) & 1u) {
-				o = M.sum1[slot * 8 + j];
+				o = octet_occ(M.leaf + slot * 64 + 8 * j);
 				f = (meta >> (2 * j)) & 3u;
 				if (M.color) c = M.sum1_rgb[slot * 8 + j];
 			}

@@ -278,9 +278,8 @@ void alloc_pools(Map* m, uint32_t brick_cap, uint32_t up_cap)
 	dev_alloc(M.leaf, nb * 64, 0, s, tot);
 	dev_alloc(M.miss_mask, nb, 0, s, tot);
 	dev_alloc(M.hit_mask, nb, 0, s, tot);
-	dev_alloc(M.agg2, nb, 0, s, tot);
 	dev_alloc(M.meta, nb, 0, s, tot);
-	dev_alloc(M.sum1, nb * 8, 0, s, tot);
+	dev_alloc(M.pair_max, nb, 0, s, tot);
 	dev_alloc(M.uh_keys, (size_t)M.uh_mask + 1, 0xff, s, tot);
 	dev_alloc(M.uh_vals, (size_t)M.uh_mask + 1, 0xff, s, tot);
 	dev_alloc(M.up_key, up_cap, 0, s, tot);
@@ -308,7 +307,7 @@ void free_pools(Map* m)
 {
 	DeviceMap& M = m->M;
 	void* ptrs[] = {M.bh_tab, M.brick_key, M.brick_stamp, M.touched, M.touched_alt, M.touched_mi, M.touched_alt_mi, M.chg_mask, M.vol, M.vol_dirty, M.vol_list, M.route, m->route_inbox, M.brick_sum3, M.brick_sum4, M.brick_rgb3, M.brick_rgb4,
-	                M.leaf, M.leaf_rgb, M.miss_mask, M.hit_mask, M.agg2, M.meta, M.sum1, M.rgb2, M.sum1_rgb,
+	                M.leaf, M.leaf_rgb, M.miss_mask, M.hit_mask, M.meta, M.pair_max, M.rgb2, M.sum1_rgb,
 	                M.alias_miss, M.alias_hit, M.uh_keys, M.uh_vals, M.up_key, M.up_agg, M.up_rgb, M.up_stamp, M.up_child, M.up_child_rgb, M.up_valid, M.up_parent, M.brick_parent, M.ctr, m->d_list[0],
 	                m->d_list[1], m->d_points[0], m->d_points[1], m->d_ray_end, m->d_hit_tab, m->d_tab_keys, m->d_tab_min,
 	                m->d_seg, m->d_seg_base, m->d_seg_count, m->d_order, m->d_nodes, m->d_items, m->d_vmask, m->d_rc,
@@ -353,9 +352,8 @@ void grow_pools(Map* m, uint32_t overflow, uint32_t want_bricks, uint32_t want_u
 		dev_grow(M.miss_mask, ob, nb, 0, s, tot);
 		dev_grow(M.hit_mask, ob, nb, 0, s, tot);
 		dev_grow(M.chg_mask, ob, nb, 0, s, tot);
-		dev_grow(M.agg2, ob, nb, 0, s, tot);
 		dev_grow(M.meta, ob, nb, 0, s, tot);
-		dev_grow(M.sum1, ob * 8, nb * 8, 0, s, tot);
+		dev_grow(M.pair_max, ob, nb, 0, s, tot);
 		dev_grow(M.leaf_rgb, ob * 64, nb * 64, 0, s, tot);
 		dev_grow(M.sum1_rgb, ob * 8, nb * 8, 0, s, tot);
 		dev_grow(M.rgb2, ob, nb, 0, s, tot);
@@ -1175,18 +1173,15 @@ __global__ void __launch_bounds__(256) k_reflag(DeviceMap M, uint32_t n_bricks)
 		const uint32_t mt = M.meta[b];
 		if (!(mt & 0xff0000u)) continue;
 		const float* leaf = M.leaf + b * 64;
-		uint32_t bfl = 0, fl16 = 0;
+		uint32_t fl16 = 0;
 		for (uint32_t o = 0; o < 8; ++o) {
-			uint32_t ofl = M.default_flags;
 			if ((mt >> (16 + o)) & 1u) {
-				ofl = 0;
+				uint32_t ofl = 0;
 				for (int j = 0; j < 8; ++j) ofl |= leaf_flags(M, leaf[8 * o + j]);
 				fl16 |= ofl << (2 * o);
 			}
-			bfl |= ofl;
 		}
-		M.meta[b] = (mt & 0xffff0000u) | fl16;
-		M.agg2[b].flags = bfl;
+		M.meta[b] = (mt & 0xffff0000u) | fl16;  // the depth-2 flags follow from it (block_flags)
 	}
 }
 
@@ -2839,7 +2834,7 @@ int ufo_b200_clear(ufo_b200_map* m)
 		CK(cudaMemsetAsync(M.leaf, 0, nb * 64 * 4, s));
 		CK(cudaMemsetAsync(M.miss_mask, 0, nb * 8, s));
 		CK(cudaMemsetAsync(M.hit_mask, 0, nb * 8, s));
-		CK(cudaMemsetAsync(M.agg2, 0, nb * sizeof(Agg), s));
+		CK(cudaMemsetAsync(M.pair_max, 0, nb * sizeof(float4), s));
 		CK(cudaMemsetAsync(M.meta, 0, nb * 4, s));
 		if (M.color) CK(cudaMemsetAsync(M.leaf_rgb, 0, nb * 64 * 4, s));
 		if (M.alias_miss) {

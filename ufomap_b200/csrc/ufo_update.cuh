@@ -136,24 +136,37 @@ struct __align__(128) WarpSlab {
 	unsigned long long mm[64];
 	unsigned long long hm[64];
 	uint32_t meta[64];
+	float4 q[64];  // pair maxima
 };
+// list entry of a loaded octet: (block << 3) | octet, plus
+constexpr uint32_t kEntInit = 1u << 9;      // the octet is initialised (its leaves are loaded; otherwise 0.0)
+constexpr uint32_t kEntTouched = 1u << 10;  // the scan marked a voxel of it (otherwise only its max is needed)
+// colour maps keep one entry in flight per lane, so a partner does not get an entry of its own: the
+// lane of the touched octet folds it into the octet's max (the slot then carries the pair's max)
+constexpr uint32_t kEntPartner = 1u << 11;      // untouched, initialised partner: loaded with the octet
+constexpr uint32_t kEntPartnerZero = 1u << 12;  // untouched, uninitialised partner: 0.0
 
 // K3: one WARP per brick of the scan's TOUCHED LIST (the cost of a scan does not depend on the size
 // of the map), no CTA-wide barrier at all: a warp waiting for its leaf sectors never holds others at
 // a __syncthreads (a CTA-cooperative version spent a large share of its stall samples there).
 //  * lane 0 stages the header slab of the warp's NEXT brick -- miss masks 512 B, hit masks 512 B,
-//    meta 256 B -- with three bulk copies (cp.async.bulk) on a per-warp mbarrier, two stages;
-//  * lane = block (twice: 64 blocks): masks from shared memory, touched-octet list of the WHOLE
-//    brick by warp prefix sums -- built one brick EARLY, right after the previous brick's leaf loop,
-//    so that the brick's leaf sectors can be pulled into the L2 (prefetch.global.L2, no registers)
-//    while the previous brick's aggregates are still being written;
-//  * the old depth-1 sectors / depth-2 aggregates the block lanes need at the end travel by
+//    meta 256 B, pair maxima 1 KB -- with four bulk copies (cp.async.bulk) on a per-warp mbarrier,
+//    two stages;
+//  * lane = block (twice: 64 blocks): masks from shared memory, list of the octets to load of the
+//    WHOLE brick by warp prefix sums: the touched octets and the initialised partners of touched
+//    octets (the pair (2k, 2k+1) is one 64 B-aligned piece of the block, so the partner's sector
+//    comes with the same DRAM access; colour maps: touched octets only, whose lane also reads the
+//    partner, see kEntPartner); built one brick EARLY, right after the previous brick's leaf
+//    loop, so that the brick's leaf sectors can be pulled into the L2 (prefetch.global.L2, no
+//    registers) while the previous brick's aggregates are still being written;
+//  * colour maps: the old depth-1 / depth-2 colours the block lanes need at the end travel by
 //    cp.async into shared memory behind the leaf loop (no registers held across it);
 //  * lanes then own list entries = 32 B leaf sectors, UFO_UB_INFLIGHT requested per lane before the
-//    first is used: v = clamp(v + hit), then v = clamp(v + miss) (float, order fixed), written back
-//    in place; octet maxima / flags return through warp-private shared memory (__syncwarp only);
-//  * block lanes write the depth-1 sector, the depth-2 aggregate, the meta word, clear the masks;
-//    depth-3 / depth-4 aggregates by shuffles.
+//    first is used (an uninitialised octet is not loaded: its leaves are 0.0): v = clamp(v + hit),
+//    then v = clamp(v + miss) (float, order fixed), written back in place; a partner is only read;
+//    octet maxima / flags return through warp-private shared memory (__syncwarp only);
+//  * block lanes write the pair maxima and the meta word, clear the masks; depth-3 / depth-4
+//    aggregates by shuffles.
 // Alternatives that were slower on the bench workload: a list per half brick (latency exposed twice
 // per brick); 2 sectors in flight at 6 CTAs of 80 registers; no L2 prefetch; more shared memory per
 // SM (less L1 left for the sectors in flight); a cp.async leaf pipeline through shared memory (fewer
@@ -161,10 +174,6 @@ struct __align__(128) WarpSlab {
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* g)
 {
 	asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(g) : "memory");
-}
-__device__ __forceinline__ void cp_async8(void* smem_dst, const void* g)
-{
-	asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(g) : "memory");
 }
 __device__ __forceinline__ void cp_async4(void* smem_dst, const void* g)
 {
@@ -195,9 +204,8 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 template <bool COLOR>
 struct __align__(128) BrickWork {
 	WarpSlab slab[2];
-	// old depth-1 sector of a marked block; for an unmarked block the slot holds its old depth-2
-	// aggregate (first 8 bytes of s1lo) and colour (first 4 bytes of s1hi) instead
-	float4 s1lo[64], s1hi[64];
+	// colour maps: old depth-1 colours of a marked block; for an unmarked block the first word of
+	// c1lo holds its old depth-2 colour instead
 	uint4 c1lo[COLOR ? 64 : 1], c1hi[COLOR ? 64 : 1];
 	float omax[512];
 	uint32_t orgb[COLOR ? 512 : 2];
@@ -237,10 +245,11 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			st_mi1 = mi;
 		}
 		fence_proxy_async();
-		mbar_expect_tx(&S.bar[stage], 512u + 512u + 256u);
+		mbar_expect_tx(&S.bar[stage], 512u + 512u + 256u + 1024u);
 		bulk_load(S.slab[stage].mm, M.mask_base + (size_t)mi * 64, 512u, &S.bar[stage]);
 		bulk_load(S.slab[stage].hm, M.hit_mask + (size_t)brick * 64, 512u, &S.bar[stage]);
 		bulk_load(S.slab[stage].meta, M.meta + (size_t)brick * 64, 256u, &S.bar[stage]);
+		bulk_load(S.slab[stage].q, M.pair_max + (size_t)brick * 64, 1024u, &S.bar[stage]);
 	};
 	if (lane == 0) {
 		mbar_init(&S.bar[0], 1);
@@ -252,35 +261,43 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 
 	unsigned int s_vox = 0, s_hit = 0, s_oct = 0, s_blk = 0, s_new = 0, s_lin = 0;
 
-	// lane = block lane of either half: touched octets of the brick in `slab`, list by warp prefix sums
+	// lane = block lane of either half: touched octets (t8) of the brick in `slab` and the octets to
+	// load (touched, and initialised partners of touched ones), list by warp prefix sums
 	auto build_list = [&](const WarpSlab& slab, uint16_t* list, uint32_t (&t8)[2], uint32_t (&excl)[2], uint32_t& total) {
 		total = 0;
 #pragma unroll
 		for (uint32_t h = 0; h < 2; ++h) {
 			const uint32_t blk = h * 32 + lane;
 			const unsigned long long u = slab.mm[blk] | slab.hm[blk];
-			uint32_t t = 0;
+			uint32_t t = 0, ld = 0, init = 0;
 			if (u) {
 #pragma unroll
 				for (uint32_t o = 0; o < 8; ++o) {
 					const uint32_t base = ((o & 1u) << 1) | ((o & 2u) << 2) | ((o & 4u) << 3);
 					t |= (((u >> base) & 0x330033ull) ? 1u : 0u) << o;
 				}
+				init = (slab.meta[blk] >> 16) & 0xffu;
+				ld = t | (COLOR ? 0u : (((t & 0x55u) << 1) | ((t & 0xaau) >> 1)) & init);
+				// out-of-tree hits (k_alias_apply, before this kernel) may have written an octet whose
+				// initialised bit is still clear: touched octets are then loaded all the same
+				if (!fold) init |= t;
 			}
-			uint32_t incl = __popc(t);
+			uint32_t incl = __popc(ld);
 #pragma unroll
 			for (int o = 1; o < 32; o <<= 1) {
 				const uint32_t v = __shfl_up_sync(FULL, incl, o);
 				if (lane >= (uint32_t)o) incl += v;
 			}
-			excl[h] = total + incl - __popc(t);
+			excl[h] = total + incl - __popc(ld);
 			t8[h] = t;
 			{
-				uint32_t bits = t, at = excl[h];
+				uint32_t bits = ld, at = excl[h];
 				while (bits) {
 					const uint32_t o = __ffs(bits) - 1;
 					bits &= bits - 1;
-					list[at++] = (uint16_t)((blk << 3) | o);
+					uint32_t pf = 0;
+					if (COLOR && !((t >> (o ^ 1u)) & 1u)) pf = ((init >> (o ^ 1u)) & 1u) ? kEntPartner : kEntPartnerZero;
+					list[at++] = (uint16_t)((blk << 3) | o | (((init >> o) & 1u) ? kEntInit : 0u) | (((t >> o) & 1u) ? kEntTouched : 0u) | pf);
 				}
 			}
 			total += __shfl_sync(FULL, incl, 31);
@@ -303,31 +320,28 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 		const uint16_t* list = S.list[st];
 		const size_t b0 = (size_t)brick * 64;
 
-		// what the block lanes need after the leaf loop: requested now, into shared memory
+		// colours the block lanes need after the leaf loop: requested now, into shared memory
+		if (COLOR) {
 #pragma unroll
-		for (uint32_t h = 0; h < 2; ++h) {
-			const uint32_t blk = h * 32 + lane;
-			if (t8[h]) {
-				if (t8[h] != 0xffu) {
-					cp_async16(&S.s1lo[blk], M.sum1 + (b0 + blk) * 8);
-					cp_async16(&S.s1hi[blk], M.sum1 + (b0 + blk) * 8 + 4);
-					if (COLOR) {
+			for (uint32_t h = 0; h < 2; ++h) {
+				const uint32_t blk = h * 32 + lane;
+				if (t8[h]) {
+					if (t8[h] != 0xffu) {
 						cp_async16(&S.c1lo[COLOR ? blk : 0], M.sum1_rgb + (b0 + blk) * 8);
 						cp_async16(&S.c1hi[COLOR ? blk : 0], M.sum1_rgb + (b0 + blk) * 8 + 4);
 					}
+				} else if (fold && (slab.meta[blk] & 0xff0000u)) {
+					cp_async4(&S.c1lo[COLOR ? blk : 0], &M.rgb2[b0 + blk]);
 				}
-			} else if (fold && (slab.meta[blk] & 0xff0000u)) {
-				cp_async8(&S.s1lo[blk], &M.agg2[b0 + blk]);
-				if (COLOR) cp_async4(&S.s1hi[blk], &M.rgb2[b0 + blk]);
 			}
+			cp_async_commit();
 		}
-		cp_async_commit();
 		__syncwarp();
 		// lanes own list entries = 32 B leaf sectors (+ the colour sector of the same octet), NF of them
 		// requested per lane before the first is used
 		constexpr int NF = COLOR ? UFO_UB_INFLIGHT_COLOR : UFO_UB_INFLIGHT;
 		for (uint32_t i = lane; i < total; i += 32 * NF) {
-			float4 a0[NF], a1[NF];
+			float4 a0[NF], a1[NF], p0[COLOR ? NF : 1], p1[COLOR ? NF : 1];
 			uint4 x0[COLOR ? NF : 1], x1[COLOR ? NF : 1];
 			uint32_t en[NF];
 #pragma unroll
@@ -335,25 +349,43 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				const uint32_t idx = i + 32 * f;
 				en[f] = idx < total ? (uint32_t)list[idx] : 0xffffffffu;
 				if (en[f] != 0xffffffffu) {
-					const size_t off = (b0 + (en[f] >> 3)) * 64 + 8 * (en[f] & 7u);
-					const float4* lp = reinterpret_cast<const float4*>(M.leaf + off);
-					a0[f] = lp[0];
-					a1[f] = lp[1];
-					if (COLOR) {
+					const size_t off = (b0 + ((en[f] >> 3) & 63u)) * 64 + 8 * (en[f] & 7u);
+					a0[f] = a1[f] = make_float4(0.f, 0.f, 0.f, 0.f);
+					if (en[f] & kEntInit) {
+						const float4* lp = reinterpret_cast<const float4*>(M.leaf + off);
+						a0[f] = lp[0];
+						a1[f] = lp[1];
+					}
+					if (COLOR && (en[f] & kEntTouched)) {
 						const uint4* cp = reinterpret_cast<const uint4*>(M.leaf_rgb + off);
 						x0[COLOR ? f : 0] = cp[0];
 						x1[COLOR ? f : 0] = cp[1];
+					}
+					if (COLOR && (en[f] & kEntPartner)) {
+						const float4* pp = reinterpret_cast<const float4*>(M.leaf + (off ^ 8u));
+						p0[COLOR ? f : 0] = pp[0];
+						p1[COLOR ? f : 0] = pp[1];
 					}
 				}
 			}
 #pragma unroll
 			for (int f = 0; f < NF; ++f) {
 				if (en[f] == 0xffffffffu) continue;
-				const uint32_t idx = i + 32 * f, t = en[f] >> 3, o = en[f] & 7u;
+				const uint32_t idx = i + 32 * f, t = (en[f] >> 3) & 63u, o = en[f] & 7u;
+				if (!(en[f] & kEntTouched)) {  // partner of a touched octet: its max only
+					const float4 p = a0[f], q = a1[f];
+					S.omax[idx] = fmaxf(fmaxf(fmaxf(p.x, p.y), fmaxf(p.z, p.w)), fmaxf(fmaxf(q.x, q.y), fmaxf(q.z, q.w)));
+					continue;
+				}
 				const uint32_t m8 = octet_bits8(slab.mm[t], o), h8 = octet_bits8(slab.hm[t], o);
 				float omax;
 				uint32_t ofl;
 				update_octet<SET>(M, miss, M.leaf + (b0 + t) * 64 + 8 * o, m8, h8, a0[f], a1[f], omax, ofl, b0 + t, o);
+				if (COLOR && (en[f] & kEntPartner)) {
+					const float4 p = p0[COLOR ? f : 0], q = p1[COLOR ? f : 0];
+					omax = fmaxf(omax, fmaxf(fmaxf(fmaxf(p.x, p.y), fmaxf(p.z, p.w)), fmaxf(fmaxf(q.x, q.y), fmaxf(q.z, q.w))));
+				}
+				if (COLOR && (en[f] & kEntPartnerZero)) omax = fmaxf(omax, 0.0f);
 				S.omax[idx] = omax;
 				S.list[st][idx] = (uint16_t)ofl;  // the entry has been consumed: the slot carries the flags back
 				if (COLOR) {
@@ -376,18 +408,16 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			const uint32_t brick_n = __shfl_sync(FULL, st == 0 ? st_brick1 : st_brick0, 0);
 			const float* leaf_n = M.leaf + (size_t)brick_n * 64 * 64;
 			for (uint32_t i = lane; i < totaln; i += 32) {
-				const uint32_t en = S.list[st ^ 1u][i];
-				prefetch_l2(leaf_n + (en >> 3) * 64 + 8 * (en & 7u));
-				if (COLOR) prefetch_l2(M.leaf_rgb + (size_t)brick_n * 64 * 64 + (en >> 3) * 64 + 8 * (en & 7u));
+				const uint32_t en = S.list[st ^ 1u][i], off = ((en >> 3) & 63u) * 64 + 8 * (en & 7u);
+				if (en & kEntInit) prefetch_l2(leaf_n + off);
+				if (COLOR && (en & kEntPartner)) prefetch_l2(leaf_n + (off ^ 8u));
+				if (COLOR && (en & kEntTouched)) prefetch_l2(M.leaf_rgb + (size_t)brick_n * 64 * 64 + off);
 			}
-#pragma unroll
-			for (uint32_t h = 0; h < 2; ++h)
-				if (t8n[h] && t8n[h] != 0xffu) prefetch_l2(M.sum1 + ((size_t)brick_n * 64 + h * 32 + lane) * 8);
 #endif
 		}
-		cp_async_wait_all();
+		if (COLOR) cp_async_wait_all();
 		__syncwarp();
-		// block lanes: depth-1 sector, depth-2 aggregate, meta, mask clearing
+		// block lanes: pair maxima, meta, mask clearing
 		float agg_occ[2];
 		uint32_t agg_fl[2], agg_rgb[2];
 #pragma unroll
@@ -400,47 +430,46 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			float my_occ = 0.0f;
 			uint32_t my_fl = M.default_flags, my_rgb = 0;
 			if (marked) {
-				float4 p0 = make_float4(0.f, 0.f, 0.f, 0.f), p1 = p0;
 				uint4 q0 = make_uint4(0u, 0u, 0u, 0u), q1 = q0;
-				if (t8[h] != 0xffu) {
-					p0 = S.s1lo[blk];
-					p1 = S.s1hi[blk];
-					if (COLOR) {
-						q0 = S.c1lo[COLOR ? blk : 0];
-						q1 = S.c1hi[COLOR ? blk : 0];
-					}
+				if (COLOR && t8[h] != 0xffu) {
+					q0 = S.c1lo[COLOR ? blk : 0];
+					q1 = S.c1hi[COLOR ? blk : 0];
 				}
-				const float old1[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
 				const uint32_t oldc[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
-				float new1[8];
+				const float4 oq = slab.q[blk];
+				const float oldq[4] = {oq.x, oq.y, oq.z, oq.w};
+				const uint32_t t = t8[h], init = (mt >> 16) & 0xffu;
+				const uint32_t ld = t | (COLOR ? 0u : (((t & 0x55u) << 1) | ((t & 0xaau) >> 1)) & init);
+				float om[8], nq[4];
 				uint32_t newc[8];
-				float bmax = -3.402823466e+38f;
 				uint32_t bfl = 0, newmeta = 0, at = excl[h];
 #pragma unroll
 				for (uint32_t o = 0; o < 8; ++o) {
-					float om = 0.0f;
-					uint32_t fl = M.default_flags, touched = 0, oc = 0;
-					if ((t8[h] >> o) & 1u) {
-						om = S.omax[at];
-						fl = S.list[st][at];
-						if (COLOR) oc = S.orgb[COLOR ? at : 0];
+					uint32_t fl = M.default_flags, oc = 0;
+					// mono: an uninitialised partner of a touched octet; colour: the partner is already in
+					// the touched octet's slot
+					om[o] = COLOR ? -3.402823466e+38f : 0.0f;
+					if ((ld >> o) & 1u) {
+						om[o] = S.omax[at];
+						if ((t >> o) & 1u) {
+							fl = S.list[st][at];
+							if (COLOR) oc = S.orgb[COLOR ? at : 0];
+						}
 						++at;
-						touched = 1;
-					} else if ((mt >> (16 + o)) & 1u) {
-						om = old1[o];
+					}
+					if (!((t >> o) & 1u) && ((init >> o) & 1u)) {
 						fl = (mt >> (2 * o)) & 3u;
 						if (COLOR) oc = oldc[o];
 					}
-					new1[o] = om;
 					newc[o] = oc;
-					bmax = fmaxf(bmax, om);
 					bfl |= fl;
-					newmeta |= (fl << (2 * o)) | (touched << (16 + o));
+					newmeta |= (fl << (2 * o)) | (((t >> o) & 1u) << (16 + o));
 				}
-				float4* sp = reinterpret_cast<float4*>(M.sum1 + b * 8);
-				sp[0] = make_float4(new1[0], new1[1], new1[2], new1[3]);
-				sp[1] = make_float4(new1[4], new1[5], new1[6], new1[7]);
-				M.agg2[b] = {bmax, bfl};
+#pragma unroll
+				for (uint32_t k = 0; k < 4; ++k) nq[k] = ((t >> (2 * k)) & 3u) ? fmaxf(om[2 * k], om[2 * k + 1]) : oldq[k];
+				const float4 q = make_float4(nq[0], nq[1], nq[2], nq[3]);
+				const float bmax = block_occ(q);
+				M.pair_max[b] = q;
 				if (COLOR) {
 					uint4* cp = reinterpret_cast<uint4*>(M.sum1_rgb + b * 8);
 					cp[0] = make_uint4(newc[0], newc[1], newc[2], newc[3]);
@@ -457,10 +486,9 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				my_occ = bmax;
 				my_fl = bfl | 0x100u;
 			} else if (fold && (mt & 0xff0000u)) {
-				const float4 o2 = S.s1lo[blk];
-				my_occ = o2.x;
-				my_fl = __float_as_uint(o2.y);
-				if (COLOR) my_rgb = __float_as_uint(S.s1hi[blk].x);
+				my_occ = block_occ(slab.q[blk]);
+				my_fl = block_flags(M, mt);
+				if (COLOR) my_rgb = S.c1lo[COLOR ? blk : 0].x;
 			}
 			agg_occ[h] = my_occ;
 			agg_fl[h] = my_fl;
@@ -567,8 +595,7 @@ __global__ void __launch_bounds__(256) k_brick_agg(DeviceMap M)
 		}
 		const size_t b = (size_t)brick * 64 + 2 * lane;
 		const uint2 mt = *reinterpret_cast<const uint2*>(&M.meta[b]);
-		const uint4 ag = *reinterpret_cast<const uint4*>(&M.agg2[b]);
-		Agg c0 = {__uint_as_float(ag.x), ag.y}, c1 = {__uint_as_float(ag.z), ag.w};
+		Agg c0 = {block_occ(M.pair_max[b]), block_flags(M, mt.x)}, c1 = {block_occ(M.pair_max[b + 1]), block_flags(M, mt.y)};
 		if (!(mt.x & 0xff0000u)) c0 = {0.0f, M.default_flags};  // never written: unknown space
 		if (!(mt.y & 0xff0000u)) c1 = {0.0f, M.default_flags};
 		const uint32_t tag = M.scan_id & 0xffu;
