@@ -29,6 +29,9 @@ constexpr uint64_t kEmptyKey = ~0ull;
 constexpr uint32_t kPending = 0xffffffffu;  // hash value not published yet
 constexpr uint32_t kFailed = 0xfffffffeu;   // allocation behind this key overflowed
 constexpr uint32_t kNone = 0xffffffffu;     // "no such brick / node"
+// touched_mi flag, set by k_gather for a brick without a hit this scan: k_update_brick does not
+// stage its hit masks.  Lists built elsewhere leave it clear, so their bricks stage them.
+constexpr uint32_t kMiNoHits = 1u << 31;
 
 // aggregate of an inner node: max log-odds of the subtree + contains_* flags
 // (occupancy_map_base.h:1179-1224).  flags: bit0 contains_free, bit1 contains_unknown.
@@ -44,6 +47,7 @@ struct Counters {
 	uint32_t overflow;   // bit1 bricks/brick hash, bit2 upper nodes, bit3 ray-record buffer, bit4 ray bound violated (bug), bit5 alias arrays needed, bit8 early-stopping buffers
 	uint32_t n_touched;    // bricks stamped by this scan = length of DeviceMap::touched
 	uint32_t item_cursor;  // next work unit of the fused walk (k_walk_mark)
+	uint32_t k3_cursor;    // touched entries claimed by k_update_brick's warps beyond their first (zeroed before each launch)
 	uint32_t max_span;     // longest ray of the scan in dominant-axis steps (sets the shell thickness)
 	uint32_t n_touched_alt;  // routed mode: length of DeviceMap::touched_alt
 	uint32_t n_dirty;        // dense mode: length of DeviceMap::vol_list (also: node list of insert depth 5/6, bricks of a write batch)
@@ -125,7 +129,8 @@ struct DeviceMap {
 	unsigned long long* brick_key;
 	uint32_t* brick_stamp;  // scan id of the last scan that touched the brick
 	uint32_t* touched;      // [brick_cap] bricks stamped by the current scan, in stamping order (touch_brick)
-	uint32_t* touched_mi;   // [brick_cap] where the free-space masks of touched[i] are: mask_base + mi * 64
+	uint32_t* touched_mi;   // [brick_cap] where the free-space masks of touched[i] are: mask_base + (mi & ~kMiNoHits) * 64
+	uint32_t* hit_stamp;    // [brick_cap] scan id of the last scan that set a hit bit of the brick
 	unsigned long long* mask_base;  // per scan: miss_mask (mi = brick slot) or the dense scan volume (mi = volume brick)
 	// Dense scan volume (ufo_walk.cuh): block masks of the cube of bricks around the sensor that a
 	// range-limited scan can reach, brick-major ([volume brick][64 blocks in Morton order]), so that

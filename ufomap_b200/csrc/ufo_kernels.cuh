@@ -347,6 +347,7 @@ __device__ __forceinline__ void mark_hit(const DeviceMap& M, Key3 k)
 	touch_or_dirty(M, brick, k.x >> 4, k.y >> 4, k.z >> 4);
 	const size_t b = (size_t)brick * 64 + morton2(k.x >> 2, k.y >> 2, k.z >> 2);
 	atomicOr(&M.hit_mask[b], 1ull << linear2(k.x, k.y, k.z));
+	M.hit_stamp[brick] = M.scan_id;
 }
 
 // ---------------------------------------------------------------------------
@@ -586,6 +587,7 @@ __global__ void __launch_bounds__(256) k_hits(DeviceMap M, ScanArgs a)
 	uint32_t v = morton2(k.x, k.y, k.z);
 	const unsigned long long hbit = 1ull << linear2(k.x, k.y, k.z);
 	unsigned long long old = atomicOr(&M.hit_mask[slot], hbit);
+	M.hit_stamp[brick] = M.scan_id;
 	if (old & hbit) return;  // re-run after a pool regrow: colour already blended
 	if (wrapped_alt(M, k.x) != k.x || wrapped_alt(M, k.y) != k.y || wrapped_alt(M, k.z) != k.z) {
 		// a voxel on the map's boundary may also receive out-of-tree hits: k_wrapped_colors blends

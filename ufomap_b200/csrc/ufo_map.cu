@@ -269,6 +269,7 @@ void alloc_pools(Map* m, uint32_t brick_cap, uint32_t up_cap)
 	dev_alloc(M.bh_tab, (size_t)M.bh_mask + 1, 0xff, s, tot);
 	dev_alloc(M.brick_key, brick_cap, 0, s, tot);
 	dev_alloc(M.brick_stamp, brick_cap, 0, s, tot);
+	dev_alloc(M.hit_stamp, brick_cap, 0, s, tot);
 	dev_alloc(M.touched, brick_cap, 0, s, tot);
 	dev_alloc(M.touched_alt, brick_cap, 0, s, tot);
 	dev_alloc(M.touched_mi, brick_cap, 0, s, tot);
@@ -306,7 +307,7 @@ void alloc_pools(Map* m, uint32_t brick_cap, uint32_t up_cap)
 void free_pools(Map* m)
 {
 	DeviceMap& M = m->M;
-	void* ptrs[] = {M.bh_tab, M.brick_key, M.brick_stamp, M.touched, M.touched_alt, M.touched_mi, M.touched_alt_mi, M.chg_mask, M.vol, M.vol_dirty, M.vol_list, M.route, m->route_inbox, M.brick_sum3, M.brick_sum4, M.brick_rgb3, M.brick_rgb4,
+	void* ptrs[] = {M.bh_tab, M.brick_key, M.brick_stamp, M.hit_stamp, M.touched, M.touched_alt, M.touched_mi, M.touched_alt_mi, M.chg_mask, M.vol, M.vol_dirty, M.vol_list, M.route, m->route_inbox, M.brick_sum3, M.brick_sum4, M.brick_rgb3, M.brick_rgb4,
 	                M.leaf, M.leaf_rgb, M.miss_mask, M.hit_mask, M.meta, M.pair_max, M.rgb2, M.sum1_rgb,
 	                M.alias_miss, M.alias_hit, M.uh_keys, M.uh_vals, M.up_key, M.up_agg, M.up_rgb, M.up_stamp, M.up_child, M.up_child_rgb, M.up_valid, M.up_parent, M.brick_parent, M.ctr, m->d_list[0],
 	                m->d_list[1], m->d_points[0], m->d_points[1], m->d_ray_end, m->d_hit_tab, m->d_tab_keys, m->d_tab_min,
@@ -361,6 +362,7 @@ void grow_pools(Map* m, uint32_t overflow, uint32_t want_bricks, uint32_t want_u
 		dev_grow(M.alias_hit, ob, nb, 0, s, tot);
 		dev_grow(M.brick_key, oc, nc, 0, s, tot);
 		dev_grow(M.brick_stamp, oc, nc, 0, s, tot);
+		dev_grow(M.hit_stamp, oc, nc, 0, s, tot);
 		dev_grow(M.brick_parent, oc, nc, 0xff, s, tot);
 		dev_grow(M.touched, oc, nc, 0, s, tot);
 		dev_grow(M.touched_alt, oc, nc, 0, s, tot);
@@ -564,6 +566,7 @@ void ensure_seg(Map* m, unsigned long long want)
 // K3 over the scan's touched list: persistent warps, the list length is read on the device.
 void launch_update(Map* m, float miss, bool set_mode = false)
 {
+	CK(cudaMemsetAsync(&m->M.ctr->k3_cursor, 0, sizeof(uint32_t), m->stream));
 	if (m->M.color) {
 		const uint32_t per_sm = UbShape<true>::kMinBlocks, T = UbShape<true>::kWarps * 32;
 		const uint32_t grid = (uint32_t)m->sm_count * (m->k3_blocks ? std::min<uint32_t>(per_sm, (uint32_t)m->k3_blocks) : per_sm);
@@ -2826,6 +2829,7 @@ int ufo_b200_clear(ufo_b200_map* m)
 		CK(cudaMemsetAsync(M.uh_keys, 0xff, ((size_t)M.uh_mask + 1) * 8, s));
 		CK(cudaMemsetAsync(M.uh_vals, 0xff, ((size_t)M.uh_mask + 1) * 4, s));
 		CK(cudaMemsetAsync(M.brick_stamp, 0, (size_t)m->n_bricks * 4, s));
+		CK(cudaMemsetAsync(M.hit_stamp, 0, (size_t)m->n_bricks * 4, s));
 		CK(cudaMemsetAsync(M.up_stamp, 0, (size_t)m->n_upper * 4, s));
 		CK(cudaMemsetAsync(M.up_valid, 0, (size_t)m->n_upper * 4, s));
 		CK(cudaMemsetAsync(M.up_parent, 0xff, (size_t)m->n_upper * 4, s));

@@ -51,7 +51,7 @@ __global__ void __launch_bounds__(256) k_outbox(DeviceMap M)
 		const uint32_t brick = M.touched[e];
 		const unsigned long long key = M.brick_key[brick];
 		const uint32_t owner = brick_owner(key, M.route_world);
-		unsigned long long* mp = M.mask_base + (size_t)M.touched_mi[e] * 64 + 2 * lane;
+		unsigned long long* mp = M.mask_base + (size_t)(M.touched_mi[e] & ~kMiNoHits) * 64 + 2 * lane;
 		const ulonglong2 mk = *reinterpret_cast<const ulonglong2*>(mp);
 		if (owner == M.route_rank && !M.route_self) {
 			// own brick, marks stay: it opens the touched list of the apply phase (scan id + 1),
@@ -180,6 +180,7 @@ __global__ void __launch_bounds__(256) k_inbox(DeviceMap M, uint32_t first, uint
 				continue;
 			}
 			atomicOr(&M.hit_mask[(size_t)brick * 64 + morton2(x >> 2, y >> 2, z >> 2)], 1ull << linear2(x, y, z));
+			M.hit_stamp[brick] = M.scan_id;
 		}
 	}
 }
@@ -206,6 +207,7 @@ __global__ void __launch_bounds__(256) k_inbox_color(DeviceMap M, uint32_t first
 			const size_t slot = (size_t)brick * 64 + morton2(x >> 2, y >> 2, z >> 2);
 			const unsigned long long hbit = 1ull << linear2(x, y, z);
 			const unsigned long long old = atomicOr(&M.hit_mask[slot], hbit);
+			M.hit_stamp[brick] = M.scan_id;
 			if ((old & hbit) || index == kNone) continue;  // already blended, or a point without colour
 			blend_color(M, slot * 64 + morton2(x, y, z), (uint32_t)(r.y >> 32));
 		}

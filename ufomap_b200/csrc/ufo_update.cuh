@@ -149,9 +149,10 @@ constexpr uint32_t kEntPartnerZero = 1u << 12;  // untouched, uninitialised part
 // K3: one WARP per brick of the scan's TOUCHED LIST (the cost of a scan does not depend on the size
 // of the map), no CTA-wide barrier at all: a warp waiting for its leaf sectors never holds others at
 // a __syncthreads (a CTA-cooperative version spent a large share of its stall samples there).
-//  * lane 0 stages the header slab of the warp's NEXT brick -- miss masks 512 B, hit masks 512 B,
-//    meta 256 B, pair maxima 1 KB -- with four bulk copies (cp.async.bulk) on a per-warp mbarrier,
-//    two stages;
+//  * warps claim their bricks from a work cursor (the cost of a brick varies by more than 10x);
+//  * lane 0 stages the header slab of the warp's NEXT brick -- miss masks 512 B, hit masks 512 B
+//    (only for a brick with a hit this scan: most bricks are crossed by free space only), meta
+//    256 B, pair maxima 1 KB -- with bulk copies (cp.async.bulk) on a per-warp mbarrier, two stages;
 //  * lane = block (twice: 64 blocks): masks from shared memory, list of the octets to load of the
 //    WHOLE brick by warp prefix sums: the touched octets and the initialised partners of touched
 //    octets (the pair (2k, 2k+1) is one 64 B-aligned piece of the block, so the partner's sector
@@ -234,7 +235,9 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 	if (gw >= n_touched) return;
 	const bool fold = M.alias_miss == nullptr;
 
-	uint32_t st_brick0 = kNone, st_brick1 = kNone, st_mi0 = 0, st_mi1 = 0;  // lane 0: (brick, mask group) of the two stages
+	// lane 0: (brick, touched_mi) of the two stages.  A brick flagged kMiNoHits has no hit bit: its
+	// hit masks are not staged, the lanes zero the slab's copy instead (zero_hits)
+	uint32_t st_brick0 = kNone, st_brick1 = kNone, st_mi0 = 0, st_mi1 = 0;
 	auto issue = [&](uint32_t stage, uint32_t e) {
 		const uint32_t brick = M.touched[e], mi = M.touched_mi[e];
 		if (stage == 0) {
@@ -244,19 +247,33 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			st_brick1 = brick;
 			st_mi1 = mi;
 		}
+		const bool hits = !(mi & kMiNoHits);
 		fence_proxy_async();
-		mbar_expect_tx(&S.bar[stage], 512u + 512u + 256u + 1024u);
-		bulk_load(S.slab[stage].mm, M.mask_base + (size_t)mi * 64, 512u, &S.bar[stage]);
-		bulk_load(S.slab[stage].hm, M.hit_mask + (size_t)brick * 64, 512u, &S.bar[stage]);
+		mbar_expect_tx(&S.bar[stage], 512u + (hits ? 512u : 0u) + 256u + 1024u);
+		bulk_load(S.slab[stage].mm, M.mask_base + (size_t)(mi & ~kMiNoHits) * 64, 512u, &S.bar[stage]);
+		if (hits) bulk_load(S.slab[stage].hm, M.hit_mask + (size_t)brick * 64, 512u, &S.bar[stage]);
 		bulk_load(S.slab[stage].meta, M.meta + (size_t)brick * 64, 256u, &S.bar[stage]);
 		bulk_load(S.slab[stage].q, M.pair_max + (size_t)brick * 64, 1024u, &S.bar[stage]);
 	};
+	// all lanes, before the stage's list is built (a __syncwarp in between)
+	auto zero_hits = [&](uint32_t stage) {
+		if (__shfl_sync(FULL, stage == 0 ? st_mi0 : st_mi1, 0) & kMiNoHits)
+			reinterpret_cast<ulonglong2*>(S.slab[stage].hm)[lane] = make_ulonglong2(0ull, 0ull);
+	};
+	// Bricks are claimed, not dealt: a warp starts with touched entry gw and then takes the next
+	// unclaimed entry (k3_cursor counts the claims beyond the first n_warps entries).  A brick next
+	// to the sensor costs an order of magnitude more than one at the end of the range, so a fixed
+	// deal ends with a few warps that drew heavy bricks and too few sectors in flight to keep the
+	// DRAM busy.  Lane 0 claims one brick ahead, so the atomic's latency is hidden behind a brick.
+	uint32_t claim = 0;
 	if (lane == 0) {
 		mbar_init(&S.bar[0], 1);
 		mbar_init(&S.bar[1], 1);
 		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 		issue(0, gw);
+		claim = n_warps + atomicAdd(&M.ctr->k3_cursor, 1u);
 	}
+	zero_hits(0);
 	__syncwarp();
 
 	unsigned int s_vox = 0, s_hit = 0, s_oct = 0, s_blk = 0, s_new = 0, s_lin = 0;
@@ -309,13 +326,16 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 	mbar_wait(&S.bar[0], 0u);
 	build_list(S.slab[0], S.list[0], t8, excl, total);
 	__syncwarp();
-	uint32_t it = 0;
-	for (uint32_t e = gw; e < n_touched; e += n_warps, ++it) {
+	for (uint32_t it = 0;; ++it) {
 		const uint32_t st = it & 1u;
-		const bool has_next = e + n_warps < n_touched;
-		if (lane == 0 && has_next) issue(st ^ 1u, e + n_warps);  // stage st^1 was released by the __syncwarp at the end of the loop
+		const uint32_t e_next = __shfl_sync(FULL, claim, 0);
+		const bool has_next = e_next < n_touched;
+		if (lane == 0 && has_next) {
+			issue(st ^ 1u, e_next);  // stage st^1 was released by the __syncwarp at the end of the loop
+			claim = n_warps + atomicAdd(&M.ctr->k3_cursor, 1u);
+		}
 		const uint32_t brick = __shfl_sync(FULL, st == 0 ? st_brick0 : st_brick1, 0);
-		const uint32_t mi = __shfl_sync(FULL, st == 0 ? st_mi0 : st_mi1, 0);
+		const uint32_t mi = __shfl_sync(FULL, st == 0 ? st_mi0 : st_mi1, 0) & ~kMiNoHits;
 		const WarpSlab& slab = S.slab[st];
 		const uint16_t* list = S.list[st];
 		const size_t b0 = (size_t)brick * 64;
@@ -401,6 +421,8 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 		if (has_next) {
 			// the next brick of this warp: its slab was requested at the top of this iteration; build its
 			// list now and pull its leaf sectors into the L2 while this brick's aggregates are written
+			zero_hits(st ^ 1u);
+			__syncwarp();
 			mbar_wait(&S.bar[st ^ 1u], ((it + 1u) >> 1) & 1u);
 			build_list(S.slab[st ^ 1u], S.list[st ^ 1u], t8n, excln, totaln);
 #if UFO_UB_PREFETCH
@@ -551,6 +573,7 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				atomicAdd(&slot[6], (unsigned long long)(__popc(ub0) + __popc(ub1)));
 			}
 		}
+		if (!has_next) break;
 		t8[0] = t8n[0];
 		t8[1] = t8n[1];
 		excl[0] = excln[0];

@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(256) k_gather(DeviceMap M)
 			base = __shfl_sync(peers, base, leader);
 			const uint32_t i = base + __popc(peers & ((1u << lane) - 1u));
 			M.touched[i] = slot;
-			M.touched_mi[i] = vb;
+			M.touched_mi[i] = vb | (M.hit_stamp[slot] == M.scan_id ? 0u : kMiNoHits);
 		}
 	}
 }
