@@ -559,6 +559,86 @@ int ufo_b200_ipc_close(void* dev_ptr);
 /* Forget everything (Octree::clear, octree.h:541-560): keeps device pools. */
 int ufo_b200_clear(ufo_b200_map* m);
 
+/* A map in bounded memory (no counterpart in the reference: pruneNode / deleteNodeChildren do not
+ * compile, SURVEY.md G5, and a pointer tree on the host has no 80 GB ceiling).  A local map follows
+ * the sensor; the rest lives with the caller, in host memory or on disk, as page blobs.
+ *
+ * One rule says which bricks (depth-4 nodes, 16^3 voxels) a volume KEEPS: a brick is kept iff every
+ * cube on its path from the root down to its own depth-4 cube passes the volume -- the chain test of
+ * ufo_b200_export_nodes_bv, stopped at depth 4.  Whole bricks only: a kept brick keeps all its
+ * voxels, those outside the volume included.  n_bv == 0 keeps everything; a volume that misses the
+ * map keeps nothing.  ufo_b200_retain is ufo_b200_retain_bv with one AABB record (box6: centre, half size).
+ *
+ * ufo_b200_retain_bv    removes every brick the volume does not keep and gives the memory back: the
+ *                       survivors are compacted into pools of max(the map's initial capacity,
+ *                       2 x survivors) bricks (peak: the old pools plus one array) and the levels
+ *                       above the bricks are rebuilt from them; a removed brick is never-touched
+ *                       space again.  Scan stamps move with their brick; the sensor model and the
+ *                       min/max change box are unchanged; the recorded changes of removed bricks are
+ *                       dropped with them.  out may be NULL.
+ * ufo_b200_page_out_bv  writes the bricks ufo_b200_retain_bv would remove for the same volume into a
+ *                       page blob and leaves the map as it is: page out, then retain.  *size receives
+ *                       the blob's size; it is written when it fits into cap (buf = NULL sizes the
+ *                       buffer).  Equal maps give equal blobs (bricks in ascending key order).
+ * ufo_b200_page_in      puts the bricks of a blob back and recomputes everything derived under the
+ *                       map's CURRENT sensor model.  Their scan stamps are 0 and change detection
+ *                       records nothing for them.  The blob must come from a map of the same
+ *                       resolution, depth_levels and colour mode, and NONE of its bricks may exist in
+ *                       the map (merging two histories of one voxel has no sound meaning): otherwise
+ *                       UFO_B200_E_INVALID and nothing is applied.  So a caller keeps the retained
+ *                       volume wider than the sensor's reach (max_range) and brings a page in before
+ *                       that reach enters it; a scan would otherwise re-create those bricks from
+ *                       unknown.
+ * ufo_b200_page_info    the header of a blob, on the host (no map needed); UFO_B200_E_INVALID when
+ *                       the magic or the version is not this library's or size is below the header's.
+ *
+ * The blob is opaque and versioned, not an interchange format; no compression, no file variant (the
+ * caller owns the bytes).  It holds nothing derived, so it stays valid when the thresholds change
+ * while it is out.  Layout: a 64-byte header {u64 magic "UFOPAGE1", u32 version, u32 colour, u64
+ * bits of the resolution double, u32 depth_levels, u32 0, u64 n bricks, 24 bytes 0}, then whole
+ * sections: brick keys u64[n] (x | y << 21 | z << 42 of the brick coordinates, ascending), leaves
+ * float[n][4096], octet-initialised bits u8[n][64], colour maps only: leaf colours u32[n][4096].
+ *
+ * Every call waits for a pending scan.  Rejected with nothing changed: routed maps
+ * (ufo_b200_route_setup) and depth_levels < 5 (UFO_B200_E_UNSUPPORTED), a map whose scan failed
+ * half-way (UFO_B200_E_INVALID).  A sharded map retains and pages within its own part. */
+typedef struct {
+	uint64_t bricks_before;
+	uint64_t bricks_kept;          /* page_in: bricks in the map afterwards */
+	uint64_t bricks_removed;       /* page_in: 0 */
+	uint64_t brick_cap_before, brick_cap_after;
+	uint64_t device_bytes_before, device_bytes_after;
+	/* CUDA-event times on the map's stream, allocation and the waits between the steps included.
+	 * retain: classify + prefix sum / compaction gather of every array / rebuild of the upper levels.
+	 * page_in: existence check + brick creation / scatter of the sections / derived values + upper levels */
+	float ms_classify, ms_compact, ms_upper;
+} ufo_b200_retain_stats;
+
+typedef struct {
+	uint32_t version;
+	uint32_t color;
+	uint32_t depth_levels;
+	uint32_t reserved;
+	double resolution;
+	uint64_t n_bricks;
+	uint64_t bytes;   /* size of the whole blob the header describes */
+} ufo_b200_page_header;
+
+int ufo_b200_retain_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, ufo_b200_retain_stats* out);
+int ufo_b200_retain(ufo_b200_map* m, const double box6[6], ufo_b200_retain_stats* out);
+int ufo_b200_page_out_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, void* buf, size_t cap, size_t* size);
+int ufo_b200_page_in(ufo_b200_map* m, const void* blob, size_t size, ufo_b200_retain_stats* out);
+int ufo_b200_page_info(const void* blob, size_t size, ufo_b200_page_header* out);
+
+/* What the map holds right now (waits for a pending scan): live bricks and upper nodes, the
+ * capacities of their pools and the device memory of the map. */
+typedef struct {
+	uint64_t bricks, brick_cap;
+	uint64_t upper_nodes, up_cap;
+	uint64_t device_bytes;
+} ufo_b200_pool_counts;
+int ufo_b200_pool_stats(ufo_b200_map* m, ufo_b200_pool_counts* out);
+
 const char* ufo_b200_version(void);
 
 #ifdef __cplusplus

@@ -762,6 +762,52 @@ class MapFacade
 		return s.good();
 	}
 
+	// EXTENSIONS (no counterpart in the reference): a map in bounded memory (ufomap_b200.h,
+	// ufo_b200_retain_bv).  retain removes every brick (16^3 voxels) the volume does not keep and gives
+	// its memory back; pageOut returns those bricks as a page blob without changing the map; pageIn puts
+	// a blob's bricks back and fails if any of them exists.  An empty BoundingVolume keeps everything.
+	// They take an AABB, one shape or a volume, like write; the status is left in lastStatus().
+	bool retain(ufo::geometry::BoundingVolume const& bounding_volume, ufo_b200_retain_stats* stats = nullptr)
+	{
+		auto const bv = ufo::geometry::toRecords(bounding_volume);
+		last_status_ = ufo_b200_retain_bv(map_, bv.data(), bv.size(), stats);
+		return UFO_B200_OK == last_status_;
+	}
+	bool retain(ufo::geometry::BoundingVar const& bounding_volume, ufo_b200_retain_stats* stats = nullptr)
+	{
+		ufo_b200_volume const r = ufo::geometry::toRecord(bounding_volume);
+		last_status_ = ufo_b200_retain_bv(map_, &r, 1, stats);
+		return UFO_B200_OK == last_status_;
+	}
+	bool retain(ufo::geometry::AABB const& bounding_volume, ufo_b200_retain_stats* stats = nullptr)
+	{
+		return retain(ufo::geometry::BoundingVar(bounding_volume), stats);
+	}
+	std::vector<std::uint8_t> pageOut(ufo::geometry::BoundingVolume const& bounding_volume)
+	{
+		return pageOutRecords(ufo::geometry::toRecords(bounding_volume));
+	}
+	std::vector<std::uint8_t> pageOut(ufo::geometry::BoundingVar const& bounding_volume)
+	{
+		return pageOutRecords({ufo::geometry::toRecord(bounding_volume)});
+	}
+	std::vector<std::uint8_t> pageOut(ufo::geometry::AABB const& bounding_volume)
+	{
+		return pageOut(ufo::geometry::BoundingVar(bounding_volume));
+	}
+	bool pageIn(std::vector<std::uint8_t> const& blob, ufo_b200_retain_stats* stats = nullptr)
+	{
+		last_status_ = ufo_b200_page_in(map_, blob.data(), blob.size(), stats);
+		return UFO_B200_OK == last_status_;
+	}
+	// live bricks / upper nodes, pool capacities and device bytes of the map right now
+	ufo_b200_pool_counts poolStats()
+	{
+		ufo_b200_pool_counts c{};
+		last_status_ = ufo_b200_pool_stats(map_, &c);
+		return c;
+	}
+
 	// setValueVolume (occupancy_map_base.h:492-518) for any one shape: the clear_volume service loops
 	// over the shapes of its BoundingVolume (server.cpp:345-354).  min_depth 0..4, colour maps at 0;
 	// other cases, and more than 2^22 nodes of one level inside the shape, set lastStatus() to
@@ -1236,6 +1282,17 @@ class MapFacade
 		if (UFO_B200_OK != ufo_b200_write_compressed(map_, box, min_depth, data_only, accel, level, data.data(), n, &n, &u)) return -1;
 		s.write(data.data(), (std::streamsize)n);
 		return s.good() ? (int)u : -1;
+	}
+	std::vector<std::uint8_t> pageOutRecords(std::vector<ufo_b200_volume> const& bv)
+	{
+		std::size_t n = 0;
+		std::vector<std::uint8_t> blob;
+		last_status_ = ufo_b200_page_out_bv(map_, bv.data(), bv.size(), nullptr, 0, &n);
+		if (UFO_B200_OK != last_status_) return blob;
+		blob.resize(n);
+		last_status_ = ufo_b200_page_out_bv(map_, bv.data(), bv.size(), blob.data(), n, &n);
+		if (UFO_B200_OK != last_status_) blob.clear();
+		return blob;
 	}
 	int writeCompressedBv(std::ostream& s, std::vector<ufo_b200_volume> const& bv, bool data_only, DepthType min_depth,
 	                      int accel, int level) const

@@ -64,6 +64,34 @@ class EarlyStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class RetainStats(C.Structure):
+    """ufo_b200_retain_stats (retain and page_in)."""
+    _fields_ = [(n, C.c_uint64) for n in (
+        "bricks_before", "bricks_kept", "bricks_removed", "brick_cap_before", "brick_cap_after",
+        "device_bytes_before", "device_bytes_after")] + [(n, C.c_float) for n in (
+            "ms_classify", "ms_compact", "ms_upper")]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class PageHeader(C.Structure):
+    """ufo_b200_page_header: what ufo_b200_page_info reads from a blob."""
+    _fields_ = [("version", C.c_uint32), ("color", C.c_uint32), ("depth_levels", C.c_uint32),
+                ("reserved", C.c_uint32), ("resolution", C.c_double), ("n_bricks", C.c_uint64),
+                ("bytes", C.c_uint64)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
+
+
+class PoolCounts(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("bricks", "brick_cap", "upper_nodes", "up_cap", "device_bytes")]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 # every symbol include/ufomap_b200.h declares
 SYMBOLS = [
     "ufo_b200_default_params", "ufo_b200_create", "ufo_b200_destroy", "ufo_b200_last_error",
@@ -88,6 +116,8 @@ SYMBOLS = [
     "ufo_b200_geometry_frustum", "ufo_b200_geometry_plane", "ufo_b200_geometry_ray",
     "ufo_b200_set_early_stopping", "ufo_b200_last_early_stats",
     "ufo_b200_iterate", "ufo_b200_update_nodes_color",
+    "ufo_b200_retain_bv", "ufo_b200_retain", "ufo_b200_page_out_bv", "ufo_b200_page_in", "ufo_b200_page_info",
+    "ufo_b200_pool_stats",
 ]
 
 # ufo_b200_volume: one shape of a bounding volume (type in BoundingVar order, members in v)
@@ -288,6 +318,12 @@ def load():
     lib.ufo_b200_set_shard.argtypes = [vp, u32, u32]
     lib.ufo_b200_set_early_stopping.argtypes = [vp, i32]
     lib.ufo_b200_last_early_stats.argtypes = [vp, C.POINTER(EarlyStats)]
+    lib.ufo_b200_retain_bv.argtypes = [vp, vp, sz, C.POINTER(RetainStats)]
+    lib.ufo_b200_retain.argtypes = [vp, vp, C.POINTER(RetainStats)]
+    lib.ufo_b200_page_out_bv.argtypes = [vp, vp, sz, vp, sz, C.POINTER(sz)]
+    lib.ufo_b200_page_in.argtypes = [vp, vp, sz, C.POINTER(RetainStats)]
+    lib.ufo_b200_page_info.argtypes = [vp, sz, C.POINTER(PageHeader)]
+    lib.ufo_b200_pool_stats.argtypes = [vp, C.POINTER(PoolCounts)]
     lib.ufo_b200_version.restype = C.c_char_p
     _lib = lib
     return lib
@@ -704,6 +740,44 @@ class Map:
             raise ValueError("set_value_volume_bv takes exactly one shape")
         self._check(self.lib.ufo_b200_set_value_volume_bv(self.h, bv.ctypes.data, float(occupancy), int(min_depth)))
 
+    # -- bounded memory: retain / page out / page in ---------------------------
+    def retain(self, volume=None, box=None):
+        """Remove every brick the volume does not keep and give the memory back; returns the
+        retain stats.  volume: see as_volume (None / []: keep everything); box = (min xyz, max xyz)
+        instead of a volume: the AABB form."""
+        st = RetainStats()
+        if box is not None:
+            b = self._box6(box)
+            self._check(self.lib.ufo_b200_retain(self.h, b.ctypes.data, C.byref(st)))
+        else:
+            bv, bp, nb = self._bv(volume)
+            self._check(self.lib.ufo_b200_retain_bv(self.h, bp, nb, C.byref(st)))
+        return st.as_dict()
+
+    def page_out(self, volume=None, box=None):
+        """The bricks retain() would remove for the same volume, as a page blob (numpy uint8); the
+        map is not changed."""
+        bv, bp, nb = self._bv(aabb(*box) if box is not None else volume)
+        n = C.c_size_t()
+        self._check(self.lib.ufo_b200_page_out_bv(self.h, bp, nb, None, 0, C.byref(n)))
+        buf = np.empty(n.value, np.uint8)
+        self._check(self.lib.ufo_b200_page_out_bv(self.h, bp, nb, buf.ctypes.data, len(buf), C.byref(n)))
+        assert n.value == len(buf)
+        return buf
+
+    def page_in(self, blob):
+        """Put the bricks of a page blob (bytes or numpy uint8) back; returns the stats."""
+        buf = np.ascontiguousarray(np.frombuffer(blob, np.uint8))
+        st = RetainStats()
+        self._check(self.lib.ufo_b200_page_in(self.h, buf.ctypes.data if len(buf) else None, len(buf), C.byref(st)))
+        return st.as_dict()
+
+    def pool_stats(self):
+        """Live bricks / upper nodes, pool capacities and device bytes of the map right now."""
+        st = PoolCounts()
+        self._check(self.lib.ufo_b200_pool_stats(self.h, C.byref(st)))
+        return st.as_dict()
+
     # -- state ----------------------------------------------------------------
     def value_field(self, sort=True):
         """(codes sorted, occ f32, rgb u8[n,3]): every voxel with a non-default payload.
@@ -846,6 +920,26 @@ class Map:
         p = np.array([occupied_thres, free_thres, prob_hit, prob_miss, clamping_thres_min,
                       clamping_thres_max], dtype=np.float64)
         self._check(self.lib.ufo_b200_set_sensor_model(self.h, p.ctypes.data))
+
+
+def page_info(blob):
+    """Header of a page blob (no map needed): version, color, depth_levels, resolution, n_bricks and
+    bytes, the size of the whole blob the header describes."""
+    buf = np.ascontiguousarray(np.frombuffer(blob, np.uint8))
+    h = PageHeader()
+    rc = load().ufo_b200_page_info(buf.ctypes.data if len(buf) else None, len(buf), C.byref(h))
+    if rc != OK:
+        raise UfoError(rc, "not a page blob of this library's format version")
+    return h.as_dict()
+
+
+def page_keys(blob):
+    """Brick coordinates (key >> 4 per axis) [n, 3] of the bricks a page blob holds, ascending by
+    packed key."""
+    n = page_info(blob)["n_bricks"]
+    k = np.frombuffer(blob, np.uint8)[64:64 + 8 * n].view(np.uint64)
+    m = np.uint64(0x1fffff)
+    return np.stack([k & m, (k >> np.uint64(21)) & m, (k >> np.uint64(42)) & m], axis=1).astype(np.uint32)
 
 
 def transform_points(frame_pose, xyz, dtype=np.float64):

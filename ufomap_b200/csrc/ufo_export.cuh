@@ -567,15 +567,14 @@ __device__ __forceinline__ void node_emit(const DeviceMap& M, const NodeFilter& 
 	}
 }
 
-// Per brick: the centre of its cube accumulated from the root, and whether every cube from the
-// root's children down to the brick itself passes the volume (the root is tested on the host).
-__global__ void __launch_bounds__(256) k_brick_chain(DeviceMap M, uint32_t n_bricks, Volume vol, uint8_t* ok_out, double* c_out)
+// The chain test of one brick: c receives the centre of its cube accumulated from the root; true iff
+// every cube from the root's children down to the brick itself passes the volume (the root is tested
+// on the host).
+__device__ __forceinline__ bool brick_chain(const DeviceMap& M, unsigned long long brick_key, const Volume& vol, double c[3])
 {
-	const uint32_t brick = blockIdx.x * blockDim.x + threadIdx.x;
-	if (brick >= n_bricks) return;
 	uint32_t kx, ky, kz;
-	unpack_key(M.brick_key[brick], kx, ky, kz);
-	double c[3] = {0.0, 0.0, 0.0};
+	unpack_key(brick_key, kx, ky, kz);
+	c[0] = c[1] = c[2] = 0.0;
 	bool ok = !((kx | ky | kz) & ~(M.g.key_mask >> 4));  // alias collector bricks own no voxels
 	for (uint32_t d = M.g.depth_levels; d > 4 && ok; --d) {
 		const uint32_t bit = d - 5;
@@ -587,6 +586,15 @@ __global__ void __launch_bounds__(256) k_brick_chain(DeviceMap M, uint32_t n_bri
 		c[2] = n[2];
 		ok = vol_hits(vol, c, M.g.half_size[d - 1]);
 	}
+	return ok;
+}
+
+__global__ void __launch_bounds__(256) k_brick_chain(DeviceMap M, uint32_t n_bricks, Volume vol, uint8_t* ok_out, double* c_out)
+{
+	const uint32_t brick = blockIdx.x * blockDim.x + threadIdx.x;
+	if (brick >= n_bricks) return;
+	double c[3];
+	const bool ok = brick_chain(M, M.brick_key[brick], vol, c);
 	ok_out[brick] = ok ? 1 : 0;
 	c_out[3 * (size_t)brick] = c[0];
 	c_out[3 * (size_t)brick + 1] = c[1];

@@ -34,6 +34,7 @@
 #include "ufo_import.cuh"
 #include "ufo_write.cuh"
 #include "ufo_early.cuh"
+#include "ufo_page.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -256,6 +257,40 @@ void reset_bbox(Map* m)
 	}
 }
 
+// capacities of a new map: the params' hint, or the default
+void initial_caps(const ufo_b200_params& p, uint32_t& bricks, uint32_t& upper)
+{
+	// a brick owns 64 block slots; the block hint is honoured through its brick equivalent
+	// (a touched brick of a lidar scan holds ~32 touched blocks)
+	const uint64_t bricks64 = p.initial_bricks ? p.initial_bricks : (p.initial_blocks ? p.initial_blocks / 32 : (1ull << 15));
+	bricks = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(bricks64, 16), 0x3ffffffull);
+	upper = std::max(bricks / 2, 4096u);
+}
+
+// the upper-node pool, its hash and the dirty lists of the propagation pass, empty
+void alloc_upper(Map* m, uint32_t up_cap)
+{
+	DeviceMap& M = m->M;
+	cudaStream_t s = m->stream;
+	size_t& tot = m->device_bytes;
+	M.up_cap = up_cap;
+	M.uh_mask = std::max(kMinHash, next_pow2(2ull * up_cap)) - 1;
+	dev_alloc(M.uh_keys, (size_t)M.uh_mask + 1, 0xff, s, tot);
+	dev_alloc(M.uh_vals, (size_t)M.uh_mask + 1, 0xff, s, tot);
+	dev_alloc(M.up_key, up_cap, 0, s, tot);
+	dev_alloc(M.up_agg, up_cap, 0, s, tot);
+	dev_alloc(M.up_stamp, up_cap, 0, s, tot);
+	dev_alloc(M.up_child, (size_t)up_cap * 8, 0, s, tot);
+	dev_alloc(M.up_valid, up_cap, 0, s, tot);
+	dev_alloc(M.up_parent, up_cap, 0xff, s, tot);
+	dev_alloc(m->d_list[0], up_cap, 0, s, tot);
+	dev_alloc(m->d_list[1], up_cap, 0, s, tot);
+	if (M.color) {
+		dev_alloc(M.up_rgb, up_cap, 0, s, tot);
+		dev_alloc(M.up_child_rgb, (size_t)up_cap * 8, 0, s, tot);
+	}
+}
+
 void alloc_pools(Map* m, uint32_t brick_cap, uint32_t up_cap)
 {
 	DeviceMap& M = m->M;
@@ -263,9 +298,7 @@ void alloc_pools(Map* m, uint32_t brick_cap, uint32_t up_cap)
 	size_t& tot = m->device_bytes;
 	const size_t nb = (size_t)brick_cap * 64;  // block slots: 64 consecutive per brick
 	M.brick_cap = brick_cap;
-	M.up_cap = up_cap;
 	M.bh_mask = std::max(kMinHash, next_pow2(2ull * brick_cap)) - 1;
-	M.uh_mask = std::max(kMinHash, next_pow2(2ull * up_cap)) - 1;
 	dev_alloc(M.bh_tab, (size_t)M.bh_mask + 1, 0xff, s, tot);
 	dev_alloc(M.brick_key, brick_cap, 0, s, tot);
 	dev_alloc(M.brick_stamp, brick_cap, 0, s, tot);
@@ -281,25 +314,14 @@ void alloc_pools(Map* m, uint32_t brick_cap, uint32_t up_cap)
 	dev_alloc(M.hit_mask, nb, 0, s, tot);
 	dev_alloc(M.meta, nb, 0, s, tot);
 	dev_alloc(M.pair_max, nb, 0, s, tot);
-	dev_alloc(M.uh_keys, (size_t)M.uh_mask + 1, 0xff, s, tot);
-	dev_alloc(M.uh_vals, (size_t)M.uh_mask + 1, 0xff, s, tot);
-	dev_alloc(M.up_key, up_cap, 0, s, tot);
-	dev_alloc(M.up_agg, up_cap, 0, s, tot);
-	dev_alloc(M.up_stamp, up_cap, 0, s, tot);
-	dev_alloc(M.up_child, (size_t)up_cap * 8, 0, s, tot);
-	dev_alloc(M.up_valid, up_cap, 0, s, tot);
-	dev_alloc(M.up_parent, up_cap, 0xff, s, tot);
 	dev_alloc(M.brick_parent, brick_cap, 0xff, s, tot);
-	dev_alloc(m->d_list[0], up_cap, 0, s, tot);
-	dev_alloc(m->d_list[1], up_cap, 0, s, tot);
+	alloc_upper(m, up_cap);
 	if (M.color) {
 		dev_alloc(M.brick_rgb3, (size_t)brick_cap * 8, 0, s, tot);
 		dev_alloc(M.brick_rgb4, brick_cap, 0, s, tot);
 		dev_alloc(M.leaf_rgb, nb * 64, 0, s, tot);
 		dev_alloc(M.sum1_rgb, nb * 8, 0, s, tot);
 		dev_alloc(M.rgb2, nb, 0, s, tot);
-		dev_alloc(M.up_rgb, up_cap, 0, s, tot);
-		dev_alloc(M.up_child_rgb, (size_t)up_cap * 8, 0, s, tot);
 	}
 	dev_alloc(M.ctr, 1, 0, s, tot);
 }
@@ -1700,12 +1722,8 @@ int ufo_b200_create(const ufo_b200_params* p, ufo_b200_map** out)
 		m->cmin_log = to_logit(p->clamping_thres_min);
 		m->cmax_log = to_logit(p->clamping_thres_max);
 		refresh_model(m);
-		// a brick owns 64 block slots; the block hint is honoured through its brick equivalent
-		// (a touched brick of a lidar scan holds ~32 touched blocks)
-		uint64_t bricks64 = p->initial_bricks ? p->initial_bricks
-		                                      : (p->initial_blocks ? p->initial_blocks / 32 : (1ull << 15));
-		uint32_t bricks = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(bricks64, 16), 0x3ffffffull);
-		uint32_t upper = std::max(bricks / 2, 4096u);
+		uint32_t bricks, upper;
+		initial_caps(*p, bricks, upper);
 		alloc_pools(m, bricks, upper);
 		m->n_blocks = 0;
 		m->n_bricks = 0;
@@ -4127,8 +4145,606 @@ int ufo_b200_insert_rays(ufo_b200_map* m, const double* origins, const double* e
 
 }  // extern "C"
 
+// ---------------------------------------------------------------------------
+// retain / page out / page in (ufo_page.cuh)
+// ---------------------------------------------------------------------------
+namespace
+{
+// device / pinned buffers and events of one call
+struct DevBuf {
+	void* p = nullptr;
+	DevBuf() = default;
+	DevBuf(const DevBuf&) = delete;
+	DevBuf& operator=(const DevBuf&) = delete;
+	~DevBuf()
+	{
+		if (p) cudaFree(p);
+	}
+	template <class T>
+	T* alloc(size_t n)
+	{
+		CK(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)));
+		return static_cast<T*>(p);
+	}
+};
 
+struct Events {
+	cudaEvent_t e[4] = {};
+	Events()
+	{
+		for (auto& x : e) CK(cudaEventCreate(&x));
+	}
+	Events(const Events&) = delete;
+	Events& operator=(const Events&) = delete;
+	~Events()
+	{
+		for (auto& x : e)
+			if (x) cudaEventDestroy(x);
+	}
+};
 
+// Pinned staging for the sections of a page: two chunks of a bounded size on each side, so that the
+// host's copy of one chunk overlaps the device's work on the next and a page of any size needs
+// 2 x kPageChunk of pinned memory.
+constexpr size_t kPageChunk = 16u << 20;
+struct PageStage {
+	uint8_t* pin[2] = {};
+	uint8_t* dev[2] = {};
+	cudaEvent_t ev[2] = {};
+	PageStage()
+	{
+		for (int b = 0; b < 2; ++b) {
+			CK(cudaHostAlloc(reinterpret_cast<void**>(&pin[b]), kPageChunk, cudaHostAllocDefault));
+			CK(cudaMalloc(reinterpret_cast<void**>(&dev[b]), kPageChunk));
+			CK(cudaEventCreateWithFlags(&ev[b], cudaEventDisableTiming));
+		}
+	}
+	PageStage(const PageStage&) = delete;
+	PageStage& operator=(const PageStage&) = delete;
+	~PageStage()
+	{
+		for (int b = 0; b < 2; ++b) {
+			if (pin[b]) cudaFreeHost(pin[b]);
+			if (dev[b]) cudaFree(dev[b]);
+			if (ev[b]) cudaEventDestroy(ev[b]);
+		}
+	}
+};
 
+// One section of a page-out: gather(device chunk, first brick, bricks) fills a device chunk, which
+// goes to pinned memory and from there into the caller's buffer.
+template <class Gather>
+void page_section_out(cudaStream_t s, PageStage& st, size_t n, size_t brick_bytes, uint8_t* dst, Gather&& gather)
+{
+	const size_t chunk = kPageChunk / brick_bytes;
+	int wait_b = -1;
+	size_t wait_first = 0, wait_n = 0;
+	auto drain = [&]() {
+		if (wait_b < 0) return;
+		CK(cudaEventSynchronize(st.ev[wait_b]));
+		memcpy(dst + wait_first * brick_bytes, st.pin[wait_b], wait_n * brick_bytes);
+	};
+	for (size_t first = 0, i = 0; first < n; first += chunk, ++i) {
+		const int b = (int)(i & 1);
+		const size_t cnt = std::min(chunk, n - first);
+		gather(st.dev[b], first, cnt);
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(st.pin[b], st.dev[b], cnt * brick_bytes, cudaMemcpyDeviceToHost, s));
+		CK(cudaEventRecord(st.ev[b], s));
+		drain();
+		wait_b = b;
+		wait_first = first;
+		wait_n = cnt;
+	}
+	drain();
+}
 
+// One section of a page-in: the caller's bytes go through pinned memory into a device chunk, which
+// scatter(device chunk, first brick, bricks) applies.
+template <class Scatter>
+void page_section_in(cudaStream_t s, PageStage& st, size_t n, size_t brick_bytes, const uint8_t* src, Scatter&& scatter)
+{
+	const size_t chunk = kPageChunk / brick_bytes;
+	bool used[2] = {false, false};
+	for (size_t first = 0, i = 0; first < n; first += chunk, ++i) {
+		const int b = (int)(i & 1);
+		const size_t cnt = std::min(chunk, n - first);
+		if (used[b]) CK(cudaEventSynchronize(st.ev[b]));  // the copy out of this pinned chunk has finished
+		memcpy(st.pin[b], src + first * brick_bytes, cnt * brick_bytes);
+		CK(cudaMemcpyAsync(st.dev[b], st.pin[b], cnt * brick_bytes, cudaMemcpyHostToDevice, s));
+		CK(cudaEventRecord(st.ev[b], s));
+		used[b] = true;
+		scatter(st.dev[b], first, cnt);
+		CK(cudaGetLastError());
+	}
+	CK(cudaStreamSynchronize(s));
+}
 
+// moves `n` whole bricks of `brick_bytes` each (k_page_move) with the widest word that divides a brick
+template <bool SCATTER>
+void launch_page_move(Map* m, void* dst, const void* src, const uint32_t* slot, size_t n, size_t brick_bytes)
+{
+	if (!n) return;
+	auto run = [&](auto* d, size_t word) {
+		using V = std::remove_pointer_t<decltype(d)>;
+		const size_t per = brick_bytes / word;
+		uint32_t lg = 0;
+		while (((size_t)1 << lg) < per) ++lg;
+		const size_t units = n * per;
+		const uint32_t grid = (uint32_t)std::min<size_t>((units + 255) / 256, (size_t)m->sm_count * 32);
+		k_page_move<V, SCATTER><<<grid, 256, 0, m->stream>>>(d, static_cast<const V*>(src), slot, units, lg);
+	};
+	if (brick_bytes % 16 == 0) run(static_cast<uint4*>(dst), 16);
+	else if (brick_bytes % 8 == 0) run(static_cast<uint2*>(dst), 8);
+	else run(static_cast<uint32_t*>(dst), 4);
+	++m->launches;
+}
+
+// checks shared by retain, page-out and page-in; they need no device
+int page_allowed(Map* m, const char* what)
+{
+	if (m->M.g.depth_levels < 5) {
+		m->set_error("%s needs depth_levels >= 5", what);
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (m->M.route_world > 1 || m->route_stage != 0) {
+		m->set_error("%s on a routed map is not supported", what);
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (m->poisoned) {
+		m->set_error("an earlier scan failed half-way; ufo_b200_clear() the map first");
+		return UFO_B200_E_INVALID;
+	}
+	return UFO_B200_OK;
+}
+
+// keep flags of the live bricks and, for a page-out, the sort keys / slots / count of the bricks to write
+void launch_page_classify(Map* m, const Volume& vol, DeviceVolume& dvol, uint32_t* d_keep, unsigned long long* d_skey,
+                          uint32_t* d_slot, uint32_t* d_count)
+{
+	const double c0[3] = {0.0, 0.0, 0.0};
+	const int none = vol_hits(vol, c0, m->M.g.half_size[m->M.g.depth_levels]) ? 0 : 1;  // the root misses
+	Volume hv = vol;
+	volume_is_general(hv);
+	const Volume dv = dvol.upload(hv, m->stream);
+	k_page_classify<<<(m->n_bricks + 255) / 256, 256, 0, m->stream>>>(m->M, m->n_bricks, dv, none, d_keep, d_skey, d_slot, d_count);
+	CK(cudaGetLastError());
+	++m->launches;
+}
+
+void fill_pool_state(Map* m, uint64_t& bricks, uint64_t& cap, uint64_t& bytes)
+{
+	bricks = m->n_bricks;
+	cap = m->M.brick_cap;
+	bytes = m->device_bytes;
+}
+
+// The levels above the bricks from the depth-4 aggregates of bricks slot[0..n) (nullptr: 0..n): the
+// scan's push-up pass with these bricks as its touched list.  `derived`: first recompute the bricks'
+// own depth 1-4 values from their leaves, as an import does.
+void page_propagate(Map* m, const uint32_t* d_slot, uint32_t n, bool derived)
+{
+	DeviceMap& M = m->M;
+	cudaStream_t s = m->stream;
+	for (int attempt = 0;; ++attempt) {
+		M.up_epoch++;
+		push_counters(m);
+		k_page_touch<<<std::max(1u, std::min((n + 255) / 256, (uint32_t)m->sm_count * 4)), 256, 0, s>>>(M, d_slot, n);
+		if (derived) {
+			k_import_refresh<<<m->sm_count * 8, 256, 0, s>>>(M);
+			if (M.color) k_brick_agg<true><<<m->sm_count * 4, 256, 0, s>>>(M);
+			else k_brick_agg<false><<<m->sm_count * 4, 256, 0, s>>>(M);
+		}
+		launch_upper(m);
+		CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		const uint32_t ov = m->h_ctr->overflow;
+		if (!ov) break;
+		if (attempt > 16 || (ov & ~4u)) {
+			m->set_error("the upper-node pool keeps overflowing (flags %u)", ov);
+			m->poisoned = true;
+			throw MapError{UFO_B200_E_NOMEM};
+		}
+		// every step above is idempotent: keep the nodes that were created, grow and run it again
+		m->n_upper = std::min(m->h_ctr->n_upper, M.up_cap);
+		grow_pools(m, 4u, 0, m->h_ctr->n_upper);
+	}
+	m->n_upper = std::min(m->h_ctr->n_upper, M.up_cap);
+}
+
+int retain(Map* m, const Volume& vol, ufo_b200_retain_stats* out)
+{
+	const int allowed = page_allowed(m, "retain");
+	if (allowed != UFO_B200_OK) return allowed;
+	CK(cudaSetDevice(m->device));
+	sync_map(m);
+	DeviceMap& M = m->M;
+	cudaStream_t s = m->stream;
+	ufo_b200_retain_stats st{};
+	fill_pool_state(m, st.bricks_before, st.brick_cap_before, st.device_bytes_before);
+	st.bricks_kept = st.bricks_before;
+	fill_pool_state(m, st.bricks_kept, st.brick_cap_after, st.device_bytes_after);
+	const uint32_t n = m->n_bricks;
+	uint32_t kept = n;
+	DevBuf b_keep, b_new, b_src, b_tmp;
+	uint32_t* d_src = nullptr;
+	Events ev;
+	if (vol.n && n) {
+		uint32_t* d_keep = b_keep.alloc<uint32_t>(n);
+		uint32_t* d_new = b_new.alloc<uint32_t>(n);
+		d_src = b_src.alloc<uint32_t>(n);
+		size_t tmp_bytes = 0;
+		CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_keep, d_new, (int)n, s));
+		void* d_tmp = b_tmp.alloc<uint8_t>(tmp_bytes);
+		DeviceVolume dvol;
+		CK(cudaEventRecord(ev.e[0], s));
+		launch_page_classify(m, vol, dvol, d_keep, nullptr, nullptr, nullptr);
+		CK(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_keep, d_new, (int)n, s));
+		k_page_sources<<<(n + 255) / 256, 256, 0, s>>>(n, d_keep, d_new, d_src);
+		CK(cudaGetLastError());
+		m->launches += 2;
+		CK(cudaEventRecord(ev.e[1], s));
+		uint32_t last[2] = {0, 0};
+		CK(cudaMemcpyAsync(&last[0], d_new + (n - 1), 4, cudaMemcpyDeviceToHost, s));
+		CK(cudaMemcpyAsync(&last[1], d_keep + (n - 1), 4, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		kept = last[0] + last[1];
+		CK(cudaEventElapsedTime(&st.ms_classify, ev.e[0], ev.e[1]));
+	}
+	if (kept == n) {  // nothing to remove: the map stays as it is, bit for bit
+		if (out) *out = st;
+		return UFO_B200_OK;
+	}
+
+	uint32_t cap0, up0;
+	initial_caps(m->params, cap0, up0);
+	const uint32_t oc = M.brick_cap;
+	const uint32_t nc = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(cap0, 2ull * kept), 0x3ffffffull);
+	size_t& tot = m->device_bytes;
+	// One array at a time: allocate the new one, gather the survivors, free the old one.  `per`:
+	// elements per brick; the slots past the survivors get the array's initial fill.
+	auto compact = [&](auto*& p, size_t per, int fill) {
+		using T = std::remove_reference_t<decltype(*p)>;
+		if (!p) return;
+		T* q = nullptr;
+		CK(cudaMalloc(reinterpret_cast<void**>(&q), (size_t)nc * per * sizeof(T)));
+		launch_page_move<false>(m, q, p, d_src, kept, per * sizeof(T));
+		CK(cudaMemsetAsync(q + (size_t)kept * per, fill, (size_t)(nc - kept) * per * sizeof(T), s));
+		CK(cudaStreamSynchronize(s));
+		CK(cudaFree(p));
+		p = q;
+		tot = tot - (size_t)oc * per * sizeof(T) + (size_t)nc * per * sizeof(T);
+	};
+	// per-scan lists and everything above the bricks start from their initial state
+	auto renew = [&](auto*& p, size_t n_new, size_t n_old, int fill) {
+		using T = std::remove_reference_t<decltype(*p)>;
+		if (!p) return;
+		CK(cudaFree(p));
+		tot -= n_old * sizeof(T);
+		dev_alloc(p, n_new, fill, s, tot);
+	};
+	CK(cudaEventRecord(ev.e[1], s));
+	// The leaves first: they are most of the map, so if the device cannot hold one more array this
+	// fails before anything has changed.  Every later array is smaller than what has been freed.
+	compact(M.leaf, 64 * 64, 0);
+	try {
+		compact(M.leaf_rgb, 64 * 64, 0);
+		compact(M.miss_mask, 64, 0);
+		compact(M.hit_mask, 64, 0);
+		compact(M.chg_mask, 64, 0);
+		compact(m->chg_paused, 64, 0);
+		compact(M.meta, 64, 0);
+		compact(M.pair_max, 64, 0);
+		compact(M.sum1_rgb, 64 * 8, 0);
+		compact(M.rgb2, 64, 0);
+		compact(M.alias_miss, 64, 0);
+		compact(M.alias_hit, 64, 0);
+		compact(M.brick_key, 1, 0);
+		compact(M.brick_stamp, 1, 0);
+		compact(M.hit_stamp, 1, 0);
+		compact(M.brick_sum3, 8, 0);
+		compact(M.brick_sum4, 1, 0);
+		compact(M.brick_rgb3, 8, 0);
+		compact(M.brick_rgb4, 1, 0);
+		CK(cudaEventRecord(ev.e[2], s));
+		renew(M.touched, nc, oc, 0);
+		renew(M.touched_alt, nc, oc, 0);
+		renew(M.touched_mi, nc, oc, 0);
+		renew(M.touched_alt_mi, nc, oc, 0);
+		renew(M.brick_parent, nc, oc, 0xff);
+		M.brick_cap = nc;
+		renew(M.bh_tab, (size_t)std::max(kMinHash, next_pow2(2ull * nc)), (size_t)M.bh_mask + 1, 0xff);
+		M.bh_mask = std::max(kMinHash, next_pow2(2ull * nc)) - 1;
+		if (kept) {
+			k_rebuild_brick_hash<<<(kept + 255) / 256, 256, 0, s>>>(M, kept);
+			++m->launches;
+		}
+		// the upper-node pool, in proportion, rebuilt from the survivors' depth-4 aggregates: a child
+		// that never reports counts as never-touched space, which is what a removed brick now is
+		const size_t ou = M.up_cap, ouh = (size_t)M.uh_mask + 1;
+		for (void* p : {(void*)M.uh_keys, (void*)M.uh_vals, (void*)M.up_key, (void*)M.up_agg, (void*)M.up_stamp, (void*)M.up_child,
+		                (void*)M.up_valid, (void*)M.up_parent, (void*)m->d_list[0], (void*)m->d_list[1], (void*)M.up_rgb,
+		                (void*)M.up_child_rgb})
+			if (p) CK(cudaFree(p));
+		tot -= ouh * 12 + ou * (8 + sizeof(Agg) + 4 + 8 * sizeof(Agg) + 4 + 4 + 4 + 4) + (M.color ? ou * (4 + 8 * 4) : 0);
+		M.up_rgb = M.up_child_rgb = nullptr;
+		alloc_upper(m, std::max(up0, nc / 2));
+		m->n_bricks = kept;
+		m->n_upper = 0;
+		page_propagate(m, nullptr, kept, false);
+		CK(cudaEventRecord(ev.e[3], s));
+		// blocks that hold a written octet, for the statistics of later scans
+		DevBuf b_cnt;
+		unsigned long long* d_cnt = b_cnt.alloc<unsigned long long>(1);
+		unsigned long long blocks = 0;
+		CK(cudaMemsetAsync(d_cnt, 0, 8, s));
+		if (kept) k_page_count_blocks<<<m->sm_count * 4, 256, 0, s>>>(M.meta, (size_t)kept * 64, d_cnt);
+		CK(cudaMemcpyAsync(&blocks, d_cnt, 8, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		m->n_blocks = (uint32_t)blocks;
+	} catch (...) {
+		// the arrays no longer agree on their slots
+		m->poisoned = true;
+		m->set_error("retain failed after the leaves were compacted; the map is unusable");
+		throw;
+	}
+	CK(cudaEventElapsedTime(&st.ms_compact, ev.e[1], ev.e[2]));
+	CK(cudaEventElapsedTime(&st.ms_upper, ev.e[2], ev.e[3]));
+	st.bricks_kept = kept;
+	st.bricks_removed = n - kept;
+	fill_pool_state(m, st.bricks_kept, st.brick_cap_after, st.device_bytes_after);
+	if (out) *out = st;
+	return UFO_B200_OK;
+}
+
+int page_out(Map* m, const Volume& vol, void* buf, size_t cap, size_t* size)
+{
+	const int allowed = page_allowed(m, "page_out");
+	if (allowed != UFO_B200_OK) return allowed;
+	CK(cudaSetDevice(m->device));
+	sync_map(m);
+	DeviceMap& M = m->M;
+	cudaStream_t s = m->stream;
+	const uint32_t n = m->n_bricks;
+	const bool color = M.color != 0;
+	uint32_t cnt = 0;
+	DevBuf b_key[2], b_slot[2], b_cnt, b_tmp;
+	unsigned long long* d_key[2] = {nullptr, nullptr};
+	uint32_t* d_slot[2] = {nullptr, nullptr};
+	if (vol.n && n) {
+		for (int k = 0; k < 2; ++k) {
+			d_key[k] = b_key[k].alloc<unsigned long long>(n);
+			d_slot[k] = b_slot[k].alloc<uint32_t>(n);
+		}
+		uint32_t* d_cnt = b_cnt.alloc<uint32_t>(1);
+		CK(cudaMemsetAsync(d_cnt, 0, 4, s));
+		DeviceVolume dvol;
+		launch_page_classify(m, vol, dvol, nullptr, d_key[0], d_slot[0], d_cnt);
+		CK(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+	}
+	*size = page_bytes(cnt, color);
+	if (!buf || cap < *size) return UFO_B200_OK;
+
+	uint8_t* o = static_cast<uint8_t*>(buf);
+	PageHeader h{};
+	h.magic = kPageMagic;
+	h.version = kPageVersion;
+	h.color = color ? 1u : 0u;
+	memcpy(&h.resolution_bits, &m->params.resolution, 8);
+	h.depth_levels = M.g.depth_levels;
+	h.n_bricks = cnt;
+	memcpy(o, &h, sizeof(h));
+	if (!cnt) return UFO_B200_OK;
+	// ascending packed key: equal maps give equal blobs whatever their slot order
+	size_t tmp_bytes = 0;
+	CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_key[0], d_key[1], d_slot[0], d_slot[1], (int)n, 0, 64, s));
+	void* d_tmp = b_tmp.alloc<uint8_t>(tmp_bytes);
+	CK(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_key[0], d_key[1], d_slot[0], d_slot[1], (int)n, 0, 64, s));
+	++m->launches;
+	const uint32_t* slots = d_slot[1];
+	o += sizeof(h);
+	CK(cudaMemcpyAsync(o, d_key[1], (size_t)cnt * 8, cudaMemcpyDeviceToHost, s));
+	CK(cudaStreamSynchronize(s));
+	o += (size_t)cnt * 8;
+	PageStage stage;
+	page_section_out(s, stage, cnt, kPageLeafBytes, o, [&](uint8_t* d, size_t first, size_t k) {
+		launch_page_move<false>(m, d, M.leaf, slots + first, k, kPageLeafBytes);
+	});
+	o += (size_t)cnt * kPageLeafBytes;
+	page_section_out(s, stage, cnt, kPageBitsBytes, o, [&](uint8_t* d, size_t first, size_t k) {
+		k_page_bits_out<<<(uint32_t)std::min<size_t>((k * 64 + 255) / 256, (size_t)m->sm_count * 8), 256, 0, s>>>(M.meta, slots + first, k * 64, d);
+		++m->launches;
+	});
+	o += (size_t)cnt * kPageBitsBytes;
+	if (color)
+		page_section_out(s, stage, cnt, kPageLeafBytes, o, [&](uint8_t* d, size_t first, size_t k) {
+			launch_page_move<false>(m, d, M.leaf_rgb, slots + first, k, kPageLeafBytes);
+		});
+	return UFO_B200_OK;
+}
+
+int page_header_ok(const void* blob, size_t size, PageHeader& h)
+{
+	if (!blob || size < sizeof(PageHeader)) return 1;
+	memcpy(&h, blob, sizeof(h));
+	if (h.magic != kPageMagic) return 2;
+	if (h.version != kPageVersion) return 3;
+	return 0;
+}
+
+int page_in(Map* m, const void* blob, size_t size, ufo_b200_retain_stats* out)
+{
+	const int allowed = page_allowed(m, "page_in");
+	if (allowed != UFO_B200_OK) return allowed;
+	DeviceMap& M = m->M;
+	PageHeader h{};
+	switch (page_header_ok(blob, size, h)) {
+		case 0: break;
+		case 1: m->set_error("page_in: %zu bytes are less than a page header", size); return UFO_B200_E_INVALID;
+		case 2: m->set_error("page_in: not a page blob (bad magic)"); return UFO_B200_E_INVALID;
+		default: m->set_error("page_in: page format version %u, this library reads version %u", h.version, kPageVersion); return UFO_B200_E_INVALID;
+	}
+	const bool color = M.color != 0;
+	unsigned long long res_bits;
+	memcpy(&res_bits, &m->params.resolution, 8);
+	if ((h.color != 0) != color || h.color > 1) {
+		m->set_error("page_in: the blob is from a %s map, this is a %s map", h.color ? "colour" : "mono", color ? "colour" : "mono");
+		return UFO_B200_E_INVALID;
+	}
+	if (h.resolution_bits != res_bits || h.depth_levels != M.g.depth_levels) {
+		double r;
+		memcpy(&r, &h.resolution_bits, 8);
+		m->set_error("page_in: the blob is from a map of resolution %.17g and %u depth levels, this map has %.17g and %u", r,
+		             h.depth_levels, m->params.resolution, M.g.depth_levels);
+		return UFO_B200_E_INVALID;
+	}
+	if (h.n_bricks > 0x3ffffffull || size != page_bytes(h.n_bricks, color)) {
+		m->set_error("page_in: the header says %llu bricks, which does not match the blob's %zu bytes", h.n_bricks, size);
+		return UFO_B200_E_INVALID;
+	}
+	CK(cudaSetDevice(m->device));
+	sync_map(m);
+	cudaStream_t s = m->stream;
+	ufo_b200_retain_stats st{};
+	fill_pool_state(m, st.bricks_before, st.brick_cap_before, st.device_bytes_before);
+	fill_pool_state(m, st.bricks_kept, st.brick_cap_after, st.device_bytes_after);
+	const uint32_t n = (uint32_t)h.n_bricks;
+	if (!n) {
+		if (out) *out = st;
+		return UFO_B200_OK;
+	}
+	const uint8_t* p_keys = static_cast<const uint8_t*>(blob) + sizeof(PageHeader);
+	const uint8_t* p_leaf = p_keys + (size_t)n * 8;
+	const uint8_t* p_bits = p_leaf + (size_t)n * kPageLeafBytes;
+	const uint8_t* p_rgb = p_bits + (size_t)n * kPageBitsBytes;
+
+	DevBuf b_keys, b_slot, b_cnt, b_bits;
+	unsigned long long* d_keys = b_keys.alloc<unsigned long long>(n);
+	uint32_t* d_slot = b_slot.alloc<uint32_t>(n);
+	uint32_t* d_cnt = b_cnt.alloc<uint32_t>(2);
+	Events ev;
+	CK(cudaEventRecord(ev.e[0], s));
+	CK(cudaMemcpyAsync(d_keys, p_keys, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+	CK(cudaMemsetAsync(d_cnt, 0, 8, s));
+	// its own pass, before anything is created: a refusal leaves no brick behind
+	k_page_lookup<<<(n + 255) / 256, 256, 0, s>>>(M, d_keys, n, d_cnt);
+	CK(cudaGetLastError());
+	++m->launches;
+	uint32_t counts[2] = {0, 0};
+	CK(cudaMemcpyAsync(counts, d_cnt, 8, cudaMemcpyDeviceToHost, s));
+	CK(cudaStreamSynchronize(s));
+	if (counts[1]) {
+		m->set_error("page_in: %u of the blob's %u brick keys lie outside the map or are out of order", counts[1], n);
+		return UFO_B200_E_INVALID;
+	}
+	if (counts[0]) {
+		m->set_error("page_in: %u of the blob's %u bricks exist in the map; a page cannot be merged into existing bricks", counts[0], n);
+		return UFO_B200_E_INVALID;
+	}
+	// Every brick first, nothing written until all exist: creation is idempotent, so a pass that
+	// ran into a full pool is repeated as a whole after the pool has grown.
+	for (int attempt = 0;; ++attempt) {
+		push_counters(m);
+		k_page_create<<<(n + 255) / 256, 256, 0, s>>>(M, d_keys, n, d_slot);
+		CK(cudaGetLastError());
+		++m->launches;
+		CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		const uint32_t ov = m->h_ctr->overflow;
+		m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
+		if (!ov) break;
+		if (attempt > 16) {
+			m->set_error("page_in: device pools keep overflowing");
+			return UFO_B200_E_NOMEM;
+		}
+		grow_pools(m, ov & 6u, m->h_ctr->n_bricks, m->h_ctr->n_upper);
+	}
+	CK(cudaEventRecord(ev.e[1], s));
+	{
+		PageStage stage;
+		page_section_in(s, stage, n, kPageLeafBytes, p_leaf, [&](uint8_t* d, size_t first, size_t k) {
+			launch_page_move<true>(m, M.leaf, d, d_slot + first, k, kPageLeafBytes);
+		});
+		if (color)
+			page_section_in(s, stage, n, kPageLeafBytes, p_rgb, [&](uint8_t* d, size_t first, size_t k) {
+				launch_page_move<true>(m, M.leaf_rgb, d, d_slot + first, k, kPageLeafBytes);
+			});
+		page_section_in(s, stage, n, kPageBitsBytes, p_bits, [&](uint8_t* d, size_t first, size_t k) {
+			k_page_bits_in<<<(uint32_t)std::min<size_t>((k * 64 + 255) / 256, (size_t)m->sm_count * 8), 256, 0, s>>>(M.meta, d_slot + first, k * 64, d);
+			++m->launches;
+		});
+	}
+	CK(cudaEventRecord(ev.e[2], s));
+	// pair maxima, flags, inner colours, depth 3 / 4 and the levels above, under the current sensor model
+	page_propagate(m, d_slot, n, true);
+	CK(cudaEventRecord(ev.e[3], s));
+	CK(cudaStreamSynchronize(s));
+	size_t blocks = 0;
+	for (size_t i = 0; i < (size_t)n * 64; ++i) blocks += p_bits[i] ? 1 : 0;
+	m->n_blocks += (uint32_t)blocks;
+	CK(cudaEventElapsedTime(&st.ms_classify, ev.e[0], ev.e[1]));
+	CK(cudaEventElapsedTime(&st.ms_compact, ev.e[1], ev.e[2]));
+	CK(cudaEventElapsedTime(&st.ms_upper, ev.e[2], ev.e[3]));
+	fill_pool_state(m, st.bricks_kept, st.brick_cap_after, st.device_bytes_after);
+	if (out) *out = st;
+	return UFO_B200_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int ufo_b200_retain_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, ufo_b200_retain_stats* out)
+{
+	if (!m) return UFO_B200_E_INVALID;
+	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() { return retain(m, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, out); });
+}
+
+int ufo_b200_retain(ufo_b200_map* m, const double box6[6], ufo_b200_retain_stats* out)
+{
+	if (!m || !box6) return UFO_B200_E_INVALID;
+	const VolRec r = aabb_record(box6);
+	return ufo_b200_retain_bv(m, reinterpret_cast<const ufo_b200_volume*>(&r), 1, out);
+}
+
+int ufo_b200_page_out_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, void* buf, size_t cap, size_t* size)
+{
+	if (!m || !size) return UFO_B200_E_INVALID;
+	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() { return page_out(m, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, buf, cap, size); });
+}
+
+int ufo_b200_page_in(ufo_b200_map* m, const void* blob, size_t size, ufo_b200_retain_stats* out)
+{
+	if (!m || (!blob && size)) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() { return page_in(m, blob, size, out); });
+}
+
+int ufo_b200_page_info(const void* blob, size_t size, ufo_b200_page_header* out)
+{
+	if (!out) return UFO_B200_E_INVALID;
+	PageHeader h{};
+	if (page_header_ok(blob, size, h) || h.color > 1 || h.n_bricks > 0x3ffffffull) return UFO_B200_E_INVALID;
+	*out = ufo_b200_page_header{};
+	out->version = h.version;
+	out->color = h.color;
+	out->depth_levels = h.depth_levels;
+	memcpy(&out->resolution, &h.resolution_bits, 8);
+	out->n_bricks = h.n_bricks;
+	out->bytes = page_bytes(h.n_bricks, h.color != 0);
+	return UFO_B200_OK;
+}
+
+int ufo_b200_pool_stats(ufo_b200_map* m, ufo_b200_pool_counts* out)
+{
+	if (!m || !out) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() {
+		CK(cudaSetDevice(m->device));
+		sync_map(m);
+		*out = ufo_b200_pool_counts{m->n_bricks, m->M.brick_cap, m->n_upper, m->M.up_cap, m->device_bytes};
+		return (int)UFO_B200_OK;
+	});
+}
+
+}  // extern "C"
