@@ -24,6 +24,7 @@
 #include <cstring>
 #include <new>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/ufomap_b200.h"
@@ -64,30 +65,27 @@ struct CudaError {
 		if (e__ != cudaSuccess) throw CudaError{e__, #call, __LINE__}; \
 	} while (0)
 
-template <class T>
-void dev_alloc(T*& p, size_t n, int fill_byte, cudaStream_t s, size_t& total)
-{
-	p = nullptr;
-	if (n == 0) n = 1;
-	CK(cudaMalloc(reinterpret_cast<void**>(&p), n * sizeof(T)));
-	CK(cudaMemsetAsync(p, fill_byte, n * sizeof(T), s));
-	total += n * sizeof(T);
-}
-
-// grow p from old_n to new_n elements (new part filled with fill_byte)
-template <class T>
-void dev_grow(T*& p, size_t old_n, size_t new_n, int fill_byte, cudaStream_t s, size_t& total)
-{
-	if (!p) return;
-	T* q = nullptr;
-	CK(cudaMalloc(reinterpret_cast<void**>(&q), new_n * sizeof(T)));
-	CK(cudaMemcpyAsync(q, p, old_n * sizeof(T), cudaMemcpyDeviceToDevice, s));
-	CK(cudaMemsetAsync(q + old_n, fill_byte, (new_n - old_n) * sizeof(T), s));
-	CK(cudaStreamSynchronize(s));
-	CK(cudaFree(p));
-	p = q;
-	total += (new_n - old_n) * sizeof(T);
-}
+// Device memory for the duration of one call, freed on every way out of it.
+struct DevBuf {
+	void* p = nullptr;
+	DevBuf() = default;
+	DevBuf(const DevBuf&) = delete;
+	DevBuf& operator=(const DevBuf&) = delete;
+	~DevBuf() { release(); }
+	// n elements of T (at least one), uninitialised, in place of what the buffer held
+	template <class T>
+	T* alloc(size_t n)
+	{
+		release();
+		CK(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)));
+		return static_cast<T*>(p);
+	}
+	void release()
+	{
+		if (p) cudaFree(p);
+		p = nullptr;
+	}
+};
 
 double to_logit(double p) { return std::log(p / (1.0 - p)); }
 }  // namespace
@@ -113,6 +111,24 @@ struct PendingScan {
 	WriteArgs w{};
 };
 
+// Device memory a map holds across calls, and its size.  Every such allocation, these and the pool
+// arrays of kPool, is made and freed by map_realloc, so device_bytes is the sum of the live ones.
+template <class T>
+struct DevMem {
+	T* p = nullptr;
+	size_t bytes = 0;
+	DevMem() = default;
+	DevMem(const DevMem&) = delete;
+	DevMem& operator=(const DevMem&) = delete;
+	~DevMem()
+	{
+		if (p) cudaFree(p);  // the map goes with it: nothing left to account for
+	}
+	// at least n bytes; a new allocation is filled with the byte `fill` (< 0: left uninitialised)
+	void ensure(ufo_b200_map* m, size_t n, int fill);
+	void release(ufo_b200_map* m);
+};
+
 struct ufo_b200_map {
 	ufo_b200_params params{};
 	DeviceMap M{};
@@ -123,55 +139,60 @@ struct ufo_b200_map {
 	double occ_thr_log = 0, free_thr_log = 0, hit_log = 0, miss_log = 0, cmin_log = 0, cmax_log = 0;
 	// host mirror of the counters (pinned)
 	Counters* h_ctr = nullptr;
+	// owners of the device memory DeviceMap sees outside the pool arrays: counters, the hashes of the
+	// two pools and the dense scan volume (setup_volume)
+	DevMem<Counters> ctr;
+	DevMem<ulonglong2> bh_tab;
+	DevMem<unsigned long long> uh_keys;
+	DevMem<uint32_t> uh_vals;
+	DevMem<unsigned long long> vol, vol_dirty;
+	DevMem<uint32_t> vol_list;
+	// change masks (a pool array): kept while detection is switched off, M.chg_mask only while recording
+	unsigned long long* chg_mask = nullptr;
+	bool chg_recording = false;
 	// scan staging: two point buffers, so that the H2D copy of scan k+1 overlaps scan k
-	void* d_points[2] = {nullptr, nullptr};
-	size_t d_points_cap[2] = {0, 0};
+	DevMem<void> d_points[2];
 	uint32_t stage = 0;
-	double* d_ray_end = nullptr;
-	uint32_t* d_hit_tab = nullptr;
+	DevMem<double> d_ray_end;
+	DevMem<uint32_t> d_hit_tab;
 	size_t ray_cap = 0;
-	unsigned long long* d_tab_keys = nullptr;
-	uint32_t* d_tab_min = nullptr;
+	DevMem<unsigned long long> d_tab_keys;
+	DevMem<uint32_t> d_tab_min;
 	uint32_t tab_size = 0;
 	uint32_t* d_list[2] = {nullptr, nullptr};
 	// generic marking path: ray-walk records
-	QEntry* d_seg = nullptr;
+	DevMem<QEntry> d_seg;
 	unsigned long long seg_cap = 0;
-	uint32_t *d_seg_base = nullptr, *d_seg_count = nullptr;
-	uint32_t* d_order = nullptr;
-	unsigned long long* d_nodes = nullptr;  // insert depth 5/6: free-space nodes of the scan
+	DevMem<uint32_t> d_seg_base, d_seg_count, d_order;
+	DevMem<unsigned long long> d_nodes;  // insert depth 5/6: free-space nodes of the scan
 	// fused walk: segments, validity masks, per-ray constants
-	Item* d_items = nullptr;
-	uint32_t* d_vmask = nullptr;
-	RayConst* d_rc = nullptr;
+	DevMem<Item> d_items;
+	DevMem<uint32_t> d_vmask;
+	DevMem<RayConst> d_rc;
 	size_t item_cap = 0;
 	// write batches: inputs + record regions, records (two key / index buffers for the sort), the
 	// brick segments of the sorted keys, sort scratch
-	unsigned char* d_w_in = nullptr;
-	size_t w_in_cap = 0;
-	unsigned long long* d_w_keys[2] = {nullptr, nullptr};
-	uint32_t* d_w_idx[2] = {nullptr, nullptr};
-	WriteRec* d_w_recs = nullptr;
+	DevMem<unsigned char> d_w_in;
+	DevMem<unsigned long long> d_w_keys[2];
+	DevMem<uint32_t> d_w_idx[2];
+	DevMem<WriteRec> d_w_recs;
 	size_t w_rec_cap = 0;
-	uint32_t* d_w_seg = nullptr;
-	size_t w_seg_cap = 0;
-	void* d_w_tmp = nullptr;
-	size_t w_tmp_cap = 0;
+	DevMem<uint32_t> d_w_seg;
+	DevMem<void> d_w_tmp;
 	bool write_pass = false;  // the last pass was a write batch (its stats carry ms_update)
 	// early stopping (ufo_early.cuh), allocated on the first such scan: node table, per-ray visit
 	// counts / offsets / prefix lengths, visit ids, scan scratch
 	int early_exact = 0;  // ufo_b200_set_early_stopping: early_stopping != 0 is computed, not rejected
 	bool early_pass = false;  // the last pass was such a scan
-	unsigned long long* d_e_keys = nullptr;
-	uint32_t* d_e_first = nullptr;
+	DevMem<unsigned long long> d_e_keys;
+	DevMem<uint32_t> d_e_first;
 	size_t e_tab_cap = 0;
-	unsigned long long *d_e_cnt = nullptr, *d_e_off = nullptr;
-	uint32_t *d_e_plen = nullptr, *d_e_pnext = nullptr;
+	DevMem<unsigned long long> d_e_cnt, d_e_off;
+	DevMem<uint32_t> d_e_plen, d_e_pnext;
 	size_t e_ray_cap = 0;
-	uint32_t* d_e_ids = nullptr;
+	DevMem<uint32_t> d_e_ids;
 	unsigned long long e_id_cap = 0;
-	void* d_e_tmp = nullptr;
-	size_t e_tmp_cap = 0;
+	DevMem<void> d_e_tmp;
 	int early_blocks_per_sm = 1;
 	ufo_b200_early_stats early_stats{};
 	// bookkeeping
@@ -191,16 +212,16 @@ struct ufo_b200_map {
 	bool stats_pending = false;
 	PendingScan pending;
 	bool poisoned = false;
-	unsigned long long* chg_paused = nullptr;  // change masks kept while detection is switched off
 	// routed multi-GPU mode
-	unsigned char* route_inbox = nullptr;  // this rank's inbox: [2 parities][world sources] regions
+	DevMem<unsigned char> route_inbox;  // this rank's inbox: [2 parities][world sources] regions
+	DevMem<RouteTable> route_table;     // M.route
 	size_t route_region = 0, route_miss_off = 0, route_hit_off = 0;
 	void* route_peer[kMaxRanks] = {};
 	RouteTable* h_route = nullptr;  // pinned mirror, pushed before every mark pass
 	uint32_t* h_route_flag = nullptr;  // pinned: RouteTable::overflow, then ::sent[3] of the last mark pass
 	// colour maps: apply table (minimum global cloud index per hit voxel of one apply call)
-	unsigned long long* d_route_tab_keys = nullptr;
-	uint32_t* d_route_tab_min = nullptr;
+	DevMem<unsigned long long> d_route_tab_keys;
+	DevMem<uint32_t> d_route_tab_min;
 	uint32_t route_tab_size = 0;
 	uint32_t route_parity = 0, route_cap_m = 0, route_cap_h = 0;
 	int route_stage = 0;  // 0 idle, 1 marked (waiting for the apply calls), 2 applied
@@ -267,78 +288,226 @@ void initial_caps(const ufo_b200_params& p, uint32_t& bricks, uint32_t& upper)
 	upper = std::max(bricks / 2, 4096u);
 }
 
-// the upper-node pool, its hash and the dirty lists of the propagation pass, empty
-void alloc_upper(Map* m, uint32_t up_cap)
+// The one place a map's device memory is allocated and freed (DevMem and the pool arrays): frees
+// `old` (`old_bytes` long) and returns n new bytes, uninitialised (nullptr for none).
+void* map_realloc(Map* m, void* old, size_t old_bytes, size_t n)
+{
+	if (old) {
+		cudaFree(old);  // a failure here is a broken context, which the next checked call reports
+		m->device_bytes -= old_bytes;
+	}
+	void* q = nullptr;
+	if (n) {
+		CK(cudaMalloc(&q, n));
+		m->device_bytes += n;
+	}
+	return q;
+}
+}  // namespace
+
+template <class T>
+void DevMem<T>::ensure(Map* m, size_t n, int fill)
+{
+	if (p && n <= bytes) return;
+	release(m);
+	p = static_cast<T*>(map_realloc(m, nullptr, 0, n));
+	bytes = n;
+	if (fill >= 0 && n) CK(cudaMemsetAsync(p, fill, n, m->stream));
+}
+
+template <class T>
+void DevMem<T>::release(Map* m)
+{
+	void* old = p;
+	p = nullptr;
+	map_realloc(m, old, bytes, 0);
+	bytes = 0;
+}
+
+namespace
+{
+// at least `bytes` (uninitialised), with an eighth to spare so that a slowly growing need does not
+// reallocate on every call
+template <class T>
+void ensure_spare(Map* m, DevMem<T>& b, size_t bytes, size_t min_bytes)
+{
+	if (!b.p || bytes > b.bytes) b.ensure(m, std::max(bytes + bytes / 8, min_bytes), -1);
+}
+
+// moves `n` whole bricks of `brick_bytes` each (k_page_move) with the widest word that divides a brick
+template <bool SCATTER>
+void launch_page_move(Map* m, void* dst, const void* src, const uint32_t* slot, size_t n, size_t brick_bytes)
+{
+	if (!n) return;
+	auto run = [&](auto* d, size_t word) {
+		using V = std::remove_pointer_t<decltype(d)>;
+		const size_t per = brick_bytes / word;
+		uint32_t lg = 0;
+		while (((size_t)1 << lg) < per) ++lg;
+		const size_t units = n * per;
+		const uint32_t grid = (uint32_t)std::min<size_t>((units + 255) / 256, (size_t)m->sm_count * 32);
+		k_page_move<V, SCATTER><<<grid, 256, 0, m->stream>>>(d, static_cast<const V*>(src), slot, units, lg);
+	};
+	if (brick_bytes % 16 == 0) run(static_cast<uint4*>(dst), 16);
+	else if (brick_bytes % 8 == 0) run(static_cast<uint2*>(dst), 8);
+	else run(static_cast<uint32_t*>(dst), 4);
+	++m->launches;
+}
+
+// ---- the two pools: every per-brick and per-upper-node array, described once ----
+enum class Pool : uint8_t { Brick, Upper };
+// when an array exists: always, on colour maps, from the first out-of-tree key a scan meets, or from
+// the first ufo_b200_enable_change_detection on
+enum class Have : uint8_t { Always, Color, Aliases, Changes };
+// what retain does with it: gather the surviving bricks, or start again from the fill
+enum class Retain : uint8_t { Compact, Renew };
+
+struct PoolArray {
+	void** (*owner)(Map*);  // where the owning pointer lives
+	size_t elem;            // bytes per element
+	uint32_t per;           // elements per brick / per upper node
+	int fill;               // byte of a slot nothing has written yet
+	Pool pool;
+	Have have;
+	Retain retain;
+};
+
+#define UFO_POOL_ARRAY(ptr) [](Map* m) { return reinterpret_cast<void**>(&m->ptr); }, sizeof(*std::declval<Map&>().ptr)
+// In the order a new map allocates them (the driver's sub-allocator packs the small arrays by it,
+// which shows in the time of the scans right after a growth).
+const PoolArray kPool[] = {
+	{UFO_POOL_ARRAY(M.brick_key), 1, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.brick_stamp), 1, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.hit_stamp), 1, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.touched), 1, 0, Pool::Brick, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.touched_alt), 1, 0, Pool::Brick, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.touched_mi), 1, 0, Pool::Brick, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.touched_alt_mi), 1, 0, Pool::Brick, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.brick_sum3), 8, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.brick_sum4), 1, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.leaf), 64 * 64, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.miss_mask), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.hit_mask), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.meta), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.pair_max), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.brick_parent), 1, 0xff, Pool::Brick, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(chg_mask), 64, 0, Pool::Brick, Have::Changes, Retain::Compact},
+	{UFO_POOL_ARRAY(M.alias_miss), 64, 0, Pool::Brick, Have::Aliases, Retain::Compact},
+	{UFO_POOL_ARRAY(M.alias_hit), 64, 0, Pool::Brick, Have::Aliases, Retain::Compact},
+	{UFO_POOL_ARRAY(M.brick_rgb3), 8, 0, Pool::Brick, Have::Color, Retain::Compact},
+	{UFO_POOL_ARRAY(M.brick_rgb4), 1, 0, Pool::Brick, Have::Color, Retain::Compact},
+	{UFO_POOL_ARRAY(M.leaf_rgb), 64 * 64, 0, Pool::Brick, Have::Color, Retain::Compact},
+	{UFO_POOL_ARRAY(M.sum1_rgb), 64 * 8, 0, Pool::Brick, Have::Color, Retain::Compact},
+	{UFO_POOL_ARRAY(M.rgb2), 64, 0, Pool::Brick, Have::Color, Retain::Compact},
+	{UFO_POOL_ARRAY(M.up_key), 1, 0, Pool::Upper, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.up_agg), 1, 0, Pool::Upper, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.up_stamp), 1, 0, Pool::Upper, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.up_child), 8, 0, Pool::Upper, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.up_valid), 1, 0, Pool::Upper, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.up_parent), 1, 0xff, Pool::Upper, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(d_list[0]), 1, 0, Pool::Upper, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(d_list[1]), 1, 0, Pool::Upper, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.up_rgb), 1, 0, Pool::Upper, Have::Color, Retain::Renew},
+	{UFO_POOL_ARRAY(M.up_child_rgb), 8, 0, Pool::Upper, Have::Color, Retain::Renew},
+};
+#undef UFO_POOL_ARRAY
+
+uint32_t pool_cap(const Map* m, Pool pool) { return pool == Pool::Brick ? m->M.brick_cap : m->M.up_cap; }
+
+// Replaces pool array `a` of old_cap bricks / nodes by one of new_cap (0: frees it).  The first
+// `kept` entries come from the old array, entries 0..kept or, with `src`, entries src[0..kept); the
+// others get the array's fill.  With nothing to keep the old array goes first.
+void reshape(Map* m, const PoolArray& a, uint32_t old_cap, uint32_t new_cap, uint32_t kept, const uint32_t* src)
+{
+	cudaStream_t s = m->stream;
+	void*& p = *a.owner(m);
+	const size_t per = a.per * a.elem;
+	void* old = p;
+	if (!kept) {
+		p = nullptr;
+		map_realloc(m, old, (size_t)old_cap * per, 0);
+		old = nullptr;
+	}
+	void* q = map_realloc(m, nullptr, 0, (size_t)new_cap * per);
+	if (kept && src) launch_page_move<false>(m, q, old, src, kept, per);
+	else if (kept) CK(cudaMemcpyAsync(q, old, (size_t)kept * per, cudaMemcpyDeviceToDevice, s));
+	if (q) CK(cudaMemsetAsync(static_cast<uint8_t*>(q) + (size_t)kept * per, a.fill, (size_t)(new_cap - kept) * per, s));
+	if (old) {
+		CK(cudaStreamSynchronize(s));
+		p = nullptr;
+		map_realloc(m, old, (size_t)old_cap * per, 0);
+	}
+	p = q;
+	m->M.chg_mask = m->chg_recording ? m->chg_mask : nullptr;  // K3 records through the view of its owner
+}
+
+// the missing arrays of `pool` that exist from `have` on, at the pool's capacity
+void alloc_arrays(Map* m, Pool pool, Have have)
+{
+	for (const PoolArray& a : kPool)
+		if (a.pool == pool && a.have == have && !*a.owner(m)) reshape(m, a, 0, pool_cap(m, pool), 0, nullptr);
+}
+
+// The existing arrays of `pool`: the per-block ones first, and of those the leaves, so that when a
+// growth or a retain cannot hold one more leaf array it fails before anything has changed.  Every
+// later array is smaller than what has been freed.
+template <class F>
+void each_array(Map* m, Pool pool, F&& f)
+{
+	for (const bool blocks : {true, false})
+		for (const PoolArray& a : kPool)
+			if (a.pool == pool && (a.per >= 64) == blocks && *a.owner(m)) f(a);
+}
+
+// The brick hash, sized for the pool's capacity and rebuilt from its first `live` bricks (which
+// drops the kFailed entries a full pool leaves behind).
+void brick_hash(Map* m, uint32_t live)
 {
 	DeviceMap& M = m->M;
-	cudaStream_t s = m->stream;
-	size_t& tot = m->device_bytes;
-	M.up_cap = up_cap;
-	M.uh_mask = std::max(kMinHash, next_pow2(2ull * up_cap)) - 1;
-	dev_alloc(M.uh_keys, (size_t)M.uh_mask + 1, 0xff, s, tot);
-	dev_alloc(M.uh_vals, (size_t)M.uh_mask + 1, 0xff, s, tot);
-	dev_alloc(M.up_key, up_cap, 0, s, tot);
-	dev_alloc(M.up_agg, up_cap, 0, s, tot);
-	dev_alloc(M.up_stamp, up_cap, 0, s, tot);
-	dev_alloc(M.up_child, (size_t)up_cap * 8, 0, s, tot);
-	dev_alloc(M.up_valid, up_cap, 0, s, tot);
-	dev_alloc(M.up_parent, up_cap, 0xff, s, tot);
-	dev_alloc(m->d_list[0], up_cap, 0, s, tot);
-	dev_alloc(m->d_list[1], up_cap, 0, s, tot);
-	if (M.color) {
-		dev_alloc(M.up_rgb, up_cap, 0, s, tot);
-		dev_alloc(M.up_child_rgb, (size_t)up_cap * 8, 0, s, tot);
-	}
+	const uint32_t n = std::max(kMinHash, next_pow2(2ull * M.brick_cap));
+	m->bh_tab.release(m);
+	m->bh_tab.ensure(m, (size_t)n * sizeof(ulonglong2), 0xff);
+	M.bh_tab = m->bh_tab.p;
+	M.bh_mask = n - 1;
+	if (live) k_rebuild_brick_hash<<<(live + 255) / 256, 256, 0, m->stream>>>(M, live);
+}
+
+// the upper-node hash, as brick_hash
+void upper_hash(Map* m, uint32_t live)
+{
+	DeviceMap& M = m->M;
+	const uint32_t n = std::max(kMinHash, next_pow2(2ull * M.up_cap));
+	m->uh_keys.release(m);
+	m->uh_vals.release(m);
+	m->uh_keys.ensure(m, (size_t)n * sizeof(unsigned long long), 0xff);
+	m->uh_vals.ensure(m, (size_t)n * sizeof(uint32_t), 0xff);
+	M.uh_keys = m->uh_keys.p;
+	M.uh_vals = m->uh_vals.p;
+	M.uh_mask = n - 1;
+	if (live) k_rebuild_upper_hash<<<(live + 255) / 256, 256, 0, m->stream>>>(M, live);
 }
 
 void alloc_pools(Map* m, uint32_t brick_cap, uint32_t up_cap)
 {
-	DeviceMap& M = m->M;
-	cudaStream_t s = m->stream;
-	size_t& tot = m->device_bytes;
-	const size_t nb = (size_t)brick_cap * 64;  // block slots: 64 consecutive per brick
-	M.brick_cap = brick_cap;
-	M.bh_mask = std::max(kMinHash, next_pow2(2ull * brick_cap)) - 1;
-	dev_alloc(M.bh_tab, (size_t)M.bh_mask + 1, 0xff, s, tot);
-	dev_alloc(M.brick_key, brick_cap, 0, s, tot);
-	dev_alloc(M.brick_stamp, brick_cap, 0, s, tot);
-	dev_alloc(M.hit_stamp, brick_cap, 0, s, tot);
-	dev_alloc(M.touched, brick_cap, 0, s, tot);
-	dev_alloc(M.touched_alt, brick_cap, 0, s, tot);
-	dev_alloc(M.touched_mi, brick_cap, 0, s, tot);
-	dev_alloc(M.touched_alt_mi, brick_cap, 0, s, tot);
-	dev_alloc(M.brick_sum3, (size_t)brick_cap * 8, 0, s, tot);
-	dev_alloc(M.brick_sum4, brick_cap, 0, s, tot);
-	dev_alloc(M.leaf, nb * 64, 0, s, tot);
-	dev_alloc(M.miss_mask, nb, 0, s, tot);
-	dev_alloc(M.hit_mask, nb, 0, s, tot);
-	dev_alloc(M.meta, nb, 0, s, tot);
-	dev_alloc(M.pair_max, nb, 0, s, tot);
-	dev_alloc(M.brick_parent, brick_cap, 0xff, s, tot);
-	alloc_upper(m, up_cap);
-	if (M.color) {
-		dev_alloc(M.brick_rgb3, (size_t)brick_cap * 8, 0, s, tot);
-		dev_alloc(M.brick_rgb4, brick_cap, 0, s, tot);
-		dev_alloc(M.leaf_rgb, nb * 64, 0, s, tot);
-		dev_alloc(M.sum1_rgb, nb * 8, 0, s, tot);
-		dev_alloc(M.rgb2, nb, 0, s, tot);
+	m->M.brick_cap = brick_cap;
+	m->M.up_cap = up_cap;
+	brick_hash(m, 0);
+	alloc_arrays(m, Pool::Brick, Have::Always);
+	upper_hash(m, 0);
+	alloc_arrays(m, Pool::Upper, Have::Always);
+	if (m->M.color) {
+		alloc_arrays(m, Pool::Upper, Have::Color);
+		alloc_arrays(m, Pool::Brick, Have::Color);
 	}
-	dev_alloc(M.ctr, 1, 0, s, tot);
+	m->ctr.ensure(m, sizeof(Counters), 0);
+	m->M.ctr = m->ctr.p;
 }
 
+// the pool arrays; the map's DevMems go with the map
 void free_pools(Map* m)
 {
-	DeviceMap& M = m->M;
-	void* ptrs[] = {M.bh_tab, M.brick_key, M.brick_stamp, M.hit_stamp, M.touched, M.touched_alt, M.touched_mi, M.touched_alt_mi, M.chg_mask, M.vol, M.vol_dirty, M.vol_list, M.route, m->route_inbox, M.brick_sum3, M.brick_sum4, M.brick_rgb3, M.brick_rgb4,
-	                M.leaf, M.leaf_rgb, M.miss_mask, M.hit_mask, M.meta, M.pair_max, M.rgb2, M.sum1_rgb,
-	                M.alias_miss, M.alias_hit, M.uh_keys, M.uh_vals, M.up_key, M.up_agg, M.up_rgb, M.up_stamp, M.up_child, M.up_child_rgb, M.up_valid, M.up_parent, M.brick_parent, M.ctr, m->d_list[0],
-	                m->d_list[1], m->d_points[0], m->d_points[1], m->d_ray_end, m->d_hit_tab, m->d_tab_keys, m->d_tab_min,
-	                m->d_seg, m->d_seg_base, m->d_seg_count, m->d_order, m->d_nodes, m->d_items, m->d_vmask, m->d_rc,
-	                m->d_w_in, m->d_w_keys[0], m->d_w_keys[1], m->d_w_idx[0], m->d_w_idx[1], m->d_w_recs, m->d_w_seg,
-	                m->d_w_tmp, m->d_route_tab_keys, m->d_route_tab_min, m->d_e_keys, m->d_e_first, m->d_e_cnt, m->d_e_off,
-	                m->d_e_plen, m->d_e_pnext, m->d_e_ids, m->d_e_tmp};
-	for (void* p : ptrs)
-		if (p) cudaFree(p);
+	for (const PoolArray& a : kPool)
+		if (*a.owner(m)) reshape(m, a, pool_cap(m, a.pool), 0, 0, nullptr);
 }
 
 void push_counters(Map* m)
@@ -361,75 +530,27 @@ void push_counters(Map* m)
 void grow_pools(Map* m, uint32_t overflow, uint32_t want_bricks, uint32_t want_upper)
 {
 	DeviceMap& M = m->M;
-	cudaStream_t s = m->stream;
-	size_t& tot = m->device_bytes;
-	CK(cudaStreamSynchronize(s));
+	CK(cudaStreamSynchronize(m->stream));
+	auto grow = [&](Pool pool, uint32_t oc, uint32_t nc) {
+		each_array(m, pool, [&](const PoolArray& a) { reshape(m, a, oc, nc, oc, nullptr); });
+	};
 	if (overflow & 2u) {
 		uint32_t oc = M.brick_cap;
 		// marking stops creating bricks once the pool is exhausted, so `want` is barely above the old
 		// capacity: small pools grow by 4x, large ones by 2x
 		uint32_t nc = (uint32_t)std::max<uint64_t>((oc < (1u << 18) ? 4ull : 2ull) * oc, (uint64_t)want_bricks + want_bricks / 4);
 		if ((uint64_t)nc * 64 > 0xfffffff0ull) throw std::bad_alloc();
-		const size_t ob = (size_t)oc * 64, nb = (size_t)nc * 64;
-		dev_grow(M.leaf, ob * 64, nb * 64, 0, s, tot);
-		dev_grow(M.miss_mask, ob, nb, 0, s, tot);
-		dev_grow(M.hit_mask, ob, nb, 0, s, tot);
-		dev_grow(M.chg_mask, ob, nb, 0, s, tot);
-		dev_grow(M.meta, ob, nb, 0, s, tot);
-		dev_grow(M.pair_max, ob, nb, 0, s, tot);
-		dev_grow(M.leaf_rgb, ob * 64, nb * 64, 0, s, tot);
-		dev_grow(M.sum1_rgb, ob * 8, nb * 8, 0, s, tot);
-		dev_grow(M.rgb2, ob, nb, 0, s, tot);
-		dev_grow(M.alias_miss, ob, nb, 0, s, tot);
-		dev_grow(M.alias_hit, ob, nb, 0, s, tot);
-		dev_grow(M.brick_key, oc, nc, 0, s, tot);
-		dev_grow(M.brick_stamp, oc, nc, 0, s, tot);
-		dev_grow(M.hit_stamp, oc, nc, 0, s, tot);
-		dev_grow(M.brick_parent, oc, nc, 0xff, s, tot);
-		dev_grow(M.touched, oc, nc, 0, s, tot);
-		dev_grow(M.touched_alt, oc, nc, 0, s, tot);
-		dev_grow(M.touched_mi, oc, nc, 0, s, tot);
-		dev_grow(M.touched_alt_mi, oc, nc, 0, s, tot);
-		dev_grow(M.brick_sum3, (size_t)oc * 8, (size_t)nc * 8, 0, s, tot);
-		dev_grow(M.brick_sum4, oc, nc, 0, s, tot);
-		dev_grow(M.brick_rgb3, (size_t)oc * 8, (size_t)nc * 8, 0, s, tot);
-		dev_grow(M.brick_rgb4, oc, nc, 0, s, tot);
+		grow(Pool::Brick, oc, nc);
 		M.brick_cap = nc;
-		// rebuild the hash from the surviving bricks (drops kFailed entries)
-		size_t old_tab = (size_t)M.bh_mask + 1;
-		uint32_t new_tab = std::max(kMinHash, next_pow2(2ull * nc));
-		CK(cudaFree(M.bh_tab));
-		tot -= old_tab * sizeof(ulonglong2);
-		M.bh_mask = new_tab - 1;
-		dev_alloc(M.bh_tab, new_tab, 0xff, s, tot);
-		uint32_t live = std::min(m->h_ctr->n_bricks, oc);
-		if (live) k_rebuild_brick_hash<<<(live + 255) / 256, 256, 0, s>>>(M, live);
+		brick_hash(m, std::min(m->h_ctr->n_bricks, oc));
 		if (M.up_cap < nc / 2) overflow |= 4u;  // keep the upper-node pool in proportion
 	}
 	if (overflow & 4u) {
 		uint32_t oc = M.up_cap;
 		uint32_t nc = (uint32_t)std::max<uint64_t>(std::max<uint64_t>(2ull * oc, M.brick_cap / 2), (uint64_t)want_upper + want_upper / 4);
-		dev_grow(M.up_key, oc, nc, 0, s, tot);
-		dev_grow(M.up_agg, oc, nc, 0, s, tot);
-		dev_grow(M.up_stamp, oc, nc, 0, s, tot);
-		dev_grow(M.up_rgb, oc, nc, 0, s, tot);
-		dev_grow(M.up_child, (size_t)oc * 8, (size_t)nc * 8, 0, s, tot);
-		dev_grow(M.up_child_rgb, (size_t)oc * 8, (size_t)nc * 8, 0, s, tot);
-		dev_grow(M.up_valid, oc, nc, 0, s, tot);
-		dev_grow(M.up_parent, oc, nc, 0xff, s, tot);
-		dev_grow(m->d_list[0], oc, nc, 0, s, tot);
-		dev_grow(m->d_list[1], oc, nc, 0, s, tot);
+		grow(Pool::Upper, oc, nc);
 		M.up_cap = nc;
-		size_t old_tab = (size_t)M.uh_mask + 1;
-		uint32_t new_tab = std::max(kMinHash, next_pow2(2ull * nc));
-		CK(cudaFree(M.uh_keys));
-		CK(cudaFree(M.uh_vals));
-		tot -= old_tab * (sizeof(unsigned long long) + sizeof(uint32_t));
-		M.uh_mask = new_tab - 1;
-		dev_alloc(M.uh_keys, new_tab, 0xff, s, tot);
-		dev_alloc(M.uh_vals, new_tab, 0xff, s, tot);
-		uint32_t nu = std::min(m->h_ctr->n_upper, oc);
-		if (nu) k_rebuild_upper_hash<<<(nu + 255) / 256, 256, 0, s>>>(M, nu);
+		upper_hash(m, std::min(m->h_ctr->n_upper, oc));
 	}
 	CK(cudaGetLastError());
 }
@@ -448,54 +569,28 @@ size_t layout_stride(int layout)
 // called with the stream idle
 void ensure_scan_buffers(Map* m, size_t n, bool need_table, bool records, bool fused)
 {
-	size_t& tot = m->device_bytes;
+	DevMem<uint32_t>* batch_bufs[] = {&m->d_seg_base, &m->d_seg_count, &m->d_order};
 	if (n > m->ray_cap) {
-		if (m->d_ray_end) {
-			cudaFree(m->d_ray_end);
-			cudaFree(m->d_hit_tab);
-			tot -= m->ray_cap * (3 * sizeof(double) + sizeof(uint32_t));
-		}
-		if (m->d_seg_base) {
-			cudaFree(m->d_seg_base);
-			cudaFree(m->d_seg_count);
-			cudaFree(m->d_order);
-			m->d_seg_base = m->d_seg_count = m->d_order = nullptr;
-			tot -= (m->ray_cap / 32 + 1) * 12;
-		}
-		size_t cap = std::max<size_t>(n, 1024);
-		dev_alloc(m->d_ray_end, cap * 3, 0, m->stream, tot);
-		dev_alloc(m->d_hit_tab, cap, 0xff, m->stream, tot);
+		const size_t cap = std::max<size_t>(n, 1024);
+		m->d_ray_end.ensure(m, cap * 3 * sizeof(double), 0);
+		m->d_hit_tab.ensure(m, cap * sizeof(uint32_t), 0xff);
+		for (auto* b : batch_bufs) b->release(m);
 		m->ray_cap = cap;
 	}
-	if (records && !m->d_seg_base) {
-		dev_alloc(m->d_seg_base, m->ray_cap / 32 + 1, 0, m->stream, tot);
-		dev_alloc(m->d_seg_count, m->ray_cap / 32 + 1, 0, m->stream, tot);
-		dev_alloc(m->d_order, m->ray_cap / 32 + 1, 0, m->stream, tot);
-	}
+	if (records)
+		for (auto* b : batch_bufs) b->ensure(m, (m->ray_cap / 32 + 1) * sizeof(uint32_t), 0);
 	if (fused && m->item_cap < m->ray_cap) {
-		if (m->d_items) {
-			cudaFree(m->d_items);
-			cudaFree(m->d_vmask);
-			cudaFree(m->d_rc);
-			tot -= m->item_cap * (kShells * sizeof(Item) + sizeof(RayConst)) + (m->item_cap / 32 + 1) * kShells * 4;
-		}
-		m->item_cap = m->ray_cap;
-		m->d_items = nullptr;
-		CK(cudaMalloc(reinterpret_cast<void**>(&m->d_items), m->item_cap * kShells * sizeof(Item)));  // written before read
-		tot += m->item_cap * kShells * sizeof(Item);
-		dev_alloc(m->d_vmask, (m->item_cap / 32 + 1) * kShells, 0, m->stream, tot);
-		dev_alloc(m->d_rc, m->item_cap, 0, m->stream, tot);
+		const size_t cap = m->ray_cap;
+		m->d_items.ensure(m, cap * kShells * sizeof(Item), -1);  // written before read
+		m->d_vmask.ensure(m, (cap / 32 + 1) * kShells * sizeof(uint32_t), 0);
+		m->d_rc.ensure(m, cap * sizeof(RayConst), 0);
+		m->item_cap = cap;
 	}
 	if (need_table) {
 		uint32_t want = std::max(1u << 12, next_pow2(4ull * n));
 		if (want > m->tab_size) {
-			if (m->d_tab_keys) {
-				cudaFree(m->d_tab_keys);
-				cudaFree(m->d_tab_min);
-				tot -= (size_t)m->tab_size * 12;
-			}
-			dev_alloc(m->d_tab_keys, want, 0xff, m->stream, tot);
-			dev_alloc(m->d_tab_min, want, 0xff, m->stream, tot);
+			m->d_tab_keys.ensure(m, (size_t)want * sizeof(unsigned long long), 0xff);
+			m->d_tab_min.ensure(m, (size_t)want * sizeof(uint32_t), 0xff);
 			m->tab_size = want;
 		}
 	}
@@ -521,8 +616,8 @@ void finish_stats(Map* m)
 		es.visits = c.e_visits;
 		es.nodes = c.e_nodes;
 		es.free_nodes = c.e_free;
-		es.table_bytes = m->e_tab_cap * (sizeof(unsigned long long) + sizeof(uint32_t));
-		es.id_bytes = m->e_id_cap * sizeof(uint32_t) + m->e_ray_cap * (2 * sizeof(unsigned long long) + 2 * sizeof(uint32_t));
+		es.table_bytes = m->d_e_keys.bytes + m->d_e_first.bytes;
+		es.id_bytes = m->d_e_ids.bytes + m->d_e_cnt.bytes + m->d_e_off.bytes + m->d_e_plen.bytes + m->d_e_pnext.bytes;
 		if (m->ev_valid && m->profiling) {
 			cudaEventElapsedTime(&es.ms_walk, m->ev[2], m->ev[1]);
 			cudaEventElapsedTime(&es.ms_rounds, m->ev[1], m->ev[4]);
@@ -575,14 +670,8 @@ void ensure_seg(Map* m, unsigned long long want)
 {
 	if (want <= m->seg_cap) return;
 	CK(cudaStreamSynchronize(m->stream));
-	if (m->d_seg) {
-		cudaFree(m->d_seg);
-		m->device_bytes -= m->seg_cap * sizeof(QEntry);
-	}
-	m->d_seg = nullptr;
-	CK(cudaMalloc(reinterpret_cast<void**>(&m->d_seg), want * sizeof(QEntry)));
+	m->d_seg.ensure(m, want * sizeof(QEntry), -1);
 	m->seg_cap = want;
-	m->device_bytes += want * sizeof(QEntry);
 }
 
 // K3 over the scan's touched list: persistent warps, the list length is read on the device.
@@ -717,24 +806,26 @@ uint32_t volume_bricks(const Map* m, const PendingScan& p)
 	return 2 * half + 1;
 }
 
+// empties the dense scan volume: its masks and the dirty bitmap
+void wipe_volume(Map* m)
+{
+	if (!m->vol.p) return;
+	CK(cudaMemsetAsync(m->vol.p, 0, m->vol.bytes, m->stream));
+	CK(cudaMemsetAsync(m->vol_dirty.p, 0, m->vol_dirty.bytes, m->stream));
+}
+
 // called with the stream idle; binds the volume to this scan's sensor position
 void setup_volume(Map* m, PendingScan& p, uint32_t db)
 {
 	DeviceMap& M = m->M;
 	if (db > m->vol_db_cap) {
-		if (M.vol) {
-			cudaFree(M.vol);
-			cudaFree(M.vol_dirty);
-			cudaFree(M.vol_list);
-			m->device_bytes -= (size_t)m->vol_db_cap * m->vol_db_cap * m->vol_db_cap * (512 + 1) ;
-		}
-		M.vol = nullptr;
-		M.vol_dirty = nullptr;
-		M.vol_list = nullptr;
 		const size_t nb = (size_t)db * db * db;
-		dev_alloc(M.vol, nb * 64, 0, m->stream, m->device_bytes);
-		dev_alloc(M.vol_dirty, nb / 64 + 1, 0, m->stream, m->device_bytes);
-		dev_alloc(M.vol_list, nb / 64 + 1, 0, m->stream, m->device_bytes);
+		m->vol.ensure(m, nb * 64 * sizeof(unsigned long long), 0);
+		m->vol_dirty.ensure(m, (nb / 64 + 1) * sizeof(unsigned long long), 0);
+		m->vol_list.ensure(m, (nb / 64 + 1) * sizeof(uint32_t), 0);
+		M.vol = m->vol.p;
+		M.vol_dirty = m->vol_dirty.p;
+		M.vol_list = m->vol_list.p;
 		m->vol_db_cap = db;
 	}
 	const Geometry& g = M.g;
@@ -787,67 +878,35 @@ __global__ void k_reset_upper_pass(Counters* c, uint32_t n_upper)
 	c->n_upper = n_upper;
 }
 
-// (re)allocates a device buffer of at least `bytes`; called with the stream idle
-template <class T>
-void ensure_dev(Map* m, T*& p, size_t& cap_bytes, size_t bytes)
-{
-	if (bytes <= cap_bytes && p) return;
-	if (p) {
-		CK(cudaFree(p));
-		m->device_bytes -= cap_bytes;
-	}
-	p = nullptr;
-	const size_t nb = std::max<size_t>(bytes + bytes / 8, 1 << 12);
-	CK(cudaMalloc(reinterpret_cast<void**>(&p), nb));
-	cap_bytes = nb;
-	m->device_bytes += nb;
-}
-
 // Early-stopping buffers (ufo_early.cuh) for n rays and `visits` walk visits; called with the stream
 // idle.  The node table stays below 80 % load (distinct nodes <= visits, plus one end node per ray of
 // a discrete scan) and every scan leaves it empty (E3 clears the slots it reads), so it is only
 // cleared when it is allocated.
 void ensure_early(Map* m, size_t n, unsigned long long visits)
 {
-	size_t& tot = m->device_bytes;
-	cudaStream_t s = m->stream;
 	if (n + 1 > m->e_ray_cap) {
-		for (void* q : {(void*)m->d_e_cnt, (void*)m->d_e_off, (void*)m->d_e_plen, (void*)m->d_e_pnext})
-			if (q) CK(cudaFree(q));
-		tot -= m->e_ray_cap * (2 * sizeof(unsigned long long) + 2 * sizeof(uint32_t));
 		const size_t cap = std::max<size_t>(n + 1, 1024);
-		dev_alloc(m->d_e_cnt, cap, 0, s, tot);
-		dev_alloc(m->d_e_off, cap, 0, s, tot);
-		dev_alloc(m->d_e_plen, cap, 0, s, tot);
-		dev_alloc(m->d_e_pnext, cap, 0, s, tot);
+		m->d_e_cnt.ensure(m, cap * sizeof(unsigned long long), 0);
+		m->d_e_off.ensure(m, cap * sizeof(unsigned long long), 0);
+		m->d_e_plen.ensure(m, cap * sizeof(uint32_t), 0);
+		m->d_e_pnext.ensure(m, cap * sizeof(uint32_t), 0);
 		m->e_ray_cap = cap;
 	}
 	if (visits > m->e_id_cap) {
-		if (m->d_e_ids) {
-			CK(cudaFree(m->d_e_ids));
-			tot -= m->e_id_cap * sizeof(uint32_t);
-		}
-		m->d_e_ids = nullptr;
+		m->d_e_ids.ensure(m, (visits + visits / 8) * sizeof(uint32_t), -1);  // written before read
 		m->e_id_cap = visits + visits / 8;
-		CK(cudaMalloc(reinterpret_cast<void**>(&m->d_e_ids), m->e_id_cap * sizeof(uint32_t)));  // written before read
-		tot += m->e_id_cap * sizeof(uint32_t);
 	}
 	const unsigned long long need = std::max<unsigned long long>(visits + visits / 4 + n + 1, 2ull * (n + 1));
 	if (need > m->e_tab_cap) {
 		if (need > (1ull << 31)) throw std::bad_alloc();
-		if (m->d_e_keys) {
-			CK(cudaFree(m->d_e_keys));
-			CK(cudaFree(m->d_e_first));
-			tot -= m->e_tab_cap * (sizeof(unsigned long long) + sizeof(uint32_t));
-		}
 		const size_t cap = next_pow2(need);
-		dev_alloc(m->d_e_keys, cap, 0xff, s, tot);
-		dev_alloc(m->d_e_first, cap, 0xff, s, tot);
+		m->d_e_keys.ensure(m, cap * sizeof(unsigned long long), 0xff);
+		m->d_e_first.ensure(m, cap * sizeof(uint32_t), 0xff);
 		m->e_tab_cap = cap;
 	}
 	size_t tmp = 0;
-	CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, m->d_e_cnt, m->d_e_off, (int)(n + 1), s));
-	ensure_dev(m, m->d_e_tmp, m->e_tmp_cap, tmp);
+	CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, m->d_e_cnt.p, m->d_e_off.p, (int)(n + 1), m->stream));
+	ensure_spare(m, m->d_e_tmp, tmp, 1 << 12);
 }
 
 // E1-E3 (ufo_early.cuh): the scan's free set under early stopping, marked like the record path
@@ -859,15 +918,15 @@ void launch_early(Map* m, const PendingScan& p)
 	EarlyArgs e{};
 	e.stop = p.early;
 	e.simple = p.simple ? 1 : 0;
-	e.keys = m->d_e_keys;
-	e.first = m->d_e_first;
+	e.keys = m->d_e_keys.p;
+	e.first = m->d_e_first.p;
 	e.tab_mask = (uint32_t)(m->e_tab_cap - 1);
-	e.cnt = m->d_e_cnt;
-	e.off = m->d_e_off;
-	e.ids = m->d_e_ids;
+	e.cnt = m->d_e_cnt.p;
+	e.off = m->d_e_off.p;
+	e.ids = m->d_e_ids.p;
 	e.id_cap = m->e_id_cap;
-	e.plen = m->d_e_plen;
-	e.pnext = m->d_e_pnext;
+	e.plen = m->d_e_plen.p;
+	e.pnext = m->d_e_pnext.p;
 	uint32_t n = a.n;
 	if (a.discrete) {
 		k_early_rank<<<(n + kEarlyThreads - 1) / kEarlyThreads, kEarlyThreads, 0, s>>>(m->M, a, e);
@@ -875,8 +934,8 @@ void launch_early(Map* m, const PendingScan& p)
 		m->launches += 2;
 	}
 	k_early_count<<<(n + kEarlyThreads) / kEarlyThreads, kEarlyThreads, 0, s>>>(m->M, a, e);  // n + 1 threads
-	size_t tmp = m->e_tmp_cap;
-	CK(cub::DeviceScan::ExclusiveSum(m->d_e_tmp, tmp, m->d_e_cnt, m->d_e_off, (int)(n + 1), s));
+	size_t tmp = m->d_e_tmp.bytes;
+	CK(cub::DeviceScan::ExclusiveSum(m->d_e_tmp.p, tmp, e.cnt, e.off, (int)(n + 1), s));
 	k_early_check<<<1, 1, 0, s>>>(m->M, e, n);
 	k_early_fill<<<(n + kEarlyThreads - 1) / kEarlyThreads, kEarlyThreads, 0, s>>>(m->M, a, e);
 	if (m->profiling) CK(cudaEventRecord(m->ev[1], s));
@@ -915,31 +974,27 @@ void enqueue_write(Map* m, PendingScan& p)
 	if (M.up_epoch == 0) M.up_epoch = 1;
 	M.dense = 0;
 	M.mask_base = M.miss_mask;
-	{
-		size_t cap = m->w_seg_cap;
-		ensure_dev(m, m->d_w_seg, cap, (size_t)M.brick_cap * 3 * sizeof(uint32_t));
-		m->w_seg_cap = cap;
-	}
-	a.seg_begin = m->d_w_seg;
-	a.seg_end = m->d_w_seg + M.brick_cap;
-	a.seg_list = m->d_w_seg + 2 * (size_t)M.brick_cap;
+	ensure_spare(m, m->d_w_seg, (size_t)M.brick_cap * 3 * sizeof(uint32_t), 1 << 12);
+	a.seg_begin = m->d_w_seg.p;
+	a.seg_end = m->d_w_seg.p + M.brick_cap;
+	a.seg_list = m->d_w_seg.p + 2 * (size_t)M.brick_cap;
 	// keys: brick slot << 32 | sequence number; only the bits a slot below brick_cap can use are sorted
 	int end_bit = 32;
 	while (end_bit < 64 && (1ull << (end_bit - 32)) <= M.brick_cap) ++end_bit;
 	size_t tmp_bytes = 0;
-	CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, m->d_w_keys[0], m->d_w_keys[1], m->d_w_idx[0],
-	                                   m->d_w_idx[1], (int)a.n_rec, 0, end_bit, s));
-	ensure_dev(m, m->d_w_tmp, m->w_tmp_cap, tmp_bytes);
+	CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, m->d_w_keys[0].p, m->d_w_keys[1].p, m->d_w_idx[0].p,
+	                                   m->d_w_idx[1].p, (int)a.n_rec, 0, end_bit, s));
+	ensure_spare(m, m->d_w_tmp, tmp_bytes, 1 << 12);
 	push_counters(m);
-	a.keys = m->d_w_keys[0];
-	a.idx = m->d_w_idx[0];
-	a.recs = m->d_w_recs;
+	a.keys = m->d_w_keys[0].p;
+	a.idx = m->d_w_idx[0].p;
+	a.recs = m->d_w_recs.p;
 	if (a.n) k_write_expand<<<(a.n + 127) / 128, 128, 0, s>>>(M, a);
-	tmp_bytes = m->w_tmp_cap;
-	CK(cub::DeviceRadixSort::SortPairs(m->d_w_tmp, tmp_bytes, m->d_w_keys[0], m->d_w_keys[1], m->d_w_idx[0],
-	                                   m->d_w_idx[1], (int)a.n_rec, 0, end_bit, s));
-	a.keys = m->d_w_keys[1];
-	a.idx = m->d_w_idx[1];
+	tmp_bytes = m->d_w_tmp.bytes;
+	CK(cub::DeviceRadixSort::SortPairs(m->d_w_tmp.p, tmp_bytes, m->d_w_keys[0].p, m->d_w_keys[1].p, m->d_w_idx[0].p,
+	                                   m->d_w_idx[1].p, (int)a.n_rec, 0, end_bit, s));
+	a.keys = m->d_w_keys[1].p;
+	a.idx = m->d_w_idx[1].p;
 	k_write_segments<<<m->sm_count * 8, 256, 0, s>>>(M, a);
 	CK(cudaEventRecord(m->ev[3], s));
 	if (a.rgb) k_write_apply<true><<<m->sm_count * 16, 64, 0, s>>>(M, a);
@@ -964,29 +1019,29 @@ void enqueue_write(Map* m, PendingScan& p)
 void bind_scan_buffers(Map* m, PendingScan& p, bool fused)
 {
 	ScanArgs& a = p.a;
-	a.ray_end = m->d_ray_end;
-	a.tab_keys = m->d_tab_keys;
-	a.tab_min = m->d_tab_min;
+	a.ray_end = m->d_ray_end.p;
+	a.tab_keys = m->d_tab_keys.p;
+	a.tab_min = m->d_tab_min.p;
 	a.tab_mask = m->tab_size ? m->tab_size - 1 : 0;
-	a.hit_tab = p.use_color ? m->d_hit_tab : nullptr;
+	a.hit_tab = p.use_color ? m->d_hit_tab.p : nullptr;
 	a.seg = nullptr;
 	a.seg_base = a.seg_count = a.order = nullptr;
 	a.items = nullptr;
 	if (fused) {
-		a.items = m->d_items;
+		a.items = m->d_items.p;
 		a.item_stride = m->item_cap;
-		a.vmask = m->d_vmask;
-		a.rc = m->d_rc;
+		a.vmask = m->d_vmask.p;
+		a.rc = m->d_rc.p;
 	} else if (!p.simple && !p.has_vol && !p.early) {
-		a.seg = m->d_seg;
+		a.seg = m->d_seg.p;
 		a.seg_cap = m->seg_cap;
-		a.seg_base = m->d_seg_base;
-		a.seg_count = m->d_seg_count;
-		a.order = m->d_order;
+		a.seg_base = m->d_seg_base.p;
+		a.seg_count = m->d_seg_count.p;
+		a.order = m->d_order.p;
 	}
 	if (a.depth >= 5) {
-		if (!m->d_nodes) dev_alloc(m->d_nodes, (size_t)1 << 20, 0, m->stream, m->device_bytes);
-		a.nodes = m->d_nodes;
+		m->d_nodes.ensure(m, sizeof(unsigned long long) << 20, 0);
+		a.nodes = m->d_nodes.p;
 		a.nodes_cap = 1u << 20;
 	}
 }
@@ -1014,8 +1069,8 @@ void enqueue_scan(Map* m, PendingScan& p)
 	m->ev7_valid = false;
 	push_counters(m);
 	if (p.need_table) {
-		CK(cudaMemsetAsync(m->d_tab_keys, 0xff, (size_t)m->tab_size * sizeof(unsigned long long), s));
-		CK(cudaMemsetAsync(m->d_tab_min, 0xff, (size_t)m->tab_size * sizeof(uint32_t), s));
+		CK(cudaMemsetAsync(m->d_tab_keys.p, 0xff, (size_t)m->tab_size * sizeof(unsigned long long), s));
+		CK(cudaMemsetAsync(m->d_tab_min.p, 0xff, (size_t)m->tab_size * sizeof(uint32_t), s));
 	}
 	if (p.has_vol) {
 		// setValueVolume: the marks come from the box instead of a scan
@@ -1133,22 +1188,15 @@ void finalize_scan(Map* m)
 					// as a safety net): wipe the volume and repeat through the brick hash
 					m->no_dense = 1;
 					p.dense = false;
-					const size_t nb = (size_t)m->vol_db_cap * m->vol_db_cap * m->vol_db_cap;
-					CK(cudaMemsetAsync(M.vol, 0, nb * 512, m->stream));
-					CK(cudaMemsetAsync(M.vol_dirty, 0, (nb / 64 + 1) * 8, m->stream));
+					wipe_volume(m);
 				}
 				if (ov & 32u) {
 					// first out-of-tree key ever seen by this map: allocate the alias mask arrays;
 					// from now on this map uses the generic record path
-					if (!M.alias_miss) {
-						dev_alloc(M.alias_miss, (size_t)M.brick_cap * 64, 0, m->stream, m->device_bytes);
-						dev_alloc(M.alias_hit, (size_t)M.brick_cap * 64, 0, m->stream, m->device_bytes);
-					}
+					alloc_arrays(m, Pool::Brick, Have::Aliases);
 					if (p.dense) {
 						// the marks the walk already left in the volume are not consumed by the record path
-						const size_t nb = (size_t)m->vol_db_cap * m->vol_db_cap * m->vol_db_cap;
-						CK(cudaMemsetAsync(M.vol, 0, nb * 512, m->stream));
-						CK(cudaMemsetAsync(M.vol_dirty, 0, (nb / 64 + 1) * 8, m->stream));
+						wipe_volume(m);
 						p.dense = false;
 					}
 				}
@@ -1237,6 +1285,15 @@ int sync_map(Map* m)
 	return UFO_B200_OK;
 }
 
+// copies a scan's points into staging buffer `stg` on the copy stream (see do_insert)
+void stage_points(Map* m, uint32_t stg, const void* points, size_t bytes)
+{
+	ensure_spare(m, m->d_points[stg], bytes, 1 << 16);
+	CK(cudaEventRecord(m->ev_copy0, m->copy_stream));
+	CK(cudaMemcpyAsync(m->d_points[stg].p, points, bytes, cudaMemcpyHostToDevice, m->copy_stream));
+	CK(cudaEventRecord(m->ev_copied, m->copy_stream));
+}
+
 int do_insert(Map* m, const double origin[3], const void* points, bool on_device, size_t n,
               const double* frame_pose,
               int layout, double max_range, uint32_t depth, int simple, uint32_t early_stopping,
@@ -1284,21 +1341,7 @@ int do_insert(Map* m, const double origin[3], const void* points, bool on_device
 	const size_t bytes = n * stride;
 	const bool copied = !on_device && bytes;
 	const uint32_t stg = m->stage ^ 1u;
-	if (copied) {
-		if (bytes > m->d_points_cap[stg]) {
-			if (m->d_points[stg]) {
-				cudaFree(m->d_points[stg]);
-				m->device_bytes -= m->d_points_cap[stg];
-			}
-			m->d_points[stg] = nullptr;
-			m->d_points_cap[stg] = std::max<size_t>(bytes + bytes / 8, 1 << 16);
-			CK(cudaMalloc(&m->d_points[stg], m->d_points_cap[stg]));
-			m->device_bytes += m->d_points_cap[stg];
-		}
-		CK(cudaEventRecord(m->ev_copy0, m->copy_stream));
-		CK(cudaMemcpyAsync(m->d_points[stg], points, bytes, cudaMemcpyHostToDevice, m->copy_stream));
-		CK(cudaEventRecord(m->ev_copied, m->copy_stream));
-	}
+	if (copied) stage_points(m, stg, points, bytes);
 	// one integration in flight at most (insertPointCloudWait, occupancy_map_base.h:315)
 	finalize_scan(m);
 
@@ -1354,7 +1397,7 @@ int do_insert(Map* m, const double origin[3], const void* points, bool on_device
 		ensure_seg(m, std::max<unsigned long long>(m->seg_cap, std::max<unsigned long long>(n, 1024) * 48ull));
 	}
 	// an on-device cloud is read in place: it has to stay valid until the scan is done
-	a.points = on_device ? points : m->d_points[stg];
+	a.points = on_device ? points : m->d_points[stg].p;
 	if (copied) m->stage = stg;
 
 	m->stats = ufo_b200_scan_stats{};
@@ -1397,7 +1440,7 @@ void route_fill_table(Map* m)
 		T.out[r].hdr = reinterpret_cast<uint32_t*>(bo);
 		T.out[r].miss = reinterpret_cast<unsigned long long*>(bo + m->route_miss_off);
 		T.out[r].hit = reinterpret_cast<unsigned long long*>(bo + m->route_hit_off);
-		unsigned char* bi = m->route_inbox + ((size_t)m->route_parity * W + r) * m->route_region;
+		unsigned char* bi = m->route_inbox.p + ((size_t)m->route_parity * W + r) * m->route_region;
 		T.in[r].hdr = reinterpret_cast<uint32_t*>(bi);
 		T.in[r].miss = reinterpret_cast<unsigned long long*>(bi + m->route_miss_off);
 		T.in[r].hit = reinterpret_cast<unsigned long long*>(bi + m->route_hit_off);
@@ -1447,21 +1490,7 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 	const size_t bytes = n * stride;
 	const bool copied = !on_device && bytes;
 	const uint32_t stg = m->stage ^ 1u;
-	if (copied) {
-		if (bytes > m->d_points_cap[stg]) {
-			if (m->d_points[stg]) {
-				cudaFree(m->d_points[stg]);
-				m->device_bytes -= m->d_points_cap[stg];
-			}
-			m->d_points[stg] = nullptr;
-			m->d_points_cap[stg] = std::max<size_t>(bytes + bytes / 8, 1 << 16);
-			CK(cudaMalloc(&m->d_points[stg], m->d_points_cap[stg]));
-			m->device_bytes += m->d_points_cap[stg];
-		}
-		CK(cudaEventRecord(m->ev_copy0, m->copy_stream));
-		CK(cudaMemcpyAsync(m->d_points[stg], points, bytes, cudaMemcpyHostToDevice, m->copy_stream));
-		CK(cudaEventRecord(m->ev_copied, m->copy_stream));
-	}
+	if (copied) stage_points(m, stg, points, bytes);
 	finalize_scan(m);
 	cudaStream_t s = m->stream;
 	PendingScan& p = m->pending;
@@ -1491,7 +1520,7 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 	}
 	M.dense = p.dense ? 1u : 0u;
 	M.mask_base = M.dense ? M.vol : M.miss_mask;
-	a.points = on_device ? points : m->d_points[stg];
+	a.points = on_device ? points : m->d_points[stg].p;
 	if (copied) m->stage = stg;
 	bind_scan_buffers(m, p, fused);
 	// a routed pass cannot be repeated after a record buffer overflow: K1 reserves without a
@@ -1513,8 +1542,8 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 	if (M.scan_id == 0) M.scan_id = 1;
 	push_counters(m);
 	if (p.need_table) {
-		CK(cudaMemsetAsync(m->d_tab_keys, 0xff, (size_t)m->tab_size * sizeof(unsigned long long), s));
-		CK(cudaMemsetAsync(m->d_tab_min, 0xff, (size_t)m->tab_size * sizeof(uint32_t), s));
+		CK(cudaMemsetAsync(m->d_tab_keys.p, 0xff, (size_t)m->tab_size * sizeof(unsigned long long), s));
+		CK(cudaMemsetAsync(m->d_tab_min.p, 0xff, (size_t)m->tab_size * sizeof(uint32_t), s));
 	}
 	if (n) {
 		const uint32_t grid = (uint32_t)((n + 255) / 256);
@@ -1532,7 +1561,7 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 				CK(cudaMemcpyAsync(&m->h_ctr->seg_total, &M.ctr->seg_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
 				CK(cudaStreamSynchronize(s));
 				ensure_seg(m, std::max<unsigned long long>(m->h_ctr->seg_total, 1024));
-				a.seg = m->d_seg;
+				a.seg = m->d_seg.p;
 				a.seg_cap = m->seg_cap;
 			}
 			launch_rays_records(m, a, p.simple);
@@ -1584,10 +1613,10 @@ int do_route_apply(Map* m, uint32_t first, uint32_t count, int last)
 	if (M.color) {
 		// apply table for the hit records of these sources: at most count * cap_h keys, half full
 		const uint32_t size = std::min(m->route_tab_size, std::max(1u << 12, next_pow2(2ull * count * m->route_cap_h)));
-		CK(cudaMemsetAsync(m->d_route_tab_keys, 0xff, (size_t)size * sizeof(unsigned long long), s));
-		CK(cudaMemsetAsync(m->d_route_tab_min, 0xff, (size_t)size * sizeof(uint32_t), s));
-		t.tab_keys = m->d_route_tab_keys;
-		t.tab_min = m->d_route_tab_min;
+		CK(cudaMemsetAsync(m->d_route_tab_keys.p, 0xff, (size_t)size * sizeof(unsigned long long), s));
+		CK(cudaMemsetAsync(m->d_route_tab_min.p, 0xff, (size_t)size * sizeof(uint32_t), s));
+		t.tab_keys = m->d_route_tab_keys.p;
+		t.tab_min = m->d_route_tab_min.p;
 		t.tab_mask = size - 1;
 	}
 	k_inbox<<<m->sm_count * 4, 256, 0, s>>>(M, first, count, t);
@@ -1980,15 +2009,12 @@ int ufo_b200_query(ufo_b200_map* m, const uint64_t* codes, const uint32_t* depth
 		CK(cudaSetDevice(m->device));
 		sync_map(m);
 		cudaStream_t s = m->stream;
-		unsigned long long* d_codes = nullptr;
-		uint32_t *d_depths = nullptr, *d_rgb = nullptr;
-		float* d_occ = nullptr;
-		uint8_t* d_flags = nullptr;
-		CK(cudaMalloc(&d_codes, n * 8));
-		CK(cudaMalloc(&d_depths, n * 4));
-		CK(cudaMalloc(&d_occ, n * 4));
-		CK(cudaMalloc(&d_flags, n));
-		if (rgb) CK(cudaMalloc(&d_rgb, n * 4));
+		DevBuf b_codes, b_depths, b_occ, b_flags, b_rgb;
+		unsigned long long* d_codes = b_codes.alloc<unsigned long long>(n);
+		uint32_t* d_depths = b_depths.alloc<uint32_t>(n);
+		float* d_occ = b_occ.alloc<float>(n);
+		uint8_t* d_flags = b_flags.alloc<uint8_t>(n);
+		uint32_t* d_rgb = rgb ? b_rgb.alloc<uint32_t>(n) : nullptr;
 		CK(cudaMemcpyAsync(d_codes, codes, n * 8, cudaMemcpyHostToDevice, s));
 		CK(cudaMemcpyAsync(d_depths, depths, n * 4, cudaMemcpyHostToDevice, s));
 		k_query<<<(uint32_t)((n + 255) / 256), 256, 0, s>>>(m->M, d_codes, d_depths, (uint32_t)n, d_occ, d_flags, d_rgb);
@@ -2007,11 +2033,6 @@ int ufo_b200_query(ufo_b200_map* m, const uint64_t* codes, const uint32_t* depth
 				rgb[3 * i + 1] = (h_rgb[i] >> 8) & 0xff;
 				rgb[3 * i + 2] = (h_rgb[i] >> 16) & 0xff;
 			}
-		cudaFree(d_codes);
-		cudaFree(d_depths);
-		cudaFree(d_occ);
-		cudaFree(d_flags);
-		if (d_rgb) cudaFree(d_rgb);
 		return (int)UFO_B200_OK;
 	});
 }
@@ -2024,17 +2045,17 @@ int ufo_b200_export_leaves(ufo_b200_map* m, uint64_t* codes, float* logodds, uin
 		CK(cudaSetDevice(m->device));
 		sync_map(m);
 		cudaStream_t s = m->stream;
-		unsigned long long* d_count = nullptr;
-		CK(cudaMalloc(&d_count, 8));
+		DevBuf b_count, b_codes, b_occ, b_rgb;
+		unsigned long long* d_count = b_count.alloc<unsigned long long>(1);
 		CK(cudaMemsetAsync(d_count, 0, 8, s));
 		unsigned long long* d_codes = nullptr;
 		float* d_occ = nullptr;
 		uint32_t* d_rgb = nullptr;
 		bool fill = codes != nullptr && cap > 0;
 		if (fill) {
-			CK(cudaMalloc(&d_codes, cap * 8));
-			CK(cudaMalloc(&d_occ, cap * 4));
-			if (rgb) CK(cudaMalloc(&d_rgb, cap * 4));
+			d_codes = b_codes.alloc<unsigned long long>(cap);
+			d_occ = b_occ.alloc<float>(cap);
+			if (rgb) d_rgb = b_rgb.alloc<uint32_t>(cap);
 		}
 		size_t threads = (size_t)m->n_bricks * 64 * 64;
 		if (threads)
@@ -2057,11 +2078,7 @@ int ufo_b200_export_leaves(ufo_b200_map* m, uint64_t* codes, float* logodds, uin
 					rgb[3 * i + 2] = (h[i] >> 16) & 0xff;
 				}
 			}
-			cudaFree(d_codes);
-			cudaFree(d_occ);
-			if (d_rgb) cudaFree(d_rgb);
 		}
-		cudaFree(d_count);
 		return (int)UFO_B200_OK;
 	});
 }
@@ -2103,20 +2120,13 @@ bool volume_ok(Map* m, const ufo_b200_volume* bv, size_t n_bv)
 
 // the records of a volume in device memory for the duration of one call
 struct DeviceVolume {
-	VolRec* d = nullptr;
-	DeviceVolume() = default;
-	DeviceVolume(const DeviceVolume&) = delete;
-	DeviceVolume& operator=(const DeviceVolume&) = delete;
-	~DeviceVolume()
-	{
-		if (d) cudaFree(d);
-	}
+	DevBuf recs;
 	Volume upload(const Volume& host, cudaStream_t s)
 	{
 		Volume out = host;  // lo / hi travel as they are
 		out.rec = nullptr;
 		if (!host.n) return out;
-		CK(cudaMalloc(&d, sizeof(VolRec) * host.n));
+		VolRec* d = recs.alloc<VolRec>(host.n);
 		CK(cudaMemcpyAsync(d, host.rec, sizeof(VolRec) * host.n, cudaMemcpyHostToDevice, s));
 		out.rec = d;
 		return out;
@@ -2298,102 +2308,90 @@ int export_image(Map* m, int pruned, uint32_t min_depth, const Volume& vol, bool
 	}
 	plan.info.resize(nb);
 	std::vector<unsigned long long> keys(nb);
+	DevBuf b_info, b_offs, b_out;
 	BrickInfo* d_info = nullptr;
-	unsigned long long* d_offs = nullptr;
-	uint8_t* d_out = nullptr;
 	DeviceVolume dvol;
-	auto cleanup = [&]() {
-		if (d_info) cudaFree(d_info);
-		if (d_offs) cudaFree(d_offs);
-		if (d_out) cudaFree(d_out);
+	// an empty or single-box volume takes the instantiation with the inline box test
+	Volume hv = plan.vol;
+	const bool general = volume_is_general(hv);
+	const Volume dv = dvol.upload(hv, s);
+	auto brick_stream = [&](uint32_t n, size_t smem, const unsigned long long* offs, uint8_t* out) {
+		if (color && general) k_brick_stream<true, true><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
+		else if (color) k_brick_stream<true, false><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
+		else if (general) k_brick_stream<false, true><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
+		else k_brick_stream<false, false><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
 	};
-	try {
-		// an empty or single-box volume takes the instantiation with the inline box test
-		Volume hv = plan.vol;
-		const bool general = volume_is_general(hv);
-		const Volume dv = dvol.upload(hv, s);
-		auto brick_stream = [&](uint32_t n, size_t smem, const unsigned long long* offs, uint8_t* out) {
-			if (color && general) k_brick_stream<true, true><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
-			else if (color) k_brick_stream<true, false><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
-			else if (general) k_brick_stream<false, true><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
-			else k_brick_stream<false, false><<<n, 64, smem, s>>>(m->M, n, pruned, min_depth, dv, d_info, offs, out);
-		};
-		if (nb) {
-			CK(cudaMalloc(&d_info, sizeof(BrickInfo) * nb));
-			brick_stream(nb, 0, nullptr, nullptr);
-			CK(cudaGetLastError());
-			CK(cudaMemcpyAsync(plan.info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
-			CK(cudaMemcpyAsync(keys.data(), m->M.brick_key, 8ull * nb, cudaMemcpyDeviceToHost, s));
-			CK(cudaStreamSynchronize(s));
-		}
-		// bricks that are part of the tree, in Morton order; a leaf brick with the default payload is
-		// indistinguishable from untouched space
-		std::vector<std::pair<unsigned long long, uint32_t>> sorted;
-		sorted.reserve(nb);
-		for (uint32_t b = 0; b < nb; ++b) {
-			const BrickInfo& bi = plan.info[b];
-			if (bi.flags & 2u) continue;
-			if (!(bi.flags & 1u) && bi.occ == 0.0f && bi.rgb == 0u) continue;
-			uint32_t x, y, z;
-			unpack_key(keys[b], x, y, z);
-			sorted.emplace_back(spread3_host(x) | (spread3_host(y) << 1) | (spread3_host(z) << 2), b);
-		}
-		std::sort(sorted.begin(), sorted.end());
-		plan.order.resize(sorted.size());
-		plan.codes.resize(sorted.size());
-		std::vector<unsigned long long> offs(nb, ~0ull);
-		unsigned long long packed_bytes = 0;
-		for (size_t i = 0; i < sorted.size(); ++i) {
-			plan.codes[i] = sorted[i].first;
-			plan.order[i] = sorted[i].second;
-			const BrickInfo& bi = plan.info[sorted[i].second];
-			if (bi.flags & 4u) {
-				offs[sorted[i].second] = packed_bytes;
-				packed_bytes += bi.size;
-			}
-		}
-		bool root_has = false;
-		unsigned long long data_size = 1 + plan.P;  // children byte + root payload
-		if (!sorted.empty()) {
-			build_upper(plan, plan.levels, 0, sorted.size(), c0);
-			root_has = plan.nodes[0].has;
-			if (root_has) data_size = 1 + plan.nodes[0].size;
-		}
-		std::vector<uint8_t> packed(packed_bytes);
-		if (packed_bytes) {
-			CK(cudaMalloc(&d_offs, 8ull * nb));
-			CK(cudaMalloc(&d_out, packed_bytes));
-			CK(cudaMemcpyAsync(d_offs, offs.data(), 8ull * nb, cudaMemcpyHostToDevice, s));
-			brick_stream(nb, kBrickStreamMax, d_offs, d_out);
-			CK(cudaGetLastError());
-			CK(cudaMemcpyAsync(packed.data(), d_out, packed_bytes, cudaMemcpyDeviceToHost, s));
-			CK(cudaStreamSynchronize(s));
-		}
-		unsigned long long produced = 0;
-		auto counted = [&](const void* p, size_t len) {
-			sink(p, len);
-			produced += len;
-		};
-		if (with_header) {
-			char head[512];
-			const int hl = header(head, sizeof head, data_size);
-			counted(head, (size_t)hl);
-		}
-		const uint8_t children = root_has ? 0xff : 0x00;
-		counted(&children, 1);
-		if (root_has) {
-			emit_upper(plan, offs, packed.data(), 0, plan.levels, counted);
-		} else {
-			const float occ = sorted.empty() ? 0.0f : plan.nodes[0].occ;
-			const uint32_t rgb = sorted.empty() ? 0u : plan.nodes[0].rgb;
-			put_payload_host(counted, plan.P, occ, rgb);
-		}
-		*total = produced;
-	} catch (...) {
-		cleanup();
-		throw;
+	if (nb) {
+		d_info = b_info.alloc<BrickInfo>(nb);
+		brick_stream(nb, 0, nullptr, nullptr);
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(plan.info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
+		CK(cudaMemcpyAsync(keys.data(), m->M.brick_key, 8ull * nb, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
 	}
-	cleanup();
+	// bricks that are part of the tree, in Morton order; a leaf brick with the default payload is
+	// indistinguishable from untouched space
+	std::vector<std::pair<unsigned long long, uint32_t>> sorted;
+	sorted.reserve(nb);
+	for (uint32_t b = 0; b < nb; ++b) {
+		const BrickInfo& bi = plan.info[b];
+		if (bi.flags & 2u) continue;
+		if (!(bi.flags & 1u) && bi.occ == 0.0f && bi.rgb == 0u) continue;
+		uint32_t x, y, z;
+		unpack_key(keys[b], x, y, z);
+		sorted.emplace_back(spread3_host(x) | (spread3_host(y) << 1) | (spread3_host(z) << 2), b);
+	}
+	std::sort(sorted.begin(), sorted.end());
+	plan.order.resize(sorted.size());
+	plan.codes.resize(sorted.size());
+	std::vector<unsigned long long> offs(nb, ~0ull);
+	unsigned long long packed_bytes = 0;
+	for (size_t i = 0; i < sorted.size(); ++i) {
+		plan.codes[i] = sorted[i].first;
+		plan.order[i] = sorted[i].second;
+		const BrickInfo& bi = plan.info[sorted[i].second];
+		if (bi.flags & 4u) {
+			offs[sorted[i].second] = packed_bytes;
+			packed_bytes += bi.size;
+		}
+	}
+	bool root_has = false;
+	unsigned long long data_size = 1 + plan.P;  // children byte + root payload
+	if (!sorted.empty()) {
+		build_upper(plan, plan.levels, 0, sorted.size(), c0);
+		root_has = plan.nodes[0].has;
+		if (root_has) data_size = 1 + plan.nodes[0].size;
+	}
+	std::vector<uint8_t> packed(packed_bytes);
+	if (packed_bytes) {
+		unsigned long long* d_offs = b_offs.alloc<unsigned long long>(nb);
+		uint8_t* d_out = b_out.alloc<uint8_t>(packed_bytes);
+		CK(cudaMemcpyAsync(d_offs, offs.data(), 8ull * nb, cudaMemcpyHostToDevice, s));
+		brick_stream(nb, kBrickStreamMax, d_offs, d_out);
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(packed.data(), d_out, packed_bytes, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+	}
+	unsigned long long produced = 0;
+	auto counted = [&](const void* p, size_t len) {
+		sink(p, len);
+		produced += len;
+	};
+	if (with_header) {
+		char head[512];
+		const int hl = header(head, sizeof head, data_size);
+		counted(head, (size_t)hl);
+	}
+	const uint8_t children = root_has ? 0xff : 0x00;
+	counted(&children, 1);
+	if (root_has) {
+		emit_upper(plan, offs, packed.data(), 0, plan.levels, counted);
+	} else {
+		const float occ = sorted.empty() ? 0.0f : plan.nodes[0].occ;
+		const uint32_t rgb = sorted.empty() ? 0u : plan.nodes[0].rgb;
+		put_payload_host(counted, plan.P, occ, rgb);
+	}
+	*total = produced;
 	return UFO_B200_OK;
 }
 }  // namespace
@@ -2552,70 +2550,49 @@ int ufo_b200_set_value_volume_bv(ufo_b200_map* m, const ufo_b200_volume* bv, dou
 		const int general = volume_is_general(hvk) ? 1 : 0;
 		const Volume dv = dvol.upload(hvk, s);
 		// descent from the root to the bricks, one level per launch; frontier = (key, centre)
-		unsigned long long *d_key[2] = {nullptr, nullptr};
-		double* d_c[2] = {nullptr, nullptr};
-		unsigned int* d_n = nullptr;
-		auto cleanup = [&]() {
-			for (int i = 0; i < 2; ++i) {
-				if (d_key[i]) cudaFree(d_key[i]);
-				if (d_c[i]) cudaFree(d_c[i]);
-				d_key[i] = nullptr;
-				d_c[i] = nullptr;
-			}
-			if (d_n) cudaFree(d_n);
-			d_n = nullptr;
-		};
+		DevBuf b_key[2], b_c[2], b_n;
+		unsigned long long* d_key[2] = {b_key[0].alloc<unsigned long long>(1), nullptr};
+		double* d_c[2] = {b_c[0].alloc<double>(3), nullptr};
+		unsigned int* d_n = b_n.alloc<unsigned int>(1);
 		int rc = UFO_B200_OK;
-		try {
-			CK(cudaMalloc(&d_n, sizeof(unsigned int)));
-			CK(cudaMalloc(&d_key[0], 8));
-			CK(cudaMalloc(&d_c[0], 24));
-			CK(cudaMemsetAsync(d_key[0], 0, 8, s));
-			CK(cudaMemsetAsync(d_c[0], 0, 24, s));
-			uint32_t n_in = 1, cur = 0;
-			for (uint32_t d = g.depth_levels; d > 4 && n_in; --d) {
-				// children of depth d - 1
-				const uint32_t cap = (uint32_t)std::min<unsigned long long>(8ull * n_in, kVolumeBrickLimit);
-				const uint32_t nxt = cur ^ 1u;
-				CK(cudaMalloc(&d_key[nxt], 8ull * cap));
-				CK(cudaMalloc(&d_c[nxt], 24ull * cap));
-				CK(cudaMemsetAsync(d_n, 0, sizeof(unsigned int), s));
-				const unsigned long long threads = 8ull * n_in;
-				k_volume_descend<<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(dv, d_key[cur], d_c[cur], n_in, g.half_size[d - 1],
-				                                                                    d_key[nxt], d_c[nxt], cap, d_n);
-				CK(cudaGetLastError());
-				unsigned int got = 0;
-				CK(cudaMemcpyAsync(&got, d_n, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
-				CK(cudaStreamSynchronize(s));
-				CK(cudaFree(d_key[cur]));
-				CK(cudaFree(d_c[cur]));
-				d_key[cur] = nullptr;
-				d_c[cur] = nullptr;
-				if (got > kVolumeBrickLimit) {
-					m->set_error("setValueVolume: %u nodes of depth %u pass the volume (limit 4194304)", got, d - 1);
-					cleanup();
-					return (int)UFO_B200_E_UNSUPPORTED;
-				}
-				n_in = got;
-				cur = nxt;
+		CK(cudaMemsetAsync(d_key[0], 0, 8, s));
+		CK(cudaMemsetAsync(d_c[0], 0, 24, s));
+		uint32_t n_in = 1, cur = 0;
+		for (uint32_t d = g.depth_levels; d > 4 && n_in; --d) {
+			// children of depth d - 1
+			const uint32_t cap = (uint32_t)std::min<unsigned long long>(8ull * n_in, kVolumeBrickLimit);
+			const uint32_t nxt = cur ^ 1u;
+			d_key[nxt] = b_key[nxt].alloc<unsigned long long>(cap);
+			d_c[nxt] = b_c[nxt].alloc<double>(3ull * cap);
+			CK(cudaMemsetAsync(d_n, 0, sizeof(unsigned int), s));
+			const unsigned long long threads = 8ull * n_in;
+			k_volume_descend<<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(dv, d_key[cur], d_c[cur], n_in, g.half_size[d - 1],
+			                                                                    d_key[nxt], d_c[nxt], cap, d_n);
+			CK(cudaGetLastError());
+			unsigned int got = 0;
+			CK(cudaMemcpyAsync(&got, d_n, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+			CK(cudaStreamSynchronize(s));
+			b_key[cur].release();
+			b_c[cur].release();
+			if (got > kVolumeBrickLimit) {
+				m->set_error("setValueVolume: %u nodes of depth %u pass the volume (limit 4194304)", got, d - 1);
+				return (int)UFO_B200_E_UNSUPPORTED;
 			}
-			if (n_in) {
-				VolumeArgs v{};
-				v.vol = dv;
-				v.min_depth = min_depth;
-				v.nx = n_in;
-				v.ny = 1;
-				v.nz = 1;
-				v.cand = d_key[cur];
-				v.general = general;
-				rc = set_value_volume_run(m, v, occupancy);
-				sync_map(m);
-			}
-		} catch (...) {
-			cleanup();
-			throw;
+			n_in = got;
+			cur = nxt;
 		}
-		cleanup();
+		if (n_in) {
+			VolumeArgs v{};
+			v.vol = dv;
+			v.min_depth = min_depth;
+			v.nx = n_in;
+			v.ny = 1;
+			v.nz = 1;
+			v.cand = d_key[cur];
+			v.general = general;
+			rc = set_value_volume_run(m, v, occupancy);
+			sync_map(m);
+		}
 		return rc;
 	});
 }
@@ -2864,11 +2841,7 @@ int ufo_b200_clear(ufo_b200_map* m)
 			CK(cudaMemsetAsync(M.alias_hit, 0, nb * 8, s));
 		}
 		if (M.chg_mask) CK(cudaMemsetAsync(M.chg_mask, 0, nb * 8, s));
-		if (M.vol) {
-			const size_t vb = (size_t)m->vol_db_cap * m->vol_db_cap * m->vol_db_cap;
-			CK(cudaMemsetAsync(M.vol, 0, vb * 512, s));
-			CK(cudaMemsetAsync(M.vol_dirty, 0, (vb / 64 + 1) * 8, s));
-		}
+		wipe_volume(m);
 		m->n_blocks = 0;
 		m->n_bricks = 0;
 		m->n_upper = 0;
@@ -2919,33 +2892,31 @@ int ufo_b200_route_setup(ufo_b200_map* m, uint32_t rank, uint32_t world, uint32_
 	return guarded(m, [&]() {
 		CK(cudaSetDevice(m->device));
 		sync_map(m);
-		if (m->n_bricks != 0 || m->route_inbox || m->M.shard_world > 1) {
+		if (m->n_bricks != 0 || m->route_inbox.p || m->M.shard_world > 1) {
 			m->set_error("ufo_b200_route_setup: needs an empty, unsharded map and may be called once");
 			return (int)UFO_B200_E_INVALID;
 		}
 		const uint32_t hit_words = m->M.color ? 2u : 1u;
 		const size_t total = route_layout(world, cap_bricks, cap_hits, hit_words, &m->route_region, &m->route_miss_off,
 		                                  &m->route_hit_off);
-		CK(cudaMalloc(reinterpret_cast<void**>(&m->route_inbox), total));
-		CK(cudaMemset(m->route_inbox, 0, total));
-		CK(cudaMalloc(reinterpret_cast<void**>(&m->M.route), sizeof(RouteTable)));
-		CK(cudaMemset(m->M.route, 0, sizeof(RouteTable)));
+		m->route_inbox.ensure(m, total, 0);
+		m->route_table.ensure(m, sizeof(RouteTable), 0);
+		m->M.route = m->route_table.p;
 		CK(cudaHostAlloc(reinterpret_cast<void**>(&m->h_route), sizeof(RouteTable), cudaHostAllocDefault));
 		CK(cudaHostAlloc(reinterpret_cast<void**>(&m->h_route_flag), 4 * sizeof(uint32_t), cudaHostAllocDefault));
 		memset(m->h_route_flag, 0, 4 * sizeof(uint32_t));
-		m->device_bytes += total + sizeof(RouteTable);
 		if (m->M.color) {
 			// apply table: every hit record of every source of one apply call, at most half full
 			m->route_tab_size = std::max(1u << 12, next_pow2(2ull * world * cap_hits));
-			dev_alloc(m->d_route_tab_keys, m->route_tab_size, 0xff, m->stream, m->device_bytes);
-			dev_alloc(m->d_route_tab_min, m->route_tab_size, 0xff, m->stream, m->device_bytes);
-			CK(cudaStreamSynchronize(m->stream));
+			m->d_route_tab_keys.ensure(m, (size_t)m->route_tab_size * sizeof(unsigned long long), 0xff);
+			m->d_route_tab_min.ensure(m, (size_t)m->route_tab_size * sizeof(uint32_t), 0xff);
 		}
+		CK(cudaStreamSynchronize(m->stream));  // peers write into the inbox as soon as they have its handle
 		m->route_cap_m = cap_bricks;
 		m->route_cap_h = cap_hits;
 		m->M.route_rank = rank;
 		m->M.route_world = world;
-		*inbox = m->route_inbox;
+		*inbox = m->route_inbox.p;
 		return (int)UFO_B200_OK;
 	});
 }
@@ -3029,20 +3000,12 @@ int ufo_b200_enable_change_detection(ufo_b200_map* m, int enable)
 	return guarded(m, [&]() {
 		CK(cudaSetDevice(m->device));
 		sync_map(m);
-		DeviceMap& M = m->M;
-		if (enable && !M.chg_mask) {
-			dev_alloc(M.chg_mask, (size_t)M.brick_cap * 64, 0, m->stream, m->device_bytes);
-			CK(cudaStreamSynchronize(m->stream));
-		} else if (!enable && M.chg_mask) {
-			// the reference keeps the recorded set when detection is switched off; so do we: the
-			// mask array stays, recording stops
-			m->chg_paused = M.chg_mask;
-			M.chg_mask = nullptr;
-		}
-		if (enable && !M.chg_mask && m->chg_paused) {
-			M.chg_mask = m->chg_paused;
-			m->chg_paused = nullptr;
-		}
+		// the reference keeps the recorded set when detection is switched off; so do we: the mask
+		// array stays, recording stops
+		m->chg_recording = enable != 0;
+		if (enable) alloc_arrays(m, Pool::Brick, Have::Changes);
+		m->M.chg_mask = m->chg_recording ? m->chg_mask : nullptr;
+		CK(cudaStreamSynchronize(m->stream));
 		return (int)UFO_B200_OK;
 	});
 }
@@ -3053,8 +3016,7 @@ int ufo_b200_reset_change_detection(ufo_b200_map* m)
 	return guarded(m, [&]() {
 		CK(cudaSetDevice(m->device));
 		sync_map(m);
-		unsigned long long* p = m->M.chg_mask ? m->M.chg_mask : m->chg_paused;
-		if (p) CK(cudaMemsetAsync(p, 0, (size_t)m->M.brick_cap * 64 * 8, m->stream));
+		if (m->chg_mask) CK(cudaMemsetAsync(m->chg_mask, 0, (size_t)m->M.brick_cap * 64 * 8, m->stream));
 		return (int)UFO_B200_OK;
 	});
 }
@@ -3067,47 +3029,37 @@ int ufo_b200_changed_codes(ufo_b200_map* m, uint32_t depth, uint64_t* codes, siz
 		sync_map(m);
 		*n = 0;
 		DeviceMap M = m->M;
-		if (!M.chg_mask) M.chg_mask = m->chg_paused;
+		M.chg_mask = m->chg_mask;  // recording or not
 		if (!M.chg_mask || !m->n_bricks) return (int)UFO_B200_OK;
 		if (depth > M.g.depth_levels) return (int)UFO_B200_E_INVALID;
 		const uint32_t dd = std::min(depth, 4u);
 		cudaStream_t s = m->stream;
-		unsigned long long *d_count = nullptr, *d_codes = nullptr;
-		CK(cudaMalloc(&d_count, 8));
-		auto cleanup = [&]() {
-			if (d_count) cudaFree(d_count);
-			if (d_codes) cudaFree(d_codes);
-		};
-		try {
-			const uint32_t grid = (uint32_t)(((size_t)m->n_bricks * 64 + 255) / 256);
+		DevBuf b_count, b_codes;
+		unsigned long long* d_count = b_count.alloc<unsigned long long>(1);
+		const uint32_t grid = (uint32_t)(((size_t)m->n_bricks * 64 + 255) / 256);
+		CK(cudaMemsetAsync(d_count, 0, 8, s));
+		k_changed<<<grid, 256, 0, s>>>(M, m->n_bricks, dd, nullptr, 0, d_count);
+		unsigned long long cnt = 0;
+		CK(cudaMemcpyAsync(&cnt, d_count, 8, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		std::vector<unsigned long long> h(cnt);
+		if (cnt) {
+			unsigned long long* d_codes = b_codes.alloc<unsigned long long>(cnt);
 			CK(cudaMemsetAsync(d_count, 0, 8, s));
-			k_changed<<<grid, 256, 0, s>>>(M, m->n_bricks, dd, nullptr, 0, d_count);
-			unsigned long long cnt = 0;
-			CK(cudaMemcpyAsync(&cnt, d_count, 8, cudaMemcpyDeviceToHost, s));
+			k_changed<<<grid, 256, 0, s>>>(M, m->n_bricks, dd, d_codes, cnt, d_count);
+			CK(cudaMemcpyAsync(h.data(), d_codes, cnt * 8, cudaMemcpyDeviceToHost, s));
 			CK(cudaStreamSynchronize(s));
-			std::vector<unsigned long long> h(cnt);
-			if (cnt) {
-				CK(cudaMalloc(&d_codes, cnt * 8));
-				CK(cudaMemsetAsync(d_count, 0, 8, s));
-				k_changed<<<grid, 256, 0, s>>>(M, m->n_bricks, dd, d_codes, cnt, d_count);
-				CK(cudaMemcpyAsync(h.data(), d_codes, cnt * 8, cudaMemcpyDeviceToHost, s));
-				CK(cudaStreamSynchronize(s));
-			}
-			if (depth >= 4) {
-				// ancestors above the brick + duplicates: snap to `depth` (with the centre bits) and unique
-				const unsigned long long lowmask = depth >= 21 ? ~0ull : ((1ull << (3 * depth)) - 1ull);
-				const unsigned long long centre = key_to_code({1u << (depth - 1), 1u << (depth - 1), 1u << (depth - 1)});
-				for (auto& c : h) c = (c & ~lowmask) | centre;
-				std::sort(h.begin(), h.end());
-				h.erase(std::unique(h.begin(), h.end()), h.end());
-			}
-			*n = h.size();
-			if (codes) std::memcpy(codes, h.data(), std::min(cap, h.size()) * 8);
-		} catch (...) {
-			cleanup();
-			throw;
 		}
-		cleanup();
+		if (depth >= 4) {
+			// ancestors above the brick + duplicates: snap to `depth` (with the centre bits) and unique
+			const unsigned long long lowmask = depth >= 21 ? ~0ull : ((1ull << (3 * depth)) - 1ull);
+			const unsigned long long centre = key_to_code({1u << (depth - 1), 1u << (depth - 1), 1u << (depth - 1)});
+			for (auto& c : h) c = (c & ~lowmask) | centre;
+			std::sort(h.begin(), h.end());
+			h.erase(std::unique(h.begin(), h.end()), h.end());
+		}
+		*n = h.size();
+		if (codes) std::memcpy(codes, h.data(), std::min(cap, h.size()) * 8);
 		return (int)UFO_B200_OK;
 	});
 }
@@ -3184,29 +3136,16 @@ int ufo_b200_cast_rays(ufo_b200_map* m, const double* origins, const double* dir
 				rays[6 * i + 3 + k] = directions[3 * i + k];
 			}
 		}
-		double* d_rays = nullptr;
-		unsigned long long* d_codes = nullptr;
-		uint8_t* d_hit = nullptr;
-		auto cleanup = [&]() {
-			if (d_rays) cudaFree(d_rays);
-			if (d_codes) cudaFree(d_codes);
-			if (d_hit) cudaFree(d_hit);
-		};
-		try {
-			CK(cudaMalloc(&d_rays, rays.size() * 8));
-			CK(cudaMalloc(&d_codes, n * 8));
-			CK(cudaMalloc(&d_hit, n));
-			CK(cudaMemcpyAsync(d_rays, rays.data(), rays.size() * 8, cudaMemcpyHostToDevice, s));
-			k_cast_rays<<<(uint32_t)((n + 127) / 128), 128, 0, s>>>(m->M, d_rays, (uint32_t)n, ignore_unknown, max_range, depth, d_codes, d_hit);
-			CK(cudaGetLastError());
-			CK(cudaMemcpyAsync(codes, d_codes, n * 8, cudaMemcpyDeviceToHost, s));
-			CK(cudaMemcpyAsync(hit, d_hit, n, cudaMemcpyDeviceToHost, s));
-			CK(cudaStreamSynchronize(s));
-		} catch (...) {
-			cleanup();
-			throw;
-		}
-		cleanup();
+		DevBuf b_rays, b_codes, b_hit;
+		double* d_rays = b_rays.alloc<double>(rays.size());
+		unsigned long long* d_codes = b_codes.alloc<unsigned long long>(n);
+		uint8_t* d_hit = b_hit.alloc<uint8_t>(n);
+		CK(cudaMemcpyAsync(d_rays, rays.data(), rays.size() * 8, cudaMemcpyHostToDevice, s));
+		k_cast_rays<<<(uint32_t)((n + 127) / 128), 128, 0, s>>>(m->M, d_rays, (uint32_t)n, ignore_unknown, max_range, depth, d_codes, d_hit);
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(codes, d_codes, n * 8, cudaMemcpyDeviceToHost, s));
+		CK(cudaMemcpyAsync(hit, d_hit, n, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
 		return (int)UFO_B200_OK;
 	});
 }
@@ -3236,69 +3175,58 @@ int export_nodes(Map* m, uint32_t depth, int occupied, int free_space, int unkno
 	}
 	{
 		cudaStream_t s = m->stream;
-		unsigned long long *d_count = nullptr, *d_codes = nullptr;
+		unsigned long long* d_codes = nullptr;
 		float* d_occ = nullptr;
 		uint32_t* d_rgb = nullptr;
-		uint8_t* d_ok = nullptr;
-		double* d_bc = nullptr;
+		DevBuf b_count, b_codes, b_occ, b_rgb, b_ok, b_bc;
 		DeviceVolume dvol;
-		auto cleanup = [&]() {
-			for (void* p : {(void*)d_count, (void*)d_codes, (void*)d_occ, (void*)d_rgb, (void*)d_ok, (void*)d_bc})
-				if (p) cudaFree(p);
-		};
-		try {
-			Volume hv = vol;
-			volume_is_general(hv);  // lo / hi of a single box, tested inline without the chain
-			f.vol = dvol.upload(hv, s);
-			if (f.chain && depth <= 4 && m->n_bricks) {
-				CK(cudaMalloc(&d_ok, m->n_bricks));
-				CK(cudaMalloc(&d_bc, 24ull * m->n_bricks));
-				k_brick_chain<<<(m->n_bricks + 255) / 256, 256, 0, s>>>(m->M, m->n_bricks, f.vol, d_ok, d_bc);
-				f.brick_ok = d_ok;
-				f.brick_c = d_bc;
-			}
-			CK(cudaMalloc(&d_count, 8));
-			const bool fill = codes != nullptr && cap > 0;
-			if (fill) {
-				CK(cudaMalloc(&d_codes, cap * 8));
-				CK(cudaMalloc(&d_occ, cap * 4));
-				if (rgb) CK(cudaMalloc(&d_rgb, cap * 4));
-			}
-			CK(cudaMemsetAsync(d_count, 0, 8, s));
-			if (depth <= 4) {
-				const size_t threads = (size_t)m->n_bricks * 64;
-				if (threads && f.chain)
-					k_export_nodes<true><<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(m->M, m->n_bricks, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
-				else if (threads)
-					k_export_nodes<false><<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(m->M, m->n_bricks, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
-			} else if (m->n_upper) {
-				if (f.chain) k_export_upper<true><<<(m->n_upper + 255) / 256, 256, 0, s>>>(m->M, m->n_upper, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
-				else k_export_upper<false><<<(m->n_upper + 255) / 256, 256, 0, s>>>(m->M, m->n_upper, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
-			}
-			CK(cudaGetLastError());
-			unsigned long long cnt = 0;
-			CK(cudaMemcpyAsync(&cnt, d_count, 8, cudaMemcpyDeviceToHost, s));
-			CK(cudaStreamSynchronize(s));
-			*n = (size_t)cnt;
-			if (fill) {
-				const size_t k = std::min<size_t>(cnt, cap);
-				CK(cudaMemcpy(codes, d_codes, k * 8, cudaMemcpyDeviceToHost));
-				if (logodds) CK(cudaMemcpy(logodds, d_occ, k * 4, cudaMemcpyDeviceToHost));
-				if (rgb) {
-					std::vector<uint32_t> h(k);
-					CK(cudaMemcpy(h.data(), d_rgb, k * 4, cudaMemcpyDeviceToHost));
-					for (size_t i = 0; i < k; ++i) {
-						rgb[3 * i] = h[i] & 0xff;
-						rgb[3 * i + 1] = (h[i] >> 8) & 0xff;
-						rgb[3 * i + 2] = (h[i] >> 16) & 0xff;
-					}
+		Volume hv = vol;
+		volume_is_general(hv);  // lo / hi of a single box, tested inline without the chain
+		f.vol = dvol.upload(hv, s);
+		if (f.chain && depth <= 4 && m->n_bricks) {
+			uint8_t* d_ok = b_ok.alloc<uint8_t>(m->n_bricks);
+			double* d_bc = b_bc.alloc<double>(3ull * m->n_bricks);
+			k_brick_chain<<<(m->n_bricks + 255) / 256, 256, 0, s>>>(m->M, m->n_bricks, f.vol, d_ok, d_bc);
+			f.brick_ok = d_ok;
+			f.brick_c = d_bc;
+		}
+		unsigned long long* d_count = b_count.alloc<unsigned long long>(1);
+		const bool fill = codes != nullptr && cap > 0;
+		if (fill) {
+			d_codes = b_codes.alloc<unsigned long long>(cap);
+			d_occ = b_occ.alloc<float>(cap);
+			if (rgb) d_rgb = b_rgb.alloc<uint32_t>(cap);
+		}
+		CK(cudaMemsetAsync(d_count, 0, 8, s));
+		if (depth <= 4) {
+			const size_t threads = (size_t)m->n_bricks * 64;
+			if (threads && f.chain)
+				k_export_nodes<true><<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(m->M, m->n_bricks, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
+			else if (threads)
+				k_export_nodes<false><<<(uint32_t)((threads + 255) / 256), 256, 0, s>>>(m->M, m->n_bricks, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
+		} else if (m->n_upper) {
+			if (f.chain) k_export_upper<true><<<(m->n_upper + 255) / 256, 256, 0, s>>>(m->M, m->n_upper, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
+			else k_export_upper<false><<<(m->n_upper + 255) / 256, 256, 0, s>>>(m->M, m->n_upper, f, d_codes, d_occ, d_rgb, fill ? cap : 0, d_count);
+		}
+		CK(cudaGetLastError());
+		unsigned long long cnt = 0;
+		CK(cudaMemcpyAsync(&cnt, d_count, 8, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		*n = (size_t)cnt;
+		if (fill) {
+			const size_t k = std::min<size_t>(cnt, cap);
+			CK(cudaMemcpy(codes, d_codes, k * 8, cudaMemcpyDeviceToHost));
+			if (logodds) CK(cudaMemcpy(logodds, d_occ, k * 4, cudaMemcpyDeviceToHost));
+			if (rgb) {
+				std::vector<uint32_t> h(k);
+				CK(cudaMemcpy(h.data(), d_rgb, k * 4, cudaMemcpyDeviceToHost));
+				for (size_t i = 0; i < k; ++i) {
+					rgb[3 * i] = h[i] & 0xff;
+					rgb[3 * i + 1] = (h[i] >> 8) & 0xff;
+					rgb[3 * i + 2] = (h[i] >> 16) & 0xff;
 				}
 			}
-		} catch (...) {
-			cleanup();
-			throw;
 		}
-		cleanup();
 	}
 	return (int)UFO_B200_OK;
 }
@@ -3421,124 +3349,108 @@ int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, floa
 	w.a.free_thr = m->M.free_thr;
 	w.default_flags = m->M.default_flags;
 	w.offs.assign(nb, ~0ull);
+	DevBuf b_info, b_offs, b_out, b_qcodes, b_qdepths, b_qocc, b_qflags, b_qrgb;
 	BrickInfo* d_info = nullptr;
-	unsigned long long* d_offs = nullptr;
-	IterRec* d_out = nullptr;
-	unsigned long long* d_qcodes = nullptr;
-	uint32_t *d_qdepths = nullptr, *d_qrgb = nullptr;
-	float* d_qocc = nullptr;
-	uint8_t* d_qflags = nullptr;
 	DeviceVolume dvol;
-	auto cleanup = [&]() {
-		for (void* p : {(void*)d_info, (void*)d_offs, (void*)d_out, (void*)d_qcodes, (void*)d_qdepths, (void*)d_qrgb, (void*)d_qocc,
-		                (void*)d_qflags})
-			if (p) cudaFree(p);
+	Volume hv = args.vol;
+	const bool general = volume_is_general(hv);
+	IterArgs da = w.a;
+	da.vol = dvol.upload(hv, s);
+	auto brick_iter = [&](const unsigned long long* offs, IterRec* out) {
+		if (color && general) k_brick_iter<true, true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+		else if (color) k_brick_iter<true, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+		else if (general) k_brick_iter<false, true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+		else k_brick_iter<false, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
 	};
-	try {
-		Volume hv = args.vol;
-		const bool general = volume_is_general(hv);
-		IterArgs da = w.a;
-		da.vol = dvol.upload(hv, s);
-		auto brick_iter = [&](const unsigned long long* offs, IterRec* out) {
-			if (color && general) k_brick_iter<true, true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
-			else if (color) k_brick_iter<true, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
-			else if (general) k_brick_iter<false, true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
-			else k_brick_iter<false, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
-		};
-		std::vector<unsigned long long> keys(nb);
-		if (nb) {
-			CK(cudaMalloc(&d_info, sizeof(BrickInfo) * nb));
-			brick_iter(nullptr, nullptr);
-			CK(cudaGetLastError());
-			CK(cudaMemcpyAsync(plan.info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
-			CK(cudaMemcpyAsync(keys.data(), m->M.brick_key, 8ull * nb, cudaMemcpyDeviceToHost, s));
-			CK(cudaStreamSynchronize(s));
-		}
-		// bricks in the tree, in Morton order (as export_image: a default leaf brick is untouched space)
-		std::vector<std::pair<unsigned long long, uint32_t>> sorted;
-		sorted.reserve(nb);
-		for (uint32_t b = 0; b < nb; ++b) {
-			const BrickInfo& bi = plan.info[b];
-			if (bi.flags & 2u) continue;
-			if (!(bi.flags & 1u) && bi.occ == 0.0f && bi.rgb == 0u) continue;
-			uint32_t x, y, z;
-			unpack_key(keys[b], x, y, z);
-			sorted.emplace_back(spread3_host(x) | (spread3_host(y) << 1) | (spread3_host(z) << 2), b);
-		}
-		std::sort(sorted.begin(), sorted.end());
-		plan.order.resize(sorted.size());
-		plan.codes.resize(sorted.size());
-		for (size_t i = 0; i < sorted.size(); ++i) {
-			plan.codes[i] = sorted[i].first;
-			plan.order[i] = sorted[i].second;
-		}
-		if (sorted.empty()) {
-			iter_walk(w, -1, L, 0ull, c0, 0.0f, w.default_flags, 0u, true);
-		} else {
-			build_upper(plan, L, 0, sorted.size(), c0);
-			// values of the nodes above the bricks: ufo_b200_query's, one batch
-			const size_t nu = plan.nodes.size();
-			std::vector<unsigned long long> qc(nu);
-			std::vector<uint32_t> qd(nu), qrgb(nu, 0u);
-			upper_codes(plan, 0, L, 0ull, qc, qd);
-			w.occ.resize(nu);
-			w.flags.resize(nu);
-			CK(cudaMalloc(&d_qcodes, 8 * nu));
-			CK(cudaMalloc(&d_qdepths, 4 * nu));
-			CK(cudaMalloc(&d_qocc, 4 * nu));
-			CK(cudaMalloc(&d_qflags, nu));
-			if (color) CK(cudaMalloc(&d_qrgb, 4 * nu));
-			CK(cudaMemcpyAsync(d_qcodes, qc.data(), 8 * nu, cudaMemcpyHostToDevice, s));
-			CK(cudaMemcpyAsync(d_qdepths, qd.data(), 4 * nu, cudaMemcpyHostToDevice, s));
-			k_query<<<(uint32_t)((nu + 255) / 256), 256, 0, s>>>(m->M, d_qcodes, d_qdepths, (uint32_t)nu, d_qocc, d_qflags, d_qrgb);
-			CK(cudaGetLastError());
-			CK(cudaMemcpyAsync(w.occ.data(), d_qocc, 4 * nu, cudaMemcpyDeviceToHost, s));
-			CK(cudaMemcpyAsync(w.flags.data(), d_qflags, nu, cudaMemcpyDeviceToHost, s));
-			if (color) CK(cudaMemcpyAsync(qrgb.data(), d_qrgb, 4 * nu, cudaMemcpyDeviceToHost, s));
-			CK(cudaStreamSynchronize(s));
-			w.rgb = std::move(qrgb);
-			const UpNode& r = plan.nodes[0];
-			iter_walk(w, 0, L, 0ull, c0, r.has ? w.occ[0] : r.occ, w.flags[0], r.has ? w.rgb[0] : r.rgb, !r.has);
-		}
-		*n = (size_t)w.total;
-		if (codes && w.total && w.total <= cap) {
-			std::vector<IterRec> packed(w.packed);
-			if (w.packed) {
-				CK(cudaMalloc(&d_offs, 8ull * nb));
-				CK(cudaMalloc(&d_out, sizeof(IterRec) * w.packed));
-				CK(cudaMemcpyAsync(d_offs, w.offs.data(), 8ull * nb, cudaMemcpyHostToDevice, s));
-				brick_iter(d_offs, d_out);
-				CK(cudaGetLastError());
-				CK(cudaMemcpyAsync(packed.data(), d_out, sizeof(IterRec) * w.packed, cudaMemcpyDeviceToHost, s));
-				CK(cudaStreamSynchronize(s));
-			}
-			size_t at = 0;
-			auto put = [&](const IterRec& r) {
-				codes[at] = r.code;
-				depths[at] = (uint8_t)((r.meta >> 24) & 31u);
-				logodds[at] = r.occ;
-				flags[at] = (uint8_t)(r.meta >> 29);
-				if (rgb) {
-					rgb[3 * at] = (uint8_t)r.meta;
-					rgb[3 * at + 1] = (uint8_t)(r.meta >> 8);
-					rgb[3 * at + 2] = (uint8_t)(r.meta >> 16);
-				}
-				++at;
-			};
-			for (const auto& p : w.pieces) {
-				if (p.second == kNone) {
-					put(p.first);
-				} else {
-					const IterRec* r = packed.data() + w.offs[p.second];
-					for (uint32_t i = 0; i < plan.info[p.second].size; ++i) put(r[i]);
-				}
-			}
-		}
-	} catch (...) {
-		cleanup();
-		throw;
+	std::vector<unsigned long long> keys(nb);
+	if (nb) {
+		d_info = b_info.alloc<BrickInfo>(nb);
+		brick_iter(nullptr, nullptr);
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(plan.info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
+		CK(cudaMemcpyAsync(keys.data(), m->M.brick_key, 8ull * nb, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
 	}
-	cleanup();
+	// bricks in the tree, in Morton order (as export_image: a default leaf brick is untouched space)
+	std::vector<std::pair<unsigned long long, uint32_t>> sorted;
+	sorted.reserve(nb);
+	for (uint32_t b = 0; b < nb; ++b) {
+		const BrickInfo& bi = plan.info[b];
+		if (bi.flags & 2u) continue;
+		if (!(bi.flags & 1u) && bi.occ == 0.0f && bi.rgb == 0u) continue;
+		uint32_t x, y, z;
+		unpack_key(keys[b], x, y, z);
+		sorted.emplace_back(spread3_host(x) | (spread3_host(y) << 1) | (spread3_host(z) << 2), b);
+	}
+	std::sort(sorted.begin(), sorted.end());
+	plan.order.resize(sorted.size());
+	plan.codes.resize(sorted.size());
+	for (size_t i = 0; i < sorted.size(); ++i) {
+		plan.codes[i] = sorted[i].first;
+		plan.order[i] = sorted[i].second;
+	}
+	if (sorted.empty()) {
+		iter_walk(w, -1, L, 0ull, c0, 0.0f, w.default_flags, 0u, true);
+	} else {
+		build_upper(plan, L, 0, sorted.size(), c0);
+		// values of the nodes above the bricks: ufo_b200_query's, one batch
+		const size_t nu = plan.nodes.size();
+		std::vector<unsigned long long> qc(nu);
+		std::vector<uint32_t> qd(nu), qrgb(nu, 0u);
+		upper_codes(plan, 0, L, 0ull, qc, qd);
+		w.occ.resize(nu);
+		w.flags.resize(nu);
+		unsigned long long* d_qcodes = b_qcodes.alloc<unsigned long long>(nu);
+		uint32_t* d_qdepths = b_qdepths.alloc<uint32_t>(nu);
+		float* d_qocc = b_qocc.alloc<float>(nu);
+		uint8_t* d_qflags = b_qflags.alloc<uint8_t>(nu);
+		uint32_t* d_qrgb = color ? b_qrgb.alloc<uint32_t>(nu) : nullptr;
+		CK(cudaMemcpyAsync(d_qcodes, qc.data(), 8 * nu, cudaMemcpyHostToDevice, s));
+		CK(cudaMemcpyAsync(d_qdepths, qd.data(), 4 * nu, cudaMemcpyHostToDevice, s));
+		k_query<<<(uint32_t)((nu + 255) / 256), 256, 0, s>>>(m->M, d_qcodes, d_qdepths, (uint32_t)nu, d_qocc, d_qflags, d_qrgb);
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(w.occ.data(), d_qocc, 4 * nu, cudaMemcpyDeviceToHost, s));
+		CK(cudaMemcpyAsync(w.flags.data(), d_qflags, nu, cudaMemcpyDeviceToHost, s));
+		if (color) CK(cudaMemcpyAsync(qrgb.data(), d_qrgb, 4 * nu, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		w.rgb = std::move(qrgb);
+		const UpNode& r = plan.nodes[0];
+		iter_walk(w, 0, L, 0ull, c0, r.has ? w.occ[0] : r.occ, w.flags[0], r.has ? w.rgb[0] : r.rgb, !r.has);
+	}
+	*n = (size_t)w.total;
+	if (codes && w.total && w.total <= cap) {
+		std::vector<IterRec> packed(w.packed);
+		if (w.packed) {
+			unsigned long long* d_offs = b_offs.alloc<unsigned long long>(nb);
+			IterRec* d_out = b_out.alloc<IterRec>(w.packed);
+			CK(cudaMemcpyAsync(d_offs, w.offs.data(), 8ull * nb, cudaMemcpyHostToDevice, s));
+			brick_iter(d_offs, d_out);
+			CK(cudaGetLastError());
+			CK(cudaMemcpyAsync(packed.data(), d_out, sizeof(IterRec) * w.packed, cudaMemcpyDeviceToHost, s));
+			CK(cudaStreamSynchronize(s));
+		}
+		size_t at = 0;
+		auto put = [&](const IterRec& r) {
+			codes[at] = r.code;
+			depths[at] = (uint8_t)((r.meta >> 24) & 31u);
+			logodds[at] = r.occ;
+			flags[at] = (uint8_t)(r.meta >> 29);
+			if (rgb) {
+				rgb[3 * at] = (uint8_t)r.meta;
+				rgb[3 * at + 1] = (uint8_t)(r.meta >> 8);
+				rgb[3 * at + 2] = (uint8_t)(r.meta >> 16);
+			}
+			++at;
+		};
+		for (const auto& p : w.pieces) {
+			if (p.second == kNone) {
+				put(p.first);
+			} else {
+				const IterRec* r = packed.data() + w.offs[p.second];
+				for (uint32_t i = 0; i < plan.info[p.second].size; ++i) put(r[i]);
+			}
+		}
+	}
 	return UFO_B200_OK;
 }
 }  // namespace
@@ -3792,60 +3704,50 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
 	// the codes of a tree of L levels use 3L bits; the pools must hold the bricks the stream creates
 	cudaStream_t s = m->stream;
 	const size_t n_small = plan.small.size(), n_bricks = plan.bricks.size(), n_wipe = plan.wipe.size();
+	DevBuf b_small, b_bricks, b_wipe;
 	ImportRec *d_small = nullptr, *d_bricks = nullptr, *d_wipe = nullptr;
-	auto cleanup = [&]() {
-		for (void* p : {(void*)d_small, (void*)d_bricks, (void*)d_wipe})
-			if (p) cudaFree(p);
-	};
-	try {
-		if (n_small) {
-			CK(cudaMalloc(&d_small, n_small * sizeof(ImportRec)));
-			CK(cudaMemcpyAsync(d_small, plan.small.data(), n_small * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
-		}
-		if (n_bricks) {
-			CK(cudaMalloc(&d_bricks, n_bricks * sizeof(ImportRec)));
-			CK(cudaMemcpyAsync(d_bricks, plan.bricks.data(), n_bricks * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
-		}
-		if (n_wipe) {
-			CK(cudaMalloc(&d_wipe, n_wipe * sizeof(ImportRec)));
-			CK(cudaMemcpyAsync(d_wipe, plan.wipe.data(), n_wipe * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
-		}
-		for (int attempt = 0;; ++attempt) {
-			M.scan_id++;
-			if (M.scan_id == 0) M.scan_id = 1;
-			M.up_epoch++;
-			M.dense = 0;
-			M.mask_base = M.miss_mask;
-			push_counters(m);
-			if (n_wipe && m->n_bricks)
-				k_import_wipe<<<(uint32_t)(((size_t)m->n_bricks * 64 + 255) / 256), 256, 0, s>>>(M, m->n_bricks, d_wipe, (uint32_t)n_wipe);
-			if (n_bricks) k_import_bricks<<<(uint32_t)std::min<size_t>(n_bricks, (size_t)m->sm_count * 16), 64, 0, s>>>(M, d_bricks, (uint32_t)n_bricks);
-			if (n_small) k_import_small<<<m->sm_count * 8, 256, 0, s>>>(M, d_small, (uint32_t)n_small);
-			k_import_refresh<<<m->sm_count * 8, 256, 0, s>>>(M);
-			if (M.color) k_brick_agg<true><<<m->sm_count * 4, 256, 0, s>>>(M);
-			else k_brick_agg<false><<<m->sm_count * 4, 256, 0, s>>>(M);
-			launch_upper(m);
-			CK(cudaGetLastError());
-			CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
-			CK(cudaStreamSynchronize(s));
-			const uint32_t ov = m->h_ctr->overflow;
-			if (!ov) break;
-			if (attempt > 16) {
-				m->set_error("readData: device pools keep overflowing");
-				cleanup();
-				return UFO_B200_E_NOMEM;
-			}
-			// writing leaves is idempotent: grow and run the whole import again
-			m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
-			grow_pools(m, ov & 6u, m->h_ctr->n_bricks, m->h_ctr->n_upper);
-		}
-		m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
-		m->n_upper = std::min(m->h_ctr->n_upper, M.up_cap);
-	} catch (...) {
-		cleanup();
-		throw;
+	if (n_small) {
+		d_small = b_small.alloc<ImportRec>(n_small);
+		CK(cudaMemcpyAsync(d_small, plan.small.data(), n_small * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
 	}
-	cleanup();
+	if (n_bricks) {
+		d_bricks = b_bricks.alloc<ImportRec>(n_bricks);
+		CK(cudaMemcpyAsync(d_bricks, plan.bricks.data(), n_bricks * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
+	}
+	if (n_wipe) {
+		d_wipe = b_wipe.alloc<ImportRec>(n_wipe);
+		CK(cudaMemcpyAsync(d_wipe, plan.wipe.data(), n_wipe * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
+	}
+	for (int attempt = 0;; ++attempt) {
+		M.scan_id++;
+		if (M.scan_id == 0) M.scan_id = 1;
+		M.up_epoch++;
+		M.dense = 0;
+		M.mask_base = M.miss_mask;
+		push_counters(m);
+		if (n_wipe && m->n_bricks)
+			k_import_wipe<<<(uint32_t)(((size_t)m->n_bricks * 64 + 255) / 256), 256, 0, s>>>(M, m->n_bricks, d_wipe, (uint32_t)n_wipe);
+		if (n_bricks) k_import_bricks<<<(uint32_t)std::min<size_t>(n_bricks, (size_t)m->sm_count * 16), 64, 0, s>>>(M, d_bricks, (uint32_t)n_bricks);
+		if (n_small) k_import_small<<<m->sm_count * 8, 256, 0, s>>>(M, d_small, (uint32_t)n_small);
+		k_import_refresh<<<m->sm_count * 8, 256, 0, s>>>(M);
+		if (M.color) k_brick_agg<true><<<m->sm_count * 4, 256, 0, s>>>(M);
+		else k_brick_agg<false><<<m->sm_count * 4, 256, 0, s>>>(M);
+		launch_upper(m);
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		const uint32_t ov = m->h_ctr->overflow;
+		if (!ov) break;
+		if (attempt > 16) {
+			m->set_error("readData: device pools keep overflowing");
+			return UFO_B200_E_NOMEM;
+		}
+		// writing leaves is idempotent: grow and run the whole import again
+		m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
+		grow_pools(m, ov & 6u, m->h_ctr->n_bricks, m->h_ctr->n_upper);
+	}
+	m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
+	m->n_upper = std::min(m->h_ctr->n_upper, M.up_cap);
 	return UFO_B200_OK;
 }
 }  // namespace
@@ -3934,32 +3836,27 @@ int do_write(Map* m, WriteArgs w, const std::vector<std::pair<const void*, size_
 	cudaStream_t s = m->stream;
 	size_t total = offs.size() * 8;
 	for (const auto& b : blobs) total += (b.second + 7) & ~size_t(7);
-	ensure_dev(m, m->d_w_in, m->w_in_cap, total);
+	ensure_spare(m, m->d_w_in, total, 1 << 12);
+	unsigned char* in = m->d_w_in.p;
 	size_t at = 0;
 	std::vector<const void*> ptrs;
 	for (const auto& b : blobs) {
-		if (b.second) CK(cudaMemcpyAsync(m->d_w_in + at, b.first, b.second, cudaMemcpyHostToDevice, s));
-		ptrs.push_back(m->d_w_in + at);
+		if (b.second) CK(cudaMemcpyAsync(in + at, b.first, b.second, cudaMemcpyHostToDevice, s));
+		ptrs.push_back(in + at);
 		at += (b.second + 7) & ~size_t(7);
 	}
-	CK(cudaMemcpyAsync(m->d_w_in + at, offs.data(), offs.size() * 8, cudaMemcpyHostToDevice, s));
+	CK(cudaMemcpyAsync(in + at, offs.data(), offs.size() * 8, cudaMemcpyHostToDevice, s));
 	bind(w, ptrs);
-	w.offs = reinterpret_cast<const unsigned long long*>(m->d_w_in + at);
+	w.offs = reinterpret_cast<const unsigned long long*>(in + at);
 	w.n_rec = n_rec;
 	if (n_rec > m->w_rec_cap) {
-		for (int i = 0; i < 2; ++i) {
-			if (m->d_w_keys[i]) CK(cudaFree(m->d_w_keys[i]));
-			if (m->d_w_idx[i]) CK(cudaFree(m->d_w_idx[i]));
-		}
-		if (m->d_w_recs) CK(cudaFree(m->d_w_recs));
-		m->device_bytes -= m->w_rec_cap * (2 * 8 + 2 * 4 + sizeof(WriteRec));
 		m->w_rec_cap = 0;
 		const size_t cap = std::max<size_t>(n_rec + n_rec / 8, 1 << 12);
 		for (int i = 0; i < 2; ++i) {
-			dev_alloc(m->d_w_keys[i], cap, 0, s, m->device_bytes);
-			dev_alloc(m->d_w_idx[i], cap, 0, s, m->device_bytes);
+			m->d_w_keys[i].ensure(m, cap * sizeof(unsigned long long), 0);
+			m->d_w_idx[i].ensure(m, cap * sizeof(uint32_t), 0);
 		}
-		dev_alloc(m->d_w_recs, cap, 0, s, m->device_bytes);
+		m->d_w_recs.ensure(m, cap * sizeof(WriteRec), 0);
 		m->w_rec_cap = cap;
 	}
 	PendingScan& p = m->pending;
@@ -4150,24 +4047,7 @@ int ufo_b200_insert_rays(ufo_b200_map* m, const double* origins, const double* e
 // ---------------------------------------------------------------------------
 namespace
 {
-// device / pinned buffers and events of one call
-struct DevBuf {
-	void* p = nullptr;
-	DevBuf() = default;
-	DevBuf(const DevBuf&) = delete;
-	DevBuf& operator=(const DevBuf&) = delete;
-	~DevBuf()
-	{
-		if (p) cudaFree(p);
-	}
-	template <class T>
-	T* alloc(size_t n)
-	{
-		CK(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)));
-		return static_cast<T*>(p);
-	}
-};
-
+// the events of one call
 struct Events {
 	cudaEvent_t e[4] = {};
 	Events()
@@ -4189,13 +4069,14 @@ struct Events {
 constexpr size_t kPageChunk = 16u << 20;
 struct PageStage {
 	uint8_t* pin[2] = {};
+	DevBuf dev_buf[2];
 	uint8_t* dev[2] = {};
 	cudaEvent_t ev[2] = {};
 	PageStage()
 	{
 		for (int b = 0; b < 2; ++b) {
 			CK(cudaHostAlloc(reinterpret_cast<void**>(&pin[b]), kPageChunk, cudaHostAllocDefault));
-			CK(cudaMalloc(reinterpret_cast<void**>(&dev[b]), kPageChunk));
+			dev[b] = dev_buf[b].alloc<uint8_t>(kPageChunk);
 			CK(cudaEventCreateWithFlags(&ev[b], cudaEventDisableTiming));
 		}
 	}
@@ -4205,7 +4086,6 @@ struct PageStage {
 	{
 		for (int b = 0; b < 2; ++b) {
 			if (pin[b]) cudaFreeHost(pin[b]);
-			if (dev[b]) cudaFree(dev[b]);
 			if (ev[b]) cudaEventDestroy(ev[b]);
 		}
 	}
@@ -4258,26 +4138,6 @@ void page_section_in(cudaStream_t s, PageStage& st, size_t n, size_t brick_bytes
 		CK(cudaGetLastError());
 	}
 	CK(cudaStreamSynchronize(s));
-}
-
-// moves `n` whole bricks of `brick_bytes` each (k_page_move) with the widest word that divides a brick
-template <bool SCATTER>
-void launch_page_move(Map* m, void* dst, const void* src, const uint32_t* slot, size_t n, size_t brick_bytes)
-{
-	if (!n) return;
-	auto run = [&](auto* d, size_t word) {
-		using V = std::remove_pointer_t<decltype(d)>;
-		const size_t per = brick_bytes / word;
-		uint32_t lg = 0;
-		while (((size_t)1 << lg) < per) ++lg;
-		const size_t units = n * per;
-		const uint32_t grid = (uint32_t)std::min<size_t>((units + 255) / 256, (size_t)m->sm_count * 32);
-		k_page_move<V, SCATTER><<<grid, 256, 0, m->stream>>>(d, static_cast<const V*>(src), slot, units, lg);
-	};
-	if (brick_bytes % 16 == 0) run(static_cast<uint4*>(dst), 16);
-	else if (brick_bytes % 8 == 0) run(static_cast<uint2*>(dst), 8);
-	else run(static_cast<uint32_t*>(dst), 4);
-	++m->launches;
 }
 
 // checks shared by retain, page-out and page-in; they need no device
@@ -4400,75 +4260,30 @@ int retain(Map* m, const Volume& vol, ufo_b200_retain_stats* out)
 	initial_caps(m->params, cap0, up0);
 	const uint32_t oc = M.brick_cap;
 	const uint32_t nc = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(cap0, 2ull * kept), 0x3ffffffull);
-	size_t& tot = m->device_bytes;
-	// One array at a time: allocate the new one, gather the survivors, free the old one.  `per`:
-	// elements per brick; the slots past the survivors get the array's initial fill.
-	auto compact = [&](auto*& p, size_t per, int fill) {
-		using T = std::remove_reference_t<decltype(*p)>;
-		if (!p) return;
-		T* q = nullptr;
-		CK(cudaMalloc(reinterpret_cast<void**>(&q), (size_t)nc * per * sizeof(T)));
-		launch_page_move<false>(m, q, p, d_src, kept, per * sizeof(T));
-		CK(cudaMemsetAsync(q + (size_t)kept * per, fill, (size_t)(nc - kept) * per * sizeof(T), s));
-		CK(cudaStreamSynchronize(s));
-		CK(cudaFree(p));
-		p = q;
-		tot = tot - (size_t)oc * per * sizeof(T) + (size_t)nc * per * sizeof(T);
-	};
-	// per-scan lists and everything above the bricks start from their initial state
-	auto renew = [&](auto*& p, size_t n_new, size_t n_old, int fill) {
-		using T = std::remove_reference_t<decltype(*p)>;
-		if (!p) return;
-		CK(cudaFree(p));
-		tot -= n_old * sizeof(T);
-		dev_alloc(p, n_new, fill, s, tot);
+	// One array at a time (each_array's order): allocate the new one, gather the survivors, free the
+	// old one.  A failure before the first array is replaced leaves the map as it was.
+	bool changed = false;
+	auto each = [&](Pool pool, Retain retain, uint32_t old_cap, uint32_t new_cap, uint32_t keep) {
+		each_array(m, pool, [&](const PoolArray& a) {
+			if (a.retain != retain) return;
+			reshape(m, a, old_cap, new_cap, keep, d_src);
+			changed = true;
+		});
 	};
 	CK(cudaEventRecord(ev.e[1], s));
-	// The leaves first: they are most of the map, so if the device cannot hold one more array this
-	// fails before anything has changed.  Every later array is smaller than what has been freed.
-	compact(M.leaf, 64 * 64, 0);
 	try {
-		compact(M.leaf_rgb, 64 * 64, 0);
-		compact(M.miss_mask, 64, 0);
-		compact(M.hit_mask, 64, 0);
-		compact(M.chg_mask, 64, 0);
-		compact(m->chg_paused, 64, 0);
-		compact(M.meta, 64, 0);
-		compact(M.pair_max, 64, 0);
-		compact(M.sum1_rgb, 64 * 8, 0);
-		compact(M.rgb2, 64, 0);
-		compact(M.alias_miss, 64, 0);
-		compact(M.alias_hit, 64, 0);
-		compact(M.brick_key, 1, 0);
-		compact(M.brick_stamp, 1, 0);
-		compact(M.hit_stamp, 1, 0);
-		compact(M.brick_sum3, 8, 0);
-		compact(M.brick_sum4, 1, 0);
-		compact(M.brick_rgb3, 8, 0);
-		compact(M.brick_rgb4, 1, 0);
+		each(Pool::Brick, Retain::Compact, oc, nc, kept);
 		CK(cudaEventRecord(ev.e[2], s));
-		renew(M.touched, nc, oc, 0);
-		renew(M.touched_alt, nc, oc, 0);
-		renew(M.touched_mi, nc, oc, 0);
-		renew(M.touched_alt_mi, nc, oc, 0);
-		renew(M.brick_parent, nc, oc, 0xff);
+		// per-scan lists and everything above the bricks start from their initial state
+		each(Pool::Brick, Retain::Renew, oc, nc, 0);
 		M.brick_cap = nc;
-		renew(M.bh_tab, (size_t)std::max(kMinHash, next_pow2(2ull * nc)), (size_t)M.bh_mask + 1, 0xff);
-		M.bh_mask = std::max(kMinHash, next_pow2(2ull * nc)) - 1;
-		if (kept) {
-			k_rebuild_brick_hash<<<(kept + 255) / 256, 256, 0, s>>>(M, kept);
-			++m->launches;
-		}
+		brick_hash(m, kept);
 		// the upper-node pool, in proportion, rebuilt from the survivors' depth-4 aggregates: a child
 		// that never reports counts as never-touched space, which is what a removed brick now is
-		const size_t ou = M.up_cap, ouh = (size_t)M.uh_mask + 1;
-		for (void* p : {(void*)M.uh_keys, (void*)M.uh_vals, (void*)M.up_key, (void*)M.up_agg, (void*)M.up_stamp, (void*)M.up_child,
-		                (void*)M.up_valid, (void*)M.up_parent, (void*)m->d_list[0], (void*)m->d_list[1], (void*)M.up_rgb,
-		                (void*)M.up_child_rgb})
-			if (p) CK(cudaFree(p));
-		tot -= ouh * 12 + ou * (8 + sizeof(Agg) + 4 + 8 * sizeof(Agg) + 4 + 4 + 4 + 4) + (M.color ? ou * (4 + 8 * 4) : 0);
-		M.up_rgb = M.up_child_rgb = nullptr;
-		alloc_upper(m, std::max(up0, nc / 2));
+		const uint32_t ou = M.up_cap, nu = std::max(up0, nc / 2);
+		each(Pool::Upper, Retain::Renew, ou, nu, 0);
+		M.up_cap = nu;
+		upper_hash(m, 0);
 		m->n_bricks = kept;
 		m->n_upper = 0;
 		page_propagate(m, nullptr, kept, false);
@@ -4483,6 +4298,7 @@ int retain(Map* m, const Volume& vol, ufo_b200_retain_stats* out)
 		CK(cudaStreamSynchronize(s));
 		m->n_blocks = (uint32_t)blocks;
 	} catch (...) {
+		if (!changed) throw;
 		// the arrays no longer agree on their slots
 		m->poisoned = true;
 		m->set_error("retain failed after the leaves were compacted; the map is unusable");
