@@ -426,7 +426,7 @@ typedef struct {
 	uint64_t regrows;         /* pool growth events during this insert     */
 	uint64_t launches;        /* kernels launched by this insert           */
 	uint64_t result_bytes;    /* bytes of per-scan counters copied device -> host by this insert */
-	uint64_t touched_lines;   /* 128-byte lines of leaf data holding a touched octet (HBM moves whole lines) */
+	uint64_t touched_lines;   /* 128-byte lines of leaf data the update read (HBM moves whole lines): lines holding a touched octet, less those whose touched octets all sit in saturated pairs (ufo_b200_last_update_stats) */
 	float ms_total;           /* CUDA-event time of the whole insert (device work) */
 	float ms_h2d;
 	float ms_points;          /* K1: discretise + hit marking              */
@@ -453,6 +453,18 @@ typedef struct {
 	uint64_t dirty_reductions; /* reductions on the bitmap of touched bricks */
 } ufo_b200_walk_stats;
 int ufo_b200_last_walk_stats(ufo_b200_map* m, ufo_b200_walk_stats* out);
+
+/* What the leaf update of the most recent insert left out (waits for it to finish).  Counted at
+ * profiling level 2 only; all zero otherwise, and always zero on colour maps, which read and write
+ * every touched pair.  A saturated pair is a pair of initialised octets
+ * (a 64 B half line) that the scan only marked free and whose 16 voxels already sit at
+ * clamping_thres_min: the update would not change it, so it is neither read nor written. */
+typedef struct {
+	uint64_t saturated_octets; /* touched octets in saturated pairs (part of touched_octets)          */
+	uint64_t saturated_lines;  /* 128 B leaf lines with touched voxels that were not read because of them */
+	uint64_t clean_sectors;    /* 32 B leaf sectors read and updated but left unchanged: not written back */
+} ufo_b200_update_stats;
+int ufo_b200_last_update_stats(ufo_b200_map* m, ufo_b200_update_stats* out);
 
 /* Early stopping.  On the CPU, early_stopping = E > 0 makes a scan cheaper: a ray stops after E
  * nodes in a row that earlier rays (or its own earlier samples) already put into the scan's free

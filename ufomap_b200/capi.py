@@ -55,6 +55,13 @@ class WalkStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class UpdateStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("saturated_octets", "saturated_lines", "clean_sectors")]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 class EarlyStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in (
         "rounds", "converged", "visits", "nodes", "free_nodes", "table_bytes", "id_bytes")] + [
@@ -117,7 +124,7 @@ SYMBOLS = [
     "ufo_b200_set_early_stopping", "ufo_b200_last_early_stats",
     "ufo_b200_iterate", "ufo_b200_update_nodes_color",
     "ufo_b200_retain_bv", "ufo_b200_retain", "ufo_b200_page_out_bv", "ufo_b200_page_in", "ufo_b200_page_info",
-    "ufo_b200_pool_stats",
+    "ufo_b200_pool_stats", "ufo_b200_last_update_stats",
 ]
 
 # ufo_b200_volume: one shape of a bounding volume (type in BoundingVar order, members in v)
@@ -283,6 +290,7 @@ def load():
     lib.ufo_b200_last_scan_stats.argtypes = [vp, C.POINTER(ScanStats)]
     lib.ufo_b200_completed_scan_stats.argtypes = [vp, C.POINTER(ScanStats)]
     lib.ufo_b200_last_walk_stats.argtypes = [vp, C.POINTER(WalkStats)]
+    lib.ufo_b200_last_update_stats.argtypes = [vp, C.POINTER(UpdateStats)]
     lib.ufo_b200_set_sensor_model_field.argtypes = [vp, i32, dbl]
     lib.ufo_b200_set_profiling.argtypes = [vp, i32]
     lib.ufo_b200_write_compressed.argtypes = [vp, vp, u32, i32, i32, i32, vp, sz, C.POINTER(sz), C.POINTER(sz)]
@@ -475,6 +483,13 @@ class Map:
         records pushed, mask reductions issued, words they found empty, dirty-bit reductions."""
         st = WalkStats()
         self._check(self.lib.ufo_b200_last_walk_stats(self.h, C.byref(st)))
+        return st.as_dict()
+
+    def update_stats(self):
+        """What the leaf update of the last insert left out (profiling level 2): touched octets of
+        saturated pairs, leaf lines not read because of them, sectors not written back."""
+        st = UpdateStats()
+        self._check(self.lib.ufo_b200_last_update_stats(self.h, C.byref(st)))
         return st.as_dict()
 
     def set_early_stopping(self, exact):

@@ -75,8 +75,15 @@ struct Counters {
 	unsigned long long e_visits, e_nodes, e_free;
 	uint32_t e_rounds, e_converged, e_low[2];
 	// k_update statistics spread over slots: [slot][0 voxels, 1 hit voxels, 2 octets, 3 blocks,
-	// 4 first-touched blocks, 5 bricks, 6 depth-3 nodes, 7 touched 128 B leaf lines]
+	// 4 first-touched blocks, 5 bricks, 6 depth-3 nodes, 7 128 B leaf lines read]
 	unsigned long long stat[64][8];
+};
+
+// k_update_brick at profiling level 2 only, in an allocation of its own (not part of the per-scan
+// copies of Counters), same slots as Counters::stat: [slot][0 touched octets of saturated pairs,
+// 1 leaf lines not read because of them, 2 leaf sectors not written back]
+struct K3Stats {
+	unsigned long long slot[64][3];
 };
 
 // Routed multi-GPU mode (SURVEY.md 8(e) variant 2): every rank walks ITS rays into its own map,
@@ -113,6 +120,10 @@ struct DeviceMap {
 	float free_ceil, occ_floor;  // float thresholds equivalent to the double compares (see leaf_flags)
 	double prob_hit;         // toProb(float(hit)) used by the colour blend
 	uint32_t default_flags;  // flags of a never-touched voxel / subtree (value 0.0)
+	// no leaf value of the map lies below clamp_min, and clamp_min is nonzero and <= clamp_max: a scan
+	// may leave saturated pairs alone (see apply_update)
+	uint32_t sat_skip;
+	K3Stats* k3_stat;  // profiling level 2: k_update_brick counts into it (nullptr: not counted)
 	uint32_t color;
 	uint32_t scan_id;
 	// spatial sharding over several GPUs: this map only keeps the bricks it owns
@@ -460,7 +471,16 @@ __device__ __forceinline__ uint32_t block_flags(const DeviceMap& M, uint32_t mt)
 	return f;
 }
 
-// float add + float clamp (occupancy_map_base.h:1139-1145)
+// float add + float clamp (occupancy_map_base.h:1139-1145).
+// Saturated pairs.  Let c = clamp_min be nonzero with c <= clamp_max, and let no leaf of the map lie
+// below c (DeviceMap::sat_skip; the voxels of an initialised octet that no update has reached hold
+// 0.0, so this needs c < 0).  If both octets of a pair are initialised and the pair maximum is c
+// bit for bit, every one of its 16 leaves is >= c and <= c, so it equals c, and being nonzero it has
+// c's bits.  For a miss u <= 0 (and not NaN), v + u <= c, so fmaxf(v + u, c) = c and fminf(c,
+// clamp_max) = c: every marked voxel keeps its bits, the reference's updateOccupancy reports no
+// change, and leaves, octet flags, pair maximum, colours, change mask and every aggregate above stay
+// as they are.  c = 0 is left out because -0.0 and +0.0 compare equal but differ in their bits.  Hits
+// are applied before misses and can raise a voxel, so a pair with a hit bit is updated as usual.
 __device__ __forceinline__ float apply_update(const DeviceMap& M, float v, float u)
 {
 	return fminf(fmaxf(__fadd_rn(v, u), M.clamp_min), M.clamp_max);

@@ -142,6 +142,8 @@ struct ufo_b200_map {
 	// owners of the device memory DeviceMap sees outside the pool arrays: counters, the hashes of the
 	// two pools and the dense scan volume (setup_volume)
 	DevMem<Counters> ctr;
+	DevMem<K3Stats> k3_stat;  // profiling level 2, allocated on first use
+	bool k3_counted = false;  // this scan's k_update_brick counts into k3_stat
 	DevMem<ulonglong2> bh_tab;
 	DevMem<unsigned long long> uh_keys;
 	DevMem<uint32_t> uh_vals;
@@ -209,6 +211,11 @@ struct ufo_b200_map {
 	ufo_b200_scan_stats stats{};       // scan in flight / last scan
 	ufo_b200_scan_stats done_stats{};  // last scan whose counters are folded into the host view
 	ufo_b200_walk_stats walk_stats{};  // last scan, profiling level 2
+	ufo_b200_update_stats update_stats{};  // last scan, profiling level 2
+	// a lower bound of every leaf value the map holds: 0.0 (the voxels of an initialised octet that no
+	// update has reached yet) and the lowest clamp_min any update could have clamped to; -inf once
+	// values came in unclamped (readData, page_in).  Sets DeviceMap::sat_skip
+	float value_floor = 0.0f;
 	bool stats_pending = false;
 	PendingScan pending;
 	bool poisoned = false;
@@ -245,6 +252,16 @@ namespace
 {
 using Map = ufo_b200_map;
 
+// Scans may skip saturated pairs (apply_update) while no leaf lies below clamp_min: the floor only
+// falls (a lowered clamp_min, unclamped values), so once clamp_min is raised above it the skip stays
+// off until the map is cleared.  The floor is at most 0.0, so a positive clamp_min never skips.
+void set_value_floor(Map* m, float floor)
+{
+	DeviceMap& M = m->M;
+	m->value_floor = floor;
+	M.sat_skip = (floor >= M.clamp_min && M.clamp_min != 0.0f && M.clamp_min <= M.clamp_max) ? 1u : 0u;
+}
+
 void refresh_model(Map* m)
 {
 	DeviceMap& M = m->M;
@@ -267,6 +284,7 @@ void refresh_model(Map* m)
 	uint32_t f = (m->free_thr_log > 0.0) ? 1u : 0u;
 	if (m->free_thr_log <= 0.0 && m->occ_thr_log >= 0.0) f |= 2u;
 	M.default_flags = f;
+	set_value_floor(m, fminf(m->value_floor, M.clamp_min));
 }
 
 void reset_bbox(Map* m)
@@ -523,6 +541,7 @@ void push_counters(Map* m)
 	}
 	*m->h_ctr = c;
 	CK(cudaMemcpyAsync(m->M.ctr, m->h_ctr, sizeof(Counters), cudaMemcpyHostToDevice, m->stream));
+	m->k3_counted = false;
 }
 
 // grow whichever pool overflowed; `want_*` are the allocation counters the failed
@@ -608,6 +627,16 @@ void finish_stats(Map* m)
 	st.rays = c.n_rays;
 	st.visits = c.visits;
 	m->walk_stats = ufo_b200_walk_stats{c.walk_records, c.walk_mask_reds, c.walk_words, c.walk_dirty_reds};
+	m->update_stats = ufo_b200_update_stats{};
+	if (m->k3_counted) {
+		K3Stats h;
+		if (cudaMemcpy(&h, m->k3_stat.p, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess) {
+			unsigned long long k3[3] = {0, 0, 0};
+			for (int sl = 0; sl < kStatSlots; ++sl)
+				for (int k = 0; k < 3; ++k) k3[k] += h.slot[sl][k];
+			m->update_stats = ufo_b200_update_stats{k3[0], k3[1], k3[2]};
+		}
+	}
 	m->early_stats = ufo_b200_early_stats{};
 	if (m->early_pass) {
 		ufo_b200_early_stats& es = m->early_stats;
@@ -678,6 +707,13 @@ void ensure_seg(Map* m, unsigned long long want)
 void launch_update(Map* m, float miss, bool set_mode = false)
 {
 	CK(cudaMemsetAsync(&m->M.ctr->k3_cursor, 0, sizeof(uint32_t), m->stream));
+	m->M.k3_stat = nullptr;
+	if (m->profiling >= 2) {
+		m->k3_stat.ensure(m, sizeof(K3Stats), 0);
+		if (!m->k3_counted) CK(cudaMemsetAsync(m->k3_stat.p, 0, sizeof(K3Stats), m->stream));
+		m->k3_counted = true;
+		m->M.k3_stat = m->k3_stat.p;
+	}
 	if (m->M.color) {
 		const uint32_t per_sm = UbShape<true>::kMinBlocks, T = UbShape<true>::kWarps * 32;
 		const uint32_t grid = (uint32_t)m->sm_count * (m->k3_blocks ? std::min<uint32_t>(per_sm, (uint32_t)m->k3_blocks) : per_sm);
@@ -2758,6 +2794,16 @@ int ufo_b200_last_walk_stats(ufo_b200_map* m, ufo_b200_walk_stats* out)
 	});
 }
 
+int ufo_b200_last_update_stats(ufo_b200_map* m, ufo_b200_update_stats* out)
+{
+	if (!m || !out) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() {
+		sync_map(m);
+		*out = m->update_stats;
+		return (int)UFO_B200_OK;
+	});
+}
+
 int ufo_b200_completed_scan_stats(ufo_b200_map* m, ufo_b200_scan_stats* out)
 {
 	if (!m || !out) return UFO_B200_E_INVALID;
@@ -2850,6 +2896,7 @@ int ufo_b200_clear(ufo_b200_map* m)
 		m->poisoned = false;
 		m->route_stage = 0;
 		reset_bbox(m);
+		set_value_floor(m, fminf(0.0f, M.clamp_min));  // no leaf left
 		CK(cudaStreamSynchronize(s));
 		return (int)UFO_B200_OK;
 	});
@@ -3718,6 +3765,7 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
 		d_wipe = b_wipe.alloc<ImportRec>(n_wipe);
 		CK(cudaMemcpyAsync(d_wipe, plan.wipe.data(), n_wipe * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
 	}
+	set_value_floor(m, -INFINITY);  // the stream's values are not clamped to this map's sensor model
 	for (int attempt = 0;; ++attempt) {
 		M.scan_id++;
 		if (M.scan_id == 0) M.scan_id = 1;
@@ -4430,6 +4478,7 @@ int page_in(Map* m, const void* blob, size_t size, ufo_b200_retain_stats* out)
 		if (out) *out = st;
 		return UFO_B200_OK;
 	}
+	set_value_floor(m, -INFINITY);  // the blob may come from a map with another sensor model
 	const uint8_t* p_keys = static_cast<const uint8_t*>(blob) + sizeof(PageHeader);
 	const uint8_t* p_leaf = p_keys + (size_t)n * 8;
 	const uint8_t* p_bits = p_leaf + (size_t)n * kPageLeafBytes;

@@ -41,10 +41,15 @@ __device__ __forceinline__ unsigned long long octet_unbits8(uint32_t c8, uint32_
 	return s << base;
 }
 
-template <bool SET = false>
-__device__ __forceinline__ void update_octet(const DeviceMap& M, float miss, float* lp, uint32_t m8,
+// CLEAN: a scan update writes the octet's 32 B sector back only when one of its voxels changed (bit
+// for bit), so that an unchanged sector leaves no dirty line in the L2; an uninitialised octet
+// (`init` false, its leaves read as 0.0 without a load) is always written.  Returns true when the
+// store was skipped.  SET always writes, and so do colour maps (K3 leaves their colour path as it was).
+template <bool SET = false, bool CLEAN = false>
+__device__ __forceinline__ bool update_octet(const DeviceMap& M, float miss, float* lp, uint32_t m8,
                                              uint32_t h8, float4 a0, float4 a1, float& omax,
-                                             uint32_t& oflags, size_t blk = 0, uint32_t oct = 0)
+                                             uint32_t& oflags, size_t blk = 0, uint32_t oct = 0,
+                                             bool init = false)
 {
 	float v[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
 	const float v0[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
@@ -70,14 +75,16 @@ __device__ __forceinline__ void update_octet(const DeviceMap& M, float miss, flo
 	}
 	// contains_free = any voxel below the free threshold, contains_unknown = any in between
 	oflags = (omin < M.free_ceil ? 1u : 0u) | (unk ? 2u : 0u);
-	if (!SET && M.chg_mask) {
+	if (!SET && (CLEAN || M.chg_mask)) {
 		uint32_t c8 = 0;
 #pragma unroll
 		for (int j = 0; j < 8; ++j) c8 |= (__float_as_uint(v[j]) != __float_as_uint(v0[j]) ? 1u : 0u) << j;
-		if (c8) atomicOr(&M.chg_mask[blk], octet_unbits8(c8, oct));
+		if (c8 && M.chg_mask) atomicOr(&M.chg_mask[blk], octet_unbits8(c8, oct));
+		if (CLEAN && !c8 && init) return true;
 	}
 	reinterpret_cast<float4*>(lp)[0] = make_float4(v[0], v[1], v[2], v[3]);
 	reinterpret_cast<float4*>(lp)[1] = make_float4(v[4], v[5], v[6], v[7]);
+	return false;
 }
 
 // ---- mbarrier + 1-D bulk copy (TMA engine, cp.async.bulk) -------------------------------
@@ -277,23 +284,48 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 	__syncwarp();
 
 	unsigned int s_vox = 0, s_hit = 0, s_oct = 0, s_blk = 0, s_new = 0, s_lin = 0;
+	// saturated pairs (see apply_update): a miss-only pair whose 16 voxels all sit at clamp_min is
+	// left as it is, so it is neither loaded nor written.  Exact only when the map holds no value below
+	// clamp_min (M.sat_skip, kept by the host) and the marks land in the tree (fold).  Mono maps only:
+	// on colour maps (config #3) the skip's extra code cost more K3 time than the lines it saved, so
+	// the colour kernel still reads every touched pair
+	const bool sat = !COLOR && !SET && fold && M.sat_skip && miss <= 0.0f;
 
-	// lane = block lane of either half: touched octets (t8) of the brick in `slab` and the octets to
-	// load (touched, and initialised partners of touched ones), list by warp prefix sums
+	// lane = block lane of either half: touched octets of the brick in `slab` and the octets to load
+	// (touched, and initialised partners of touched ones), list by warp prefix sums.  t8 = the touched
+	// octets that are loaded | the touched octets of saturated pairs << 8 (not loaded)
 	auto build_list = [&](const WarpSlab& slab, uint16_t* list, uint32_t (&t8)[2], uint32_t (&excl)[2], uint32_t& total) {
 		total = 0;
 #pragma unroll
 		for (uint32_t h = 0; h < 2; ++h) {
 			const uint32_t blk = h * 32 + lane;
-			const unsigned long long u = slab.mm[blk] | slab.hm[blk];
-			uint32_t t = 0, ld = 0, init = 0;
+			const unsigned long long hm = slab.hm[blk], u = slab.mm[blk] | hm;
+			uint32_t t = 0, ld = 0, init = 0, sk = 0;
 			if (u) {
 #pragma unroll
 				for (uint32_t o = 0; o < 8; ++o) {
 					const uint32_t base = ((o & 1u) << 1) | ((o & 2u) << 2) | ((o & 4u) << 3);
 					t |= (((u >> base) & 0x330033ull) ? 1u : 0u) << o;
 				}
+				if (!COLOR) {  // colour maps skip nothing and count in the leaf loop
+					s_vox += __popcll(u);
+					s_hit += __popcll(hm);
+					s_oct += __popc(t);
+				}
 				init = (slab.meta[blk] >> 16) & 0xffu;
+				if (sat) {
+					const float4 q = slab.q[blk];
+					const float qk[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+					for (uint32_t k = 0; k < 4; ++k) {
+						// pair k = octets 2k, 2k+1: x 0..3, y and z from the bits of k (linear mask order)
+						const unsigned long long pm = 0x00ff00ffull << (8 * (k & 1u) + 32 * (k >> 1));
+						const bool s = ((init >> (2 * k)) & 3u) == 3u && !(hm & pm) &&
+						               __float_as_uint(qk[k]) == __float_as_uint(M.clamp_min);
+						sk |= s ? t & (3u << (2 * k)) : 0u;
+					}
+					t &= ~sk;
+				}
 				ld = t | (COLOR ? 0u : (((t & 0x55u) << 1) | ((t & 0xaau) >> 1)) & init);
 				// out-of-tree hits (k_alias_apply, before this kernel) may have written an octet whose
 				// initialised bit is still clear: touched octets are then loaded all the same
@@ -306,7 +338,7 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				if (lane >= (uint32_t)o) incl += v;
 			}
 			excl[h] = total + incl - __popc(ld);
-			t8[h] = t;
+			t8[h] = t | (sk << 8);
 			{
 				uint32_t bits = ld, at = excl[h];
 				while (bits) {
@@ -345,8 +377,8 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 #pragma unroll
 			for (uint32_t h = 0; h < 2; ++h) {
 				const uint32_t blk = h * 32 + lane;
-				if (t8[h]) {
-					if (t8[h] != 0xffu) {
+				if (t8[h]) {  // a marked block; its octets that are not loaded keep their old colour
+					if ((t8[h] & 0xffu) != 0xffu) {
 						cp_async16(&S.c1lo[COLOR ? blk : 0], M.sum1_rgb + (b0 + blk) * 8);
 						cp_async16(&S.c1hi[COLOR ? blk : 0], M.sum1_rgb + (b0 + blk) * 8 + 4);
 					}
@@ -400,22 +432,24 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				const uint32_t m8 = octet_bits8(slab.mm[t], o), h8 = octet_bits8(slab.hm[t], o);
 				float omax;
 				uint32_t ofl;
-				update_octet<SET>(M, miss, M.leaf + (b0 + t) * 64 + 8 * o, m8, h8, a0[f], a1[f], omax, ofl, b0 + t, o);
+				const bool clean = update_octet<SET, !COLOR>(M, miss, M.leaf + (b0 + t) * 64 + 8 * o, m8, h8, a0[f], a1[f], omax, ofl,
+				                                     b0 + t, o, (en[f] & kEntInit) != 0u);
 				if (COLOR && (en[f] & kEntPartner)) {
 					const float4 p = p0[COLOR ? f : 0], q = p1[COLOR ? f : 0];
 					omax = fmaxf(omax, fmaxf(fmaxf(fmaxf(p.x, p.y), fmaxf(p.z, p.w)), fmaxf(fmaxf(q.x, q.y), fmaxf(q.z, q.w))));
 				}
 				if (COLOR && (en[f] & kEntPartnerZero)) omax = fmaxf(omax, 0.0f);
 				S.omax[idx] = omax;
-				S.list[st][idx] = (uint16_t)ofl;  // the entry has been consumed: the slot carries the flags back
+				// the entry has been consumed: the slot carries the flags back (bit 2: not written back)
+				S.list[st][idx] = (uint16_t)(ofl | (clean ? 4u : 0u));
 				if (COLOR) {
 					const uint4 c0 = x0[COLOR ? f : 0], c1 = x1[COLOR ? f : 0];
 					const uint32_t cc[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
 					S.orgb[COLOR ? idx : 0] = rms_rgb(cc, 8);
+					s_vox += __popc(m8 | h8);
+					s_hit += __popc(h8);
+					s_oct += 1;
 				}
-				s_vox += __popc(m8 | h8);
-				s_hit += __popc(h8);
-				s_oct += 1;
 			}
 		}
 		if (has_next) {
@@ -442,6 +476,7 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 		// block lanes: pair maxima, meta, mask clearing
 		float agg_occ[2];
 		uint32_t agg_fl[2], agg_rgb[2];
+		uint32_t n_clean = 0;  // profiling level 2: this lane's sectors that were not written back
 #pragma unroll
 		for (uint32_t h = 0; h < 2; ++h) {
 			const uint32_t blk = h * 32 + lane;
@@ -452,15 +487,17 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			float my_occ = 0.0f;
 			uint32_t my_fl = M.default_flags, my_rgb = 0;
 			if (marked) {
+				// t: the touched octets that were loaded.  An octet of a saturated pair (t8 bits 8..15) is
+				// treated like an untouched initialised one: flags from meta, old colour, old pair max
+				const uint32_t t = t8[h] & 0xffu, init = (mt >> 16) & 0xffu;
 				uint4 q0 = make_uint4(0u, 0u, 0u, 0u), q1 = q0;
-				if (COLOR && t8[h] != 0xffu) {
+				if (COLOR && t != 0xffu) {
 					q0 = S.c1lo[COLOR ? blk : 0];
 					q1 = S.c1hi[COLOR ? blk : 0];
 				}
 				const uint32_t oldc[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
 				const float4 oq = slab.q[blk];
 				const float oldq[4] = {oq.x, oq.y, oq.z, oq.w};
-				const uint32_t t = t8[h], init = (mt >> 16) & 0xffu;
 				const uint32_t ld = t | (COLOR ? 0u : (((t & 0x55u) << 1) | ((t & 0xaau) >> 1)) & init);
 				float om[8], nq[4];
 				uint32_t newc[8];
@@ -475,6 +512,10 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 						om[o] = S.omax[at];
 						if ((t >> o) & 1u) {
 							fl = S.list[st][at];
+							if (!COLOR) {  // colour maps write every sector back
+								n_clean += fl >> 2;
+								fl &= 3u;
+							}
 							if (COLOR) oc = S.orgb[COLOR ? at : 0];
 						}
 						++at;
@@ -503,7 +544,7 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				M.mask_base[(size_t)mi * 64 + blk] = 0ull;  // masks cleared for the next scan
 				if (hm) M.hit_mask[b] = 0ull;
 				s_blk += 1;
-				s_lin += ((t8[h] & 0x0fu) ? 1u : 0u) + ((t8[h] & 0xf0u) ? 1u : 0u);
+				s_lin += ((t & 0x0fu) ? 1u : 0u) + ((t & 0xf0u) ? 1u : 0u);  // leaf lines read
 				s_new += (mt & 0xff0000u) ? 0u : 1u;
 				my_occ = bmax;
 				my_fl = bfl | 0x100u;
@@ -571,6 +612,26 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				unsigned long long* slot = M.ctr->stat[brick % kStatSlots];
 				atomicAdd(&slot[5], 1ull);
 				atomicAdd(&slot[6], (unsigned long long)(__popc(ub0) + __popc(ub1)));
+			}
+		}
+		if (!COLOR && M.k3_stat) {
+			// profiling level 2: octets of saturated pairs, leaf lines that were not read because of
+			// them, sectors not written back
+			uint32_t n_sat = 0, n_lin = 0;
+#pragma unroll
+			for (uint32_t h = 0; h < 2; ++h) {
+				const uint32_t t = t8[h] & 0xffu, sk = t8[h] >> 8;
+				n_sat += __popc(sk);
+				n_lin += ((sk & 0x0fu) && !(t & 0x0fu) ? 1u : 0u) + ((sk & 0xf0u) && !(t & 0xf0u) ? 1u : 0u);
+			}
+			n_sat = __reduce_add_sync(FULL, n_sat);
+			n_lin = __reduce_add_sync(FULL, n_lin);
+			n_clean = __reduce_add_sync(FULL, n_clean);
+			if (lane == 0) {
+				unsigned long long* slot = M.k3_stat->slot[brick % kStatSlots];
+				if (n_sat) atomicAdd(&slot[0], (unsigned long long)n_sat);
+				if (n_lin) atomicAdd(&slot[1], (unsigned long long)n_lin);
+				if (n_clean) atomicAdd(&slot[2], (unsigned long long)n_clean);
 			}
 		}
 		if (!has_next) break;
