@@ -171,7 +171,10 @@ int ufo_b200_export_leaves(ufo_b200_map* m, uint64_t* codes, float* logodds, uin
  * node of depth min_depth whose cube -- and every ancestor cube -- intersects the box is set to
  * clamp(float(logit(occupancy))) (setOccupancy, :1151-1157), i.e. all voxels below it.
  * min_depth 0..4; colour maps at min_depth 0 only (deeper, the reference also replaces the
- * voxels' colours by the node's mean colour). */
+ * voxels' colours by the node's mean colour).  On a routed map (ufo_b200_route_setup) every rank
+ * takes the same call and sets the bricks it owns; the union of the ranks is the single map.
+ * Between ufo_b200_route_mark and the last ufo_b200_route_apply of a pass: UFO_B200_E_INVALID,
+ * nothing written.  A sharded map: UFO_B200_E_UNSUPPORTED. */
 int ufo_b200_set_value_volume(ufo_b200_map* m, const double box6[6], double occupancy, uint32_t min_depth);
 
 /* Per-node writes as one ordered batch, the same as making the calls one after the other in array
@@ -183,10 +186,16 @@ int ufo_b200_set_value_volume(ufo_b200_map* m, const double box6[6], double occu
  *   op[i] = 1  SET value[i]: setOccupancy :524-538 -> setNodeValue :1037-1057 as intended (the
  *              reference's does not compile): every voxel below the node becomes clamp(value).
  * depths[i] 0..6.  Host arrays.  Rejected as a whole (nothing applied): a code whose depth-0 key lies
- * outside the map (UFO_B200_E_INVALID); depth > 6, a sharded or routed map, SET at depth > 0 on a
- * colour map (UFO_B200_E_UNSUPPORTED).  Leaf colours are not changed.  The min/max change box is not
+ * outside the map (UFO_B200_E_INVALID); depth > 6, a sharded map, SET at depth > 0 on a colour map
+ * (UFO_B200_E_UNSUPPORTED).  Leaf colours are not changed.  The min/max change box is not
  * updated (the reference does not update it for these calls); change detection records the voxels
- * whose value changed.  async != 0 returns after the work is enqueued. */
+ * whose value changed.  async != 0 returns after the work is enqueued.
+ * Routed maps: every rank takes the same batch and applies it to the bricks it owns (a node of
+ * depth 5/6 to its share of the node's bricks), so the union of the ranks is the single map; each
+ * voxel's updates are applied in batch order by its one owner.  A batch between
+ * ufo_b200_route_mark and the last ufo_b200_route_apply of a pass is UFO_B200_E_INVALID.  The
+ * rejections above depend on the arguments and the map's parameters only, so they are the same
+ * on every rank. */
 int ufo_b200_update_nodes(ufo_b200_map* m, const uint64_t* codes, const uint32_t* depths, const uint8_t* ops,
                           const float* values, size_t n, int async);
 
@@ -216,8 +225,9 @@ int ufo_b200_update_nodes_color(ufo_b200_map* m, const uint64_t* codes, const ui
  * origins / ends [n][3] (host arrays): integrateMiss on every node computeRay (octree.h:449-496, as
  * ufo_b200_compute_ray) walks at `depth`, then with hit_end integrateHit on the depth-0 voxel of the
  * GIVEN end point (not the one max_range truncates to).  Rays are applied in array order.  Rejected
- * as a whole: an origin or end outside the map (UFO_B200_E_INVALID); depth > 6, sharded or routed
- * maps (UFO_B200_E_UNSUPPORTED). */
+ * as a whole: an origin or end outside the map (UFO_B200_E_INVALID); depth > 6, sharded maps
+ * (UFO_B200_E_UNSUPPORTED).  Routed maps as ufo_b200_update_nodes: every rank walks every ray and
+ * applies the nodes whose bricks it owns, the hit_end voxel included. */
 int ufo_b200_insert_rays(ufo_b200_map* m, const double* origins, const double* ends, size_t n,
                          double max_range, uint32_t depth, int hit_end, int async);
 
@@ -310,7 +320,8 @@ int ufo_b200_read_data(ufo_b200_map* m, const double* box6, const void* data, si
  * decide this way).  n_bv == 0: the whole map.  An unknown type: UFO_B200_E_INVALID.  reserved is
  * ignored (set it to 0).
  * Each *_bv entry point is its box6 twin with the volume in place of the AABB; the box6 forms are
- * the *_bv forms with one AABB record. */
+ * the *_bv forms with one AABB record.  ufo_b200_set_value_volume_bv takes routed maps like
+ * ufo_b200_set_value_volume: the descent is the same on every rank, each sets the bricks it owns. */
 #define UFO_B200_VOLUME_AABB 0
 #define UFO_B200_VOLUME_FRUSTUM 1
 #define UFO_B200_VOLUME_LINE_SEGMENT 2
@@ -334,6 +345,37 @@ int ufo_b200_write_compressed_bv(ufo_b200_map* m, const ufo_b200_volume* bv, siz
                                  size_t* size, size_t* uncompressed_size);
 int ufo_b200_read_data_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, const void* data, size_t size,
                           int compressed, size_t uncompressed_size);
+/* One file image from several maps that hold disjoint bricks -- the ranks of a routed map.  Every
+ * level above the 16^3-voxel bricks of an image is a function of the bricks' own shapes and
+ * payloads, so the image of the union is assembled from one part per rank:
+ *   ufo_b200_image_part_bv  this map's part of the image for (bv[n_bv], min_depth, expanded), as
+ *                           ufo_b200_write_bv would write it: an opaque, versioned blob holding
+ *                           those arguments, the map's resolution, depth_levels and colour mode,
+ *                           and per brick of the tree its code, shape and node stream.  *size =
+ *                           the blob's bytes; copied when it fits into cap (buf = NULL sizes it).
+ *                           Waits for a pending scan; between ufo_b200_route_mark and the last
+ *                           ufo_b200_route_apply of a pass UFO_B200_E_INVALID.  Other rejections
+ *                           as ufo_b200_write_bv.
+ *   ufo_b200_image_assemble the image of the union of parts[0..n_parts) (sizes[i] bytes each, host
+ *                           memory, any order) on the host; no map or device needed.  with_header:
+ *                           the file image (ufo_b200_write_bv), else the bare node stream
+ *                           (ufo_b200_write_data_bv); compress: the stream as one LZ4 block, as
+ *                           ufo_b200_write_compressed_bv (data_only = !with_header), with
+ *                           acceleration_level / compression_level as there.  *uncompressed_size
+ *                           (may be NULL) = bytes of the node stream.  *size = the image's bytes;
+ *                           copied only when it fits into cap.  UFO_B200_E_INVALID: no parts, a
+ *                           truncated or malformed part, parts that differ in resolution,
+ *                           depth_levels, colour, volume, min_depth or expanded, a brick in two
+ *                           parts (two histories of one brick; also the same part given twice).
+ * A single map's writers are its own part assembled alone, so assembling the ranks' parts gives
+ * the bytes one map holding the union would write.  The parts travel however the caller's ranks
+ * talk (e.g. an all-gather of byte tensors); for a change-box publish take the min / max of the
+ * ranks' ufo_b200_change_bbox first and ask every rank for the part of that box. */
+int ufo_b200_image_part_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, uint32_t min_depth, int expanded,
+                           void* buf, size_t cap, size_t* size);
+int ufo_b200_image_assemble(const void* const* parts, const size_t* sizes, size_t n_parts, int with_header, int compress,
+                            int acceleration_level, int compression_level, void* buf, size_t cap, size_t* size,
+                            size_t* uncompressed_size);
 /* Leaf iteration as ufo_b200_export_nodes, with the reference iterator's rule: a node is returned
  * iff every cube on its path from the root passes the volume (ufo_b200_export_nodes tests the
  * node's own cube only). */
@@ -551,7 +593,9 @@ int ufo_b200_set_shard(ufo_b200_map* m, uint32_t rank, uint32_t world);
  *                           (its own included) in its last mark pass
  * The union of the ranks' value fields equals the single-GPU map (tests/test_gpu_route.py,
  * tests/test_gpu_route_discrete.py).  Pools do not grow during a routed pass: size the map with
- * initial_bricks.  Maps that have seen out-of-tree keys are rejected. */
+ * initial_bricks.  Maps that have seen out-of-tree keys are rejected.  Between passes the ranks
+ * also take setValueVolume and write batches (each applies what it owns; pools grow there as on
+ * one map), and ufo_b200_image_part_bv / ufo_b200_image_assemble give the union's file image. */
 int ufo_b200_route_inbox_bytes(uint32_t world, uint32_t cap_bricks, uint32_t cap_hits, size_t* bytes);
 int ufo_b200_route_inbox_bytes_color(uint32_t world, uint32_t cap_bricks, uint32_t cap_hits, size_t* bytes);
 int ufo_b200_route_setup(ufo_b200_map* m, uint32_t rank, uint32_t world, uint32_t cap_bricks, uint32_t cap_hits,

@@ -124,7 +124,7 @@ SYMBOLS = [
     "ufo_b200_set_early_stopping", "ufo_b200_last_early_stats",
     "ufo_b200_iterate", "ufo_b200_update_nodes_color",
     "ufo_b200_retain_bv", "ufo_b200_retain", "ufo_b200_page_out_bv", "ufo_b200_page_in", "ufo_b200_page_info",
-    "ufo_b200_pool_stats", "ufo_b200_last_update_stats",
+    "ufo_b200_pool_stats", "ufo_b200_last_update_stats", "ufo_b200_image_part_bv", "ufo_b200_image_assemble",
 ]
 
 # ufo_b200_volume: one shape of a bounding volume (type in BoundingVar order, members in v)
@@ -315,6 +315,9 @@ def load():
     lib.ufo_b200_write_data_bv.argtypes = [vp, vp, sz, u32, vp, sz, C.POINTER(sz)]
     lib.ufo_b200_write_compressed_bv.argtypes = [vp, vp, sz, u32, i32, i32, i32, vp, sz, C.POINTER(sz), C.POINTER(sz)]
     lib.ufo_b200_read_data_bv.argtypes = [vp, vp, sz, vp, sz, i32, sz]
+    lib.ufo_b200_image_part_bv.argtypes = [vp, vp, sz, u32, i32, vp, sz, C.POINTER(sz)]
+    lib.ufo_b200_image_assemble.argtypes = [C.POINTER(vp), C.POINTER(sz), sz, i32, i32, i32, i32, vp, sz,
+                                            C.POINTER(sz), C.POINTER(sz)]
     lib.ufo_b200_export_nodes_bv.argtypes = [vp, u32, i32, i32, i32, vp, sz, vp, vp, vp, sz, C.POINTER(sz)]
     lib.ufo_b200_iterate.argtypes = [vp, i32, i32, i32, i32, i32, u32, vp, sz, vp, vp, vp, vp, vp, sz, C.POINTER(sz)]
     lib.ufo_b200_set_value_volume_bv.argtypes = [vp, vp, dbl, u32]
@@ -702,6 +705,19 @@ class Map:
                                                           C.byref(u)))
         return buf[:n.value].tobytes(), int(u.value)
 
+    def image_part(self, volume=None, box=None, min_depth=0, expanded=False):
+        """This map's part of the file image for (volume or box = (min xyz, max xyz), min_depth,
+        expanded) as bytes; assemble_image() of the parts of maps holding disjoint bricks (the ranks
+        of a routed map) is the image of their union."""
+        bv, bp, nb = self._bv(aabb(*box) if box is not None else volume)
+        n = C.c_size_t()
+        self._check(self.lib.ufo_b200_image_part_bv(self.h, bp, nb, int(min_depth), int(expanded), None, 0, C.byref(n)))
+        buf = np.empty(n.value, np.uint8)
+        self._check(self.lib.ufo_b200_image_part_bv(self.h, bp, nb, int(min_depth), int(expanded), buf.ctypes.data,
+                                                    n.value, C.byref(n)))
+        assert n.value == len(buf)
+        return buf.tobytes()
+
     def read_data_bv(self, data, volume=None, compressed=False, uncompressed_size=0):
         """Octree::readData(stream, BoundingVolume, ...): merge a node stream into the map."""
         bv, bp, nb = self._bv(volume)
@@ -935,6 +951,27 @@ class Map:
         p = np.array([occupied_thres, free_thres, prob_hit, prob_miss, clamping_thres_min,
                       clamping_thres_max], dtype=np.float64)
         self._check(self.lib.ufo_b200_set_sensor_model(self.h, p.ctypes.data))
+
+
+def assemble_image(parts, with_header=True, compressed=False, acceleration=1, level=0):
+    """The file image (with_header) or node stream of the union of image parts (Map.image_part,
+    any order), on the host.  compressed: (bytes, uncompressed node-stream size) as
+    Map.write_compressed_bv with data_only = not with_header; otherwise bytes."""
+    lib = load()
+    bufs = [np.ascontiguousarray(np.frombuffer(p, np.uint8)) for p in parts]
+    ptrs = (C.c_void_p * max(len(bufs), 1))(*[b.ctypes.data for b in bufs])
+    sizes = (C.c_size_t * max(len(bufs), 1))(*[len(b) for b in bufs])
+    args = (ptrs, sizes, len(bufs), int(with_header), int(compressed), int(acceleration), int(level))
+    n, u = C.c_size_t(), C.c_size_t()
+    rc = lib.ufo_b200_image_assemble(*args, None, 0, C.byref(n), C.byref(u))
+    if rc != OK:
+        raise UfoError(rc, "ufo_b200_image_assemble failed")
+    out = np.empty(max(n.value, 1), np.uint8)
+    rc = lib.ufo_b200_image_assemble(*args, out.ctypes.data, n.value, C.byref(n), C.byref(u))
+    if rc != OK:
+        raise UfoError(rc, "ufo_b200_image_assemble failed")
+    data = out[:n.value].tobytes()
+    return (data, int(u.value)) if compressed else data
 
 
 def page_info(blob):

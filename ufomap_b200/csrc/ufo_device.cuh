@@ -232,6 +232,14 @@ UFO_HD uint32_t brick_owner(uint64_t brick_key, uint32_t world)
 	return (uint32_t)((hash_u64(brick_key ^ 0x9e3779b97f4a7c15ull) >> 7) % world);
 }
 
+// Whether a write batch or setValueVolume applies to the brick on this map: every rank of a routed
+// map takes the same call and only the owner creates and writes the brick, so that the ranks keep
+// disjoint bricks whose union is the single map.
+UFO_HD bool brick_owned(const DeviceMap& M, uint64_t brick_key)
+{
+	return M.route_world <= 1 || brick_owner(brick_key, M.route_world) == M.route_rank;
+}
+
 // 21 bits per axis
 UFO_HD uint64_t pack_key(uint32_t x, uint32_t y, uint32_t z)
 {

@@ -757,7 +757,7 @@ __global__ void __launch_bounds__(64) k_volume_mark(DeviceMap M, VolumeArgs v)
 			ok = ok && vol_hits_t<G>(v.vol, c, M.g.half_size[d - 1]);  // cube of the depth d-1 ancestor
 		}
 		uint32_t slot = kNone;
-		if (ok) {
+		if (ok && brick_owned(M, pack_key(kx, ky, kz))) {
 			slot = brick_find_or_create(M, pack_key(kx, ky, kz));
 			if (slot != kNone) touch_brick(M, slot);
 		}

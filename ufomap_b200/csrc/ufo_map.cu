@@ -2181,10 +2181,10 @@ struct UpNode {
 };
 
 struct ExportPlan {
-	std::vector<uint32_t> order;  // bricks of the map in Morton (= stream) order
-	std::vector<BrickInfo> info;  // indexed by brick slot
+	std::vector<uint32_t> order;  // bricks in Morton (= stream) order, as indices into info
+	const BrickInfo* info = nullptr;
 	std::vector<UpNode> nodes;    // nodes[0] = root (if any brick exists)
-	std::vector<unsigned long long> codes;
+	const unsigned long long* codes = nullptr;  // Morton code of brick order[i]
 	uint32_t P = 4;
 	uint32_t levels = 16;
 	uint32_t min_depth = 0;
@@ -2270,9 +2270,9 @@ void put_payload_host(Sink& sink, uint32_t P, float occ, uint32_t rgb)
 	sink(b, P);
 }
 
+// rec[i]: the stream bytes of brick info[i] when it is written as a record
 template <class Sink>
-void emit_upper(const ExportPlan& plan, const std::vector<unsigned long long>& offs, const uint8_t* packed,
-                int32_t idx, uint32_t d, Sink& sink)
+void emit_upper(const ExportPlan& plan, const std::vector<const uint8_t*>& rec, int32_t idx, uint32_t d, Sink& sink)
 {
 	const UpNode& n = plan.nodes[idx];
 	sink(&n.mask, 1);
@@ -2285,21 +2285,45 @@ void emit_upper(const ExportPlan& plan, const std::vector<unsigned long long>& o
 			const uint32_t slot = plan.order[c];
 			const BrickInfo& bi = plan.info[slot];
 			if (bi.size == 0) continue;
-			if (bi.flags & 4u) sink(packed + offs[slot], bi.size);
+			if (bi.flags & 4u) sink(rec[slot], bi.size);
 			else put_payload_host(sink, plan.P, bi.occ, bi.rgb);
 		} else if (plan.nodes[c].has) {
-			emit_upper(plan, offs, packed, c, d - 1, sink);
+			emit_upper(plan, rec, c, d - 1, sink);
 		} else {
 			put_payload_host(sink, plan.P, plan.nodes[c].occ, plan.nodes[c].rgb);
 		}
 	}
 }
 
-// Produces the node stream (optionally behind the file header) through sink(ptr, len) calls, in
-// order.  *total = bytes produced.
-template <class Sink>
-int export_image(Map* m, int pruned, uint32_t min_depth, const Volume& vol, bool with_header, Sink&& sink,
-                 unsigned long long* total)
+// octree.h:850-860; doubles print with the default ostream precision = %g
+int image_header(char* head, size_t cap, bool color, double resolution, uint32_t levels, bool compressed,
+                 unsigned long long data_size)
+{
+	return snprintf(head, cap,
+	                "# UFOMap file\n# (feel free to add / change comments, but leave the first line as it "
+	                "is!)\n#\nversion 1.0.0\nid %s\nresolution %g\ndepth_levels %u\ncompressed %d\n"
+	                "uncompressed_data_size %d\ndata\n",
+	                color ? "occupancy_map_color" : "occupancy_map", resolution, levels, compressed ? 1 : 0, (int)data_size);
+}
+
+// One map's share of a file image for (volume, min_depth, pruned): the bricks that are part of the
+// tree, ascending by Morton code, with their BrickInfo (k_brick_stream) and the stream bytes of those
+// written as records.  Everything above the bricks is a function of these alone (build_upper), so
+// the image of a union of maps that hold disjoint bricks -- the ranks of a routed map -- is the
+// image of the union of their parts.
+struct ImagePart {
+	uint32_t color = 0, depth_levels = 0, min_depth = 0, pruned = 1;
+	double resolution = 0.0;
+	std::vector<VolRec> vol;                // the volume records as given (reserved = 0)
+	std::vector<unsigned long long> codes;  // brick codes (Morton code of the brick key), ascending
+	std::vector<BrickInfo> info;
+	const uint8_t* stream = nullptr;  // record bytes of the bricks with info.flags & 4, in order
+	size_t stream_bytes = 0;
+	std::vector<uint8_t> own;  // the stream of a part made from a map
+};
+
+// The map's part (the device work of the file writers: both passes of k_brick_stream).
+int make_part(Map* m, int pruned, uint32_t min_depth, const Volume& vol, ImagePart& part)
 {
 	if (m->device == -2) return UFO_B200_E_CUDA;
 	if (m->M.g.depth_levels < 5) {
@@ -2315,40 +2339,23 @@ int export_image(Map* m, int pruned, uint32_t min_depth, const Volume& vol, bool
 	cudaStream_t s = m->stream;
 	const uint32_t nb = m->n_bricks;
 	const bool color = m->M.color != 0;
-	ExportPlan plan;
-	plan.P = color ? 7 : 4;
-	plan.levels = m->M.g.depth_levels;
-	plan.min_depth = min_depth;
-	plan.pruned = pruned != 0;
-	plan.g = &m->M.g;
-	plan.vol = vol;
-	*total = 0;
+	part.color = color ? 1u : 0u;
+	part.depth_levels = m->M.g.depth_levels;
+	part.min_depth = min_depth;
+	part.pruned = pruned ? 1u : 0u;
+	part.resolution = m->M.g.resolution;
+	part.vol.assign(vol.rec, vol.rec + vol.n);
+	for (VolRec& r : part.vol) r.reserved = 0;
 	const double c0[3] = {0.0, 0.0, 0.0};
-	auto header = [&](char* head, size_t cap, unsigned long long data_size) {
-		// octree.h:850-860; doubles print with the default ostream precision = %g
-		return snprintf(head, cap,
-		                "# UFOMap file\n# (feel free to add / change comments, but leave the first line as it "
-		                "is!)\n#\nversion 1.0.0\nid %s\nresolution %g\ndepth_levels %u\ncompressed 0\n"
-		                "uncompressed_data_size %d\ndata\n",
-		                color ? "occupancy_map_color" : "occupancy_map", m->M.g.resolution, plan.levels, (int)data_size);
-	};
-	if (!vol_hits(plan.vol, c0, plan.g->half_size[plan.levels])) {
-		// "No node intersects": the reference writes no node data at all (OMB:1462-1468)
-		if (with_header) {
-			char head[512];
-			const int hl = header(head, sizeof head, 0);
-			sink(head, (size_t)hl);
-			*total = (unsigned long long)hl;
-		}
-		return UFO_B200_OK;
-	}
-	plan.info.resize(nb);
+	// "No node intersects": the reference writes no node data at all (OMB:1462-1468)
+	if (!vol_hits(vol, c0, m->M.g.half_size[part.depth_levels])) return UFO_B200_OK;
+	std::vector<BrickInfo> info(nb);
 	std::vector<unsigned long long> keys(nb);
 	DevBuf b_info, b_offs, b_out;
 	BrickInfo* d_info = nullptr;
 	DeviceVolume dvol;
 	// an empty or single-box volume takes the instantiation with the inline box test
-	Volume hv = plan.vol;
+	Volume hv = vol;
 	const bool general = volume_is_general(hv);
 	const Volume dv = dvol.upload(hv, s);
 	auto brick_stream = [&](uint32_t n, size_t smem, const unsigned long long* offs, uint8_t* out) {
@@ -2361,16 +2368,16 @@ int export_image(Map* m, int pruned, uint32_t min_depth, const Volume& vol, bool
 		d_info = b_info.alloc<BrickInfo>(nb);
 		brick_stream(nb, 0, nullptr, nullptr);
 		CK(cudaGetLastError());
-		CK(cudaMemcpyAsync(plan.info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
+		CK(cudaMemcpyAsync(info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
 		CK(cudaMemcpyAsync(keys.data(), m->M.brick_key, 8ull * nb, cudaMemcpyDeviceToHost, s));
 		CK(cudaStreamSynchronize(s));
 	}
 	// bricks that are part of the tree, in Morton order; a leaf brick with the default payload is
-	// indistinguishable from untouched space
+	// indistinguishable from untouched space (so are the empty foreign bricks a routed rank keeps)
 	std::vector<std::pair<unsigned long long, uint32_t>> sorted;
 	sorted.reserve(nb);
 	for (uint32_t b = 0; b < nb; ++b) {
-		const BrickInfo& bi = plan.info[b];
+		const BrickInfo& bi = info[b];
 		if (bi.flags & 2u) continue;
 		if (!(bi.flags & 1u) && bi.occ == 0.0f && bi.rgb == 0u) continue;
 		uint32_t x, y, z;
@@ -2378,35 +2385,121 @@ int export_image(Map* m, int pruned, uint32_t min_depth, const Volume& vol, bool
 		sorted.emplace_back(spread3_host(x) | (spread3_host(y) << 1) | (spread3_host(z) << 2), b);
 	}
 	std::sort(sorted.begin(), sorted.end());
-	plan.order.resize(sorted.size());
-	plan.codes.resize(sorted.size());
+	part.codes.resize(sorted.size());
+	part.info.resize(sorted.size());
 	std::vector<unsigned long long> offs(nb, ~0ull);
 	unsigned long long packed_bytes = 0;
 	for (size_t i = 0; i < sorted.size(); ++i) {
-		plan.codes[i] = sorted[i].first;
-		plan.order[i] = sorted[i].second;
-		const BrickInfo& bi = plan.info[sorted[i].second];
+		part.codes[i] = sorted[i].first;
+		const BrickInfo& bi = info[sorted[i].second];
+		part.info[i] = bi;
 		if (bi.flags & 4u) {
 			offs[sorted[i].second] = packed_bytes;
 			packed_bytes += bi.size;
 		}
 	}
-	bool root_has = false;
-	unsigned long long data_size = 1 + plan.P;  // children byte + root payload
-	if (!sorted.empty()) {
-		build_upper(plan, plan.levels, 0, sorted.size(), c0);
-		root_has = plan.nodes[0].has;
-		if (root_has) data_size = 1 + plan.nodes[0].size;
-	}
-	std::vector<uint8_t> packed(packed_bytes);
+	part.own.resize(packed_bytes);
 	if (packed_bytes) {
 		unsigned long long* d_offs = b_offs.alloc<unsigned long long>(nb);
 		uint8_t* d_out = b_out.alloc<uint8_t>(packed_bytes);
 		CK(cudaMemcpyAsync(d_offs, offs.data(), 8ull * nb, cudaMemcpyHostToDevice, s));
 		brick_stream(nb, kBrickStreamMax, d_offs, d_out);
 		CK(cudaGetLastError());
-		CK(cudaMemcpyAsync(packed.data(), d_out, packed_bytes, cudaMemcpyDeviceToHost, s));
+		CK(cudaMemcpyAsync(part.own.data(), d_out, packed_bytes, cudaMemcpyDeviceToHost, s));
 		CK(cudaStreamSynchronize(s));
+	}
+	part.stream = part.own.data();
+	part.stream_bytes = packed_bytes;
+	return UFO_B200_OK;
+}
+
+bool same_image(const ImagePart& a, const ImagePart& b)
+{
+	return a.color == b.color && a.depth_levels == b.depth_levels && a.min_depth == b.min_depth && a.pruned == b.pruned &&
+	       std::memcmp(&a.resolution, &b.resolution, sizeof(double)) == 0 && a.vol.size() == b.vol.size() &&
+	       (a.vol.empty() || std::memcmp(a.vol.data(), b.vol.data(), sizeof(VolRec) * a.vol.size()) == 0);
+}
+
+// The image of the union of the parts through sink(ptr, len) calls, in order: the file image when
+// with_header, else the bare node stream.  The parts must agree on everything but their bricks, and
+// no brick may be in two of them (UFO_B200_E_INVALID).  *total = bytes produced, *data = bytes of the
+// node stream among them.
+template <class Sink>
+int assemble(const std::vector<const ImagePart*>& parts, bool with_header, Sink&& sink, unsigned long long* total,
+             unsigned long long* data = nullptr)
+{
+	*total = 0;
+	if (data) *data = 0;
+	if (parts.empty()) return UFO_B200_E_INVALID;
+	const ImagePart& h = *parts[0];
+	for (const ImagePart* p : parts)
+		if (!same_image(*p, h)) return UFO_B200_E_INVALID;
+	const Geometry g = make_geometry(h.resolution, h.depth_levels);
+	ExportPlan plan;
+	plan.P = h.color ? 7 : 4;
+	plan.levels = h.depth_levels;
+	plan.min_depth = h.min_depth;
+	plan.pruned = h.pruned != 0;
+	plan.g = &g;
+	plan.vol = Volume{h.vol.data(), (uint32_t)h.vol.size(), {}, {}};
+	const double c0[3] = {0.0, 0.0, 0.0};
+	if (!vol_hits(plan.vol, c0, g.half_size[plan.levels])) {
+		if (with_header) {
+			char head[512];
+			const int hl = image_header(head, sizeof head, h.color, h.resolution, plan.levels, false, 0);
+			sink(head, (size_t)hl);
+			*total = (unsigned long long)hl;
+		}
+		return UFO_B200_OK;
+	}
+	// the bricks of all parts in Morton order; rec[i]: stream bytes of brick i
+	std::vector<BrickInfo> merged;
+	std::vector<unsigned long long> merged_codes;
+	std::vector<const uint8_t*> rec;
+	if (parts.size() == 1) {
+		plan.info = h.info.data();
+		plan.codes = h.codes.data();
+		rec.resize(h.info.size());
+		const uint8_t* at = h.stream;
+		for (size_t i = 0; i < h.info.size(); ++i) {
+			rec[i] = at;
+			if (h.info[i].flags & 4u) at += h.info[i].size;
+		}
+	} else {
+		std::vector<std::pair<unsigned long long, std::pair<const BrickInfo*, const uint8_t*>>> all;
+		size_t n = 0;
+		for (const ImagePart* p : parts) n += p->codes.size();
+		all.reserve(n);
+		for (const ImagePart* p : parts) {
+			const uint8_t* at = p->stream;
+			for (size_t i = 0; i < p->codes.size(); ++i) {
+				all.push_back({p->codes[i], {&p->info[i], at}});
+				if (p->info[i].flags & 4u) at += p->info[i].size;
+			}
+		}
+		std::sort(all.begin(), all.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+		for (size_t i = 1; i < all.size(); ++i)
+			if (all[i].first == all[i - 1].first) return UFO_B200_E_INVALID;  // two histories of one brick
+		merged_codes.resize(n);
+		merged.resize(n);
+		rec.resize(n);
+		for (size_t i = 0; i < n; ++i) {
+			merged_codes[i] = all[i].first;
+			merged[i] = *all[i].second.first;
+			rec[i] = all[i].second.second;
+		}
+		plan.info = merged.data();
+		plan.codes = merged_codes.data();
+	}
+	const size_t nb = rec.size();
+	plan.order.resize(nb);
+	std::iota(plan.order.begin(), plan.order.end(), 0u);
+	bool root_has = false;
+	unsigned long long data_size = 1 + plan.P;  // children byte + root payload
+	if (nb) {
+		build_upper(plan, plan.levels, 0, nb, c0);
+		root_has = plan.nodes[0].has;
+		if (root_has) data_size = 1 + plan.nodes[0].size;
 	}
 	unsigned long long produced = 0;
 	auto counted = [&](const void* p, size_t len) {
@@ -2415,20 +2508,34 @@ int export_image(Map* m, int pruned, uint32_t min_depth, const Volume& vol, bool
 	};
 	if (with_header) {
 		char head[512];
-		const int hl = header(head, sizeof head, data_size);
+		const int hl = image_header(head, sizeof head, h.color, h.resolution, plan.levels, false, data_size);
 		counted(head, (size_t)hl);
 	}
+	const unsigned long long head_bytes = produced;
 	const uint8_t children = root_has ? 0xff : 0x00;
 	counted(&children, 1);
 	if (root_has) {
-		emit_upper(plan, offs, packed.data(), 0, plan.levels, counted);
+		emit_upper(plan, rec, 0, plan.levels, counted);
 	} else {
-		const float occ = sorted.empty() ? 0.0f : plan.nodes[0].occ;
-		const uint32_t rgb = sorted.empty() ? 0u : plan.nodes[0].rgb;
+		const float occ = nb ? plan.nodes[0].occ : 0.0f;
+		const uint32_t rgb = nb ? plan.nodes[0].rgb : 0u;
 		put_payload_host(counted, plan.P, occ, rgb);
 	}
 	*total = produced;
+	if (data) *data = produced - head_bytes;
 	return UFO_B200_OK;
+}
+
+// the map's image through sink: its part, assembled alone
+template <class Sink>
+int export_image(Map* m, int pruned, uint32_t min_depth, const Volume& vol, bool with_header, Sink&& sink,
+                 unsigned long long* total)
+{
+	*total = 0;
+	ImagePart part;
+	const int rc = make_part(m, pruned, min_depth, vol, part);
+	if (rc != UFO_B200_OK) return rc;
+	return assemble({&part}, with_header, sink, total);
 }
 }  // namespace
 
@@ -2475,6 +2582,137 @@ bool lz4_compress(const std::vector<uint8_t>& in, int acceleration, int level, s
 	out.resize((size_t)n);
 	return true;
 }
+
+// The image of the parts into buf (*size = its bytes; copied only when it fits into cap): the file
+// image (with_header) or the bare node stream; compress: the node stream as one LZ4 block, behind
+// the header with "compressed 1" when with_header.  *uncompressed_size = bytes of the node stream.
+int image_to_buffer(const std::vector<const ImagePart*>& parts, bool with_header, bool compress, int acceleration, int level,
+                    void* buf, size_t cap, size_t* size, size_t* uncompressed_size, Map* m)
+{
+	std::vector<uint8_t> raw;
+	unsigned long long total = 0, data = 0;
+	const int rc = assemble(parts, with_header && !compress, [&](const void* p, size_t len) {
+		const uint8_t* b = static_cast<const uint8_t*>(p);
+		raw.insert(raw.end(), b, b + len);
+	}, &total, &data);
+	if (rc != UFO_B200_OK) return rc;
+	std::vector<uint8_t> packed;
+	std::string head;
+	if (compress) {
+		if (!lz4_compress(raw, acceleration, level, packed)) {
+			if (m) m->set_error("LZ4 compression failed");
+			return UFO_B200_E_INVALID;
+		}
+		if (with_header) {
+			const ImagePart& p = *parts[0];
+			char h[512];
+			const int hl = image_header(h, sizeof h, p.color != 0, p.resolution, p.depth_levels, true, raw.size());
+			head.assign(h, (size_t)hl);
+		}
+	}
+	const std::vector<uint8_t>& body = compress ? packed : raw;
+	const size_t need = head.size() + body.size();
+	*size = need;
+	if (uncompressed_size) *uncompressed_size = (size_t)data;
+	if (buf && cap >= need) {
+		std::memcpy(buf, head.data(), head.size());
+		std::memcpy(static_cast<uint8_t*>(buf) + head.size(), body.data(), body.size());
+	}
+	return UFO_B200_OK;
+}
+
+// ---- a part as bytes (ufo_b200_image_part_bv): header, volume records, {code, BrickInfo} per brick
+// ascending, then the record bytes.  Little-endian, as the devices that make it.
+constexpr uint32_t kPartMagic = 0x50494655u;  // "UFIP"
+constexpr uint32_t kPartVersion = 1;
+
+struct PartHeader {
+	uint32_t magic, version, color, depth_levels, min_depth, pruned;
+	uint64_t resolution_bits, n_bv, n_bricks, stream_bytes;
+};
+static_assert(sizeof(PartHeader) == 56, "the part header stays 56 bytes");
+
+struct PartBrick {
+	uint64_t code;
+	BrickInfo info;
+};
+static_assert(sizeof(PartBrick) == 24, "a part's brick entry stays 24 bytes");
+
+size_t part_bytes(const ImagePart& p)
+{
+	return sizeof(PartHeader) + sizeof(VolRec) * p.vol.size() + sizeof(PartBrick) * p.codes.size() + p.stream_bytes;
+}
+
+void put_part(const ImagePart& p, uint8_t* out)
+{
+	PartHeader h{kPartMagic, kPartVersion, p.color, p.depth_levels, p.min_depth, p.pruned, 0, p.vol.size(), p.codes.size(), p.stream_bytes};
+	std::memcpy(&h.resolution_bits, &p.resolution, 8);
+	std::memcpy(out, &h, sizeof h);
+	out += sizeof h;
+	if (!p.vol.empty()) std::memcpy(out, p.vol.data(), sizeof(VolRec) * p.vol.size());
+	out += sizeof(VolRec) * p.vol.size();
+	for (size_t i = 0; i < p.codes.size(); ++i) {
+		const PartBrick b{p.codes[i], p.info[i]};
+		std::memcpy(out, &b, sizeof b);
+		out += sizeof b;
+	}
+	if (p.stream_bytes) std::memcpy(out, p.stream, p.stream_bytes);
+}
+
+// A part as put_part wrote it, or false: every field in range, sizes that add up, brick codes inside
+// the tree and strictly ascending, BrickInfo of the shapes k_brick_stream produces.  The stream stays
+// in the caller's blob.
+bool parse_part(const void* blob, size_t size, ImagePart& p)
+{
+	if (!blob || size < sizeof(PartHeader)) return false;
+	const uint8_t* b = static_cast<const uint8_t*>(blob);
+	PartHeader h;
+	std::memcpy(&h, b, sizeof h);
+	if (h.magic != kPartMagic || h.version != kPartVersion) return false;
+	if (h.color > 1 || h.pruned > 1 || h.min_depth > 4 || h.depth_levels < 5 || h.depth_levels > 21) return false;
+	double res;
+	std::memcpy(&res, &h.resolution_bits, 8);
+	if (!(res > 0.0) || !std::isfinite(res)) return false;
+	size_t rest = size - sizeof h;
+	if (h.n_bv > 0xffffffffull || h.n_bv > rest / sizeof(VolRec)) return false;
+	rest -= (size_t)h.n_bv * sizeof(VolRec);
+	if (h.n_bricks > rest / sizeof(PartBrick)) return false;
+	rest -= (size_t)h.n_bricks * sizeof(PartBrick);
+	if (h.stream_bytes != rest) return false;
+	p.color = h.color;
+	p.depth_levels = h.depth_levels;
+	p.min_depth = h.min_depth;
+	p.pruned = h.pruned;
+	p.resolution = res;
+	b += sizeof h;
+	p.vol.resize((size_t)h.n_bv);
+	if (h.n_bv) std::memcpy(p.vol.data(), b, sizeof(VolRec) * (size_t)h.n_bv);
+	for (const VolRec& r : p.vol)
+		if (r.type >= kVolTypes) return false;
+	b += sizeof(VolRec) * (size_t)h.n_bv;
+	const unsigned long long code_end = 1ull << (3 * (h.depth_levels - 4));
+	const uint32_t P = h.color ? 7u : 4u;
+	unsigned long long record_bytes = 0;
+	p.codes.resize((size_t)h.n_bricks);
+	p.info.resize((size_t)h.n_bricks);
+	for (size_t i = 0; i < p.codes.size(); ++i) {
+		PartBrick e;
+		std::memcpy(&e, b + i * sizeof e, sizeof e);
+		if (e.code >= code_end || (i && e.code <= p.codes[i - 1])) return false;
+		if (e.info.flags == 5u) {
+			if (e.info.size == 0 || e.info.size > (uint32_t)kBrickStreamMax) return false;
+			record_bytes += e.info.size;
+		} else if (e.info.flags > 1u || (e.info.size != 0 && e.info.size != P)) {
+			return false;
+		}
+		p.codes[i] = e.code;
+		p.info[i] = e.info;
+	}
+	if (record_bytes != h.stream_bytes) return false;
+	p.stream = b + sizeof(PartBrick) * p.codes.size();
+	p.stream_bytes = (size_t)h.stream_bytes;
+	return true;
+}
 }  // namespace
 
 namespace
@@ -2493,6 +2731,10 @@ int set_value_volume_allowed(Map* m, uint32_t min_depth)
 	if (m->M.shard_world > 1) {
 		m->set_error("setValueVolume on a sharded map is not supported");
 		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (m->route_stage == 1) {
+		m->set_error("setValueVolume between ufo_b200_route_mark and the last ufo_b200_route_apply of the pass");
+		return UFO_B200_E_INVALID;
 	}
 	return UFO_B200_OK;
 }
@@ -2569,10 +2811,6 @@ int ufo_b200_set_value_volume_bv(ufo_b200_map* m, const ufo_b200_volume* bv, dou
 	if (!volume_ok(m, bv, 1)) return UFO_B200_E_INVALID;
 	const int allowed = set_value_volume_allowed(m, min_depth);
 	if (allowed != UFO_B200_OK) return allowed;
-	if (m->M.route_world > 1) {
-		m->set_error("setValueVolume on a routed map is not supported");
-		return UFO_B200_E_UNSUPPORTED;
-	}
 	return guarded(m, [&]() {
 		const Geometry& g = m->M.g;
 		const Volume hv{as_records(bv), 1, {}, {}};
@@ -3122,39 +3360,51 @@ int ufo_b200_write_compressed_bv(ufo_b200_map* m, const ufo_b200_volume* bv, siz
 			m->set_error("liblz4.so.1 not found: compressed output is unavailable");
 			return (int)UFO_B200_E_UNSUPPORTED;
 		}
-		std::vector<uint8_t> raw;
-		unsigned long long total = 0;
-		int rc = export_image(m, 1, min_depth, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, false, [&](const void* p, size_t len) {
-			const uint8_t* b = static_cast<const uint8_t*>(p);
-			raw.insert(raw.end(), b, b + len);
-		}, &total);
+		ImagePart part;
+		const int rc = make_part(m, 1, min_depth, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, part);
 		if (rc != UFO_B200_OK) return rc;
-		std::vector<uint8_t> packed;
-		if (!lz4_compress(raw, acceleration_level, compression_level, packed)) {
-			m->set_error("LZ4 compression failed");
-			return (int)UFO_B200_E_INVALID;
-		}
-		std::string head;
-		if (!data_only) {
-			// octree.h:850-860 with "compressed 1"
-			char h[512];
-			const int hl = snprintf(h, sizeof h,
-			                        "# UFOMap file\n# (feel free to add / change comments, but leave the first line as it "
-			                        "is!)\n#\nversion 1.0.0\nid %s\nresolution %g\ndepth_levels %u\ncompressed 1\n"
-			                        "uncompressed_data_size %d\ndata\n",
-			                        m->M.color ? "occupancy_map_color" : "occupancy_map", m->M.g.resolution, m->M.g.depth_levels,
-			                        (int)raw.size());
-			head.assign(h, (size_t)hl);
-		}
-		const size_t need = head.size() + packed.size();
-		*size = need;
-		if (uncompressed_size) *uncompressed_size = raw.size();
-		if (buf && cap >= need) {
-			std::memcpy(buf, head.data(), head.size());
-			std::memcpy(static_cast<uint8_t*>(buf) + head.size(), packed.data(), packed.size());
-		}
+		return image_to_buffer({&part}, !data_only, true, acceleration_level, compression_level, buf, cap, size,
+		                       uncompressed_size, m);
+	});
+}
+
+int ufo_b200_image_part_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, uint32_t min_depth, int expanded,
+                           void* buf, size_t cap, size_t* size)
+{
+	if (!m || !size) return UFO_B200_E_INVALID;
+	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
+	if (m->route_stage == 1) {
+		m->set_error("ufo_b200_image_part_bv between ufo_b200_route_mark and the last ufo_b200_route_apply of the pass");
+		return UFO_B200_E_INVALID;
+	}
+	return guarded(m, [&]() {
+		ImagePart part;
+		const int rc = make_part(m, expanded ? 0 : 1, min_depth, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, part);
+		if (rc != UFO_B200_OK) return rc;
+		*size = part_bytes(part);
+		if (buf && cap >= *size) put_part(part, static_cast<uint8_t*>(buf));
 		return (int)UFO_B200_OK;
 	});
+}
+
+int ufo_b200_image_assemble(const void* const* parts, const size_t* sizes, size_t n_parts, int with_header, int compress,
+                            int acceleration_level, int compression_level, void* buf, size_t cap, size_t* size,
+                            size_t* uncompressed_size)
+{
+	if (!parts || !sizes || !n_parts || !size) return UFO_B200_E_INVALID;
+	if (compress && !lz4().ok) return UFO_B200_E_UNSUPPORTED;
+	try {
+		std::vector<ImagePart> ps(n_parts);
+		std::vector<const ImagePart*> ptrs(n_parts);
+		for (size_t i = 0; i < n_parts; ++i) {
+			if (!parse_part(parts[i], sizes[i], ps[i])) return (int)UFO_B200_E_INVALID;
+			ptrs[i] = &ps[i];
+		}
+		return image_to_buffer(ptrs, with_header != 0, compress != 0, acceleration_level, compression_level, buf, cap, size,
+		                       uncompressed_size, nullptr);
+	} catch (std::bad_alloc&) {
+		return (int)UFO_B200_E_NOMEM;
+	}
 }
 
 int ufo_b200_write_compressed(ufo_b200_map* m, const double* box6, uint32_t min_depth, int data_only,
@@ -3388,7 +3638,9 @@ int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, floa
 	plan.levels = L;
 	plan.pruned = true;
 	plan.g = &m->M.g;
-	plan.info.resize(nb);
+	std::vector<BrickInfo> info(nb);
+	std::vector<unsigned long long> brick_codes;
+	plan.info = info.data();
 	IterWalk w;
 	w.plan = &plan;
 	w.a = args;
@@ -3414,15 +3666,15 @@ int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, floa
 		d_info = b_info.alloc<BrickInfo>(nb);
 		brick_iter(nullptr, nullptr);
 		CK(cudaGetLastError());
-		CK(cudaMemcpyAsync(plan.info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
+		CK(cudaMemcpyAsync(info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
 		CK(cudaMemcpyAsync(keys.data(), m->M.brick_key, 8ull * nb, cudaMemcpyDeviceToHost, s));
 		CK(cudaStreamSynchronize(s));
 	}
-	// bricks in the tree, in Morton order (as export_image: a default leaf brick is untouched space)
+	// bricks in the tree, in Morton order (as make_part: a default leaf brick is untouched space)
 	std::vector<std::pair<unsigned long long, uint32_t>> sorted;
 	sorted.reserve(nb);
 	for (uint32_t b = 0; b < nb; ++b) {
-		const BrickInfo& bi = plan.info[b];
+		const BrickInfo& bi = info[b];
 		if (bi.flags & 2u) continue;
 		if (!(bi.flags & 1u) && bi.occ == 0.0f && bi.rgb == 0u) continue;
 		uint32_t x, y, z;
@@ -3431,11 +3683,12 @@ int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, floa
 	}
 	std::sort(sorted.begin(), sorted.end());
 	plan.order.resize(sorted.size());
-	plan.codes.resize(sorted.size());
+	brick_codes.resize(sorted.size());
 	for (size_t i = 0; i < sorted.size(); ++i) {
-		plan.codes[i] = sorted[i].first;
+		brick_codes[i] = sorted[i].first;
 		plan.order[i] = sorted[i].second;
 	}
+	plan.codes = brick_codes.data();
 	if (sorted.empty()) {
 		iter_walk(w, -1, L, 0ull, c0, 0.0f, w.default_flags, 0u, true);
 	} else {
@@ -3494,7 +3747,7 @@ int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, floa
 				put(p.first);
 			} else {
 				const IterRec* r = packed.data() + w.offs[p.second];
-				for (uint32_t i = 0; i < plan.info[p.second].size; ++i) put(r[i]);
+				for (uint32_t i = 0; i < info[p.second].size; ++i) put(r[i]);
 			}
 		}
 	}
@@ -3848,9 +4101,13 @@ int write_allowed(Map* m, uint32_t depth)
 		m->set_error("write depth %u exceeds the tree's depth_levels %u", depth, m->M.g.depth_levels);
 		return UFO_B200_E_INVALID;
 	}
-	if (m->M.shard_world > 1 || m->M.route_world > 1) {
-		m->set_error("per-node writes on a sharded / routed map are not supported");
+	if (m->M.shard_world > 1) {
+		m->set_error("per-node writes on a sharded map are not supported");
 		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (m->route_stage == 1) {
+		m->set_error("a write between ufo_b200_route_mark and the last ufo_b200_route_apply of the pass");
+		return UFO_B200_E_INVALID;
 	}
 	if (m->poisoned) {
 		m->set_error("an earlier scan failed half-way; ufo_b200_clear() the map before writing again");

@@ -7,7 +7,9 @@
 //   1. k_write_expand: one thread per entry (or ray) finds or creates the bricks it covers and
 //      writes WRITE RECORDS -- (brick slot, sequence number) -> which blocks / voxels, ADD or SET,
 //      value -- into a region the host reserved for it.  No leaf is written here, so the phase can
-//      be repeated after a pool growth.
+//      be repeated after a pool growth.  On a routed map every rank expands the whole batch --
+//      ray walks included -- and keeps the records of the bricks it owns (brick_owned); the
+//      others become padding.
 //   2. a stable radix sort of the record keys (brick slot << 32 | sequence number), then
 //      k_write_segments finds each brick's run of records.
 //   3. k_write_apply: one CTA of 64 threads per brick, thread = 4^3 block; the brick's records
@@ -94,7 +96,14 @@ __device__ __forceinline__ void put_record(const DeviceMap& M, const WriteArgs& 
                                            uint32_t bx, uint32_t by, uint32_t bz, unsigned long long bmask,
                                            unsigned long long vmask, float value, uint32_t op)
 {
-	const uint32_t slot = brick_find_or_create(M, pack_key(bx, by, bz));  // kNone: a pool overflowed
+	const unsigned long long key = pack_key(bx, by, bz);
+	if (!brick_owned(M, key)) {
+		// another rank of a routed map applies it: the slot stays padding
+		a.keys[at] = kWritePad;
+		a.idx[at] = (uint32_t)at;
+		return;
+	}
+	const uint32_t slot = brick_find_or_create(M, key);  // kNone: a pool overflowed
 	a.keys[at] = ((unsigned long long)slot << 32) | seq;
 	a.idx[at] = (uint32_t)at;
 	a.recs[at] = WriteRec{bmask, vmask, value, op};
