@@ -299,7 +299,18 @@ int ufo_b200_write_compressed(ufo_b200_map* m, const double* box6, uint32_t min_
  * this map's resolution / depth_levels (the reference clears and resizes otherwise: call
  * ufo_b200_clear_resize first).  compressed != 0: `data` is one LZ4 block of uncompressed_size
  * bytes.  A collapsed non-default node above the brick level is expanded into bricks (at most 2^20
- * per call, else UFO_B200_E_UNSUPPORTED). */
+ * per call, else UFO_B200_E_UNSUPPORTED).
+ * Routed maps (ufo_b200_route_setup): every rank takes the same call -- stream, box or volume,
+ * compressed flag and sizes -- and applies the part of the stream that falls in the bricks it owns;
+ * it creates no brick another rank owns.  The union of the ranks equals one map that read the same
+ * stream after the same history, and ufo_b200_image_part_bv / ufo_b200_image_assemble of the ranks
+ * give that map's image, so a map written by any number of ranks (or by one map) loads onto any
+ * number of ranks.  The 2^20 limit counts every brick of a node, owned or not.  Every rejection --
+ * a call between ufo_b200_route_mark and the last ufo_b200_route_apply of a pass, a truncated
+ * stream, a failed decompression, an invalid volume (UFO_B200_E_INVALID), depth_levels < 5 or the
+ * 2^20 limit (UFO_B200_E_UNSUPPORTED) -- is decided from the arguments before any device work, so
+ * every rank returns the same status and none changes.  Pools grow as on one map.  Sharded maps
+ * (ufo_b200_set_shard): UFO_B200_E_UNSUPPORTED. */
 int ufo_b200_read_data(ufo_b200_map* m, const double* box6, const void* data, size_t size, int compressed,
                        size_t uncompressed_size);
 
@@ -594,8 +605,8 @@ int ufo_b200_set_shard(ufo_b200_map* m, uint32_t rank, uint32_t world);
  * The union of the ranks' value fields equals the single-GPU map (tests/test_gpu_route.py,
  * tests/test_gpu_route_discrete.py).  Pools do not grow during a routed pass: size the map with
  * initial_bricks.  Maps that have seen out-of-tree keys are rejected.  Between passes the ranks
- * also take setValueVolume and write batches (each applies what it owns; pools grow there as on
- * one map), and ufo_b200_image_part_bv / ufo_b200_image_assemble give the union's file image. */
+ * also take setValueVolume, write batches and readData (each applies what it owns; pools grow there
+ * as on one map), and ufo_b200_image_part_bv / ufo_b200_image_assemble give the union's file image. */
 int ufo_b200_route_inbox_bytes(uint32_t world, uint32_t cap_bricks, uint32_t cap_hits, size_t* bytes);
 int ufo_b200_route_inbox_bytes_color(uint32_t world, uint32_t cap_bricks, uint32_t cap_hits, size_t* bytes);
 int ufo_b200_route_setup(ufo_b200_map* m, uint32_t rank, uint32_t world, uint32_t cap_bricks, uint32_t cap_hits,

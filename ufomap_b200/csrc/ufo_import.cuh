@@ -6,6 +6,11 @@
 // CTA each, default-payload nodes above the brick level wipe the existing bricks below them; the
 // depth 1-4 aggregates of every touched brick are then rebuilt from its leaves and the usual
 // propagation pass (k_upper_*) follows.
+//
+// On a routed map every rank takes the same stream and applies the records of the bricks it owns
+// (brick_owned): a foreign record is skipped before its brick is found or created, and a wipe
+// leaves the foreign bricks a rank holds alone, so the ranks keep disjoint bricks whose union is
+// the single map that read the stream.
 #pragma once
 
 #include "ufo_kernels.cuh"
@@ -20,14 +25,23 @@ struct ImportRec {
 	uint32_t pad;
 };
 
+// key of the brick that holds a record's first voxel
+UFO_HD uint64_t record_brick(unsigned long long code)
+{
+	const Key3 k = code_to_key(code);
+	return pack_key(k.x >> 4, k.y >> 4, k.z >> 4);
+}
+
 // records of depth 0..2: one thread each
 __global__ void __launch_bounds__(256) k_import_small(DeviceMap M, const ImportRec* recs, uint32_t n)
 {
 	for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
 		const ImportRec r = recs[i];
-		const Key3 k = code_to_key(r.code);
-		const uint32_t brick = brick_find_or_create(M, pack_key(k.x >> 4, k.y >> 4, k.z >> 4));
+		const uint64_t key = record_brick(r.code);
+		if (!brick_owned(M, key)) continue;
+		const uint32_t brick = brick_find_or_create(M, key);
 		if (brick == kNone) continue;
+		const Key3 k = code_to_key(r.code);
 		touch_brick(M, brick);
 		const size_t b = (size_t)brick * 64 + morton2(k.x >> 2, k.y >> 2, k.z >> 2);
 		float* leaf = M.leaf + b * 64;
@@ -61,8 +75,8 @@ __global__ void __launch_bounds__(64) k_import_bricks(DeviceMap M, const ImportR
 	for (uint32_t i = blockIdx.x; i < n; i += gridDim.x) {
 		const ImportRec r = recs[i];
 		if (threadIdx.x == 0) {
-			const Key3 k = code_to_key(r.code);
-			const uint32_t brick = brick_find_or_create(M, pack_key(k.x >> 4, k.y >> 4, k.z >> 4));
+			const uint64_t key = record_brick(r.code);
+			const uint32_t brick = brick_owned(M, key) ? brick_find_or_create(M, key) : kNone;
 			if (brick != kNone) touch_brick(M, brick);
 			s_brick = brick;
 		}
@@ -85,15 +99,17 @@ __global__ void __launch_bounds__(64) k_import_bricks(DeviceMap M, const ImportR
 }
 
 // nodes above the brick level: every EXISTING brick below one of them takes the node's payload
-// (for the default payload this is how a subtree is deleted).  One thread per (brick, block).
+// (for the default payload this is how a subtree is deleted).  One thread per (brick, block).  A
+// routed rank may hold empty foreign bricks (gathered by its fused walk); they stay empty.
 __global__ void __launch_bounds__(256) k_import_wipe(DeviceMap M, uint32_t n_bricks, const ImportRec* recs, uint32_t n)
 {
 	const size_t b = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
 	if (b >= (size_t)n_bricks * 64) return;
 	const uint32_t brick = (uint32_t)(b >> 6);
+	const uint64_t key = M.brick_key[brick];
 	uint32_t x, y, z;
-	unpack_key(M.brick_key[brick], x, y, z);
-	if ((x | y | z) & ~(M.g.key_mask >> 4)) return;
+	unpack_key(key, x, y, z);
+	if (((x | y | z) & ~(M.g.key_mask >> 4)) || !brick_owned(M, key)) return;
 	const unsigned long long code = key_to_code({x << 4, y << 4, z << 4});
 	for (uint32_t i = 0; i < n; ++i) {
 		const ImportRec r = recs[i];

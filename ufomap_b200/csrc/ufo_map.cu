@@ -3893,6 +3893,7 @@ struct ImportPlan {
 	uint32_t P = 4;
 	uint64_t budget = 1ull << 20;  // bricks a stream may create through collapsed nodes above the brick level
 	bool too_big = false;
+	uint32_t route_world = 1, route_rank = 0;  // a routed rank expands only the bricks it owns
 };
 
 void import_leaf(ImportPlan& plan, uint64_t code, uint32_t depth, float occ, uint32_t rgb)
@@ -3906,7 +3907,9 @@ void import_leaf(ImportPlan& plan, uint64_t code, uint32_t depth, float occ, uin
 		plan.bricks.push_back(r);
 	} else {
 		// existing bricks below the node take the payload; if it is not the default, the bricks that
-		// do not exist yet have to be created as well (the value field has no collapsed nodes)
+		// do not exist yet have to be created as well (the value field has no collapsed nodes).  The
+		// budget counts every brick of the node on every rank, so that all ranks of a routed map
+		// reach the same decision.
 		plan.wipe.push_back(r);
 		if (occ != 0.0f || rgb != 0u) {
 			const uint64_t nb = depth >= 11 ? ~0ull : 1ull << (3 * (depth - 4));
@@ -3915,7 +3918,11 @@ void import_leaf(ImportPlan& plan, uint64_t code, uint32_t depth, float occ, uin
 				return;
 			}
 			plan.budget -= nb;
-			for (uint64_t i = 0; i < nb; ++i) plan.bricks.push_back(ImportRec{code + (i << 12), 4u, occ, rgb, 0u});
+			for (uint64_t i = 0; i < nb; ++i) {
+				const uint64_t c = code + (i << 12);
+				if (plan.route_world <= 1 || brick_owner(record_brick(c), plan.route_world) == plan.route_rank)
+					plan.bricks.push_back(ImportRec{c, 4u, occ, rgb, 0u});
+			}
 		}
 	}
 }
@@ -3970,16 +3977,19 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
 		m->set_error("readData needs depth_levels >= 5");
 		return UFO_B200_E_UNSUPPORTED;
 	}
-	if (M.route_world > 1 || M.shard_world > 1) {
-		m->set_error("readData on a sharded / routed map is not supported");
+	if (M.shard_world > 1) {
+		m->set_error("readData on a sharded map is not supported");
 		return UFO_B200_E_UNSUPPORTED;
 	}
-	CK(cudaSetDevice(m->device));
-	finalize_scan(m);
+	// the stream is parsed and every rejection decided before any device work, so that the ranks
+	// of a routed map, which take the same call, reach the same status and a rejected call changes
+	// nothing
 	ImportPlan plan;
 	plan.g = &M.g;
 	plan.P = M.color ? 7 : 4;
 	plan.vol = vol;
+	plan.route_world = M.route_world;
+	plan.route_rank = M.route_rank;
 	const double c0[3] = {0.0, 0.0, 0.0};
 	if (!vol_hits(plan.vol, c0, M.g.half_size[M.g.depth_levels])) return UFO_B200_OK;  // no node intersects
 	StreamReader in{data, size};
@@ -4001,6 +4011,8 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
 		m->set_error("readData: a collapsed node above the brick level would expand into more than 2^20 bricks");
 		return UFO_B200_E_UNSUPPORTED;
 	}
+	CK(cudaSetDevice(m->device));
+	finalize_scan(m);
 	// the codes of a tree of L levels use 3L bits; the pools must hold the bricks the stream creates
 	cudaStream_t s = m->stream;
 	const size_t n_small = plan.small.size(), n_bricks = plan.bricks.size(), n_wipe = plan.wipe.size();
@@ -4060,6 +4072,10 @@ int ufo_b200_read_data_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_b
 {
 	if (!m || (!data && size)) return UFO_B200_E_INVALID;
 	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
+	if (m->route_stage == 1) {
+		m->set_error("readData between ufo_b200_route_mark and the last ufo_b200_route_apply of the pass");
+		return UFO_B200_E_INVALID;
+	}
 	return guarded(m, [&]() {
 		const Volume vol{as_records(bv), (uint32_t)n_bv};
 		if (!compressed) return import_stream(m, static_cast<const uint8_t*>(data), size, vol);
