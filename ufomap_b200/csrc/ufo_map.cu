@@ -574,6 +574,62 @@ void grow_pools(Map* m, uint32_t overflow, uint32_t want_bricks, uint32_t want_u
 	CK(cudaGetLastError());
 }
 
+// The host takes the device's brick and upper-node counts, also after a pass that a full pool cut
+// short: grow_pools rebuilds the hashes from these slots, so a repeated attempt must not hand them
+// out again.
+void keep_created(Map* m)
+{
+	m->n_bricks = std::min(m->h_ctr->n_bricks, m->M.brick_cap);
+	m->n_upper = std::min(m->h_ctr->n_upper, m->M.up_cap);
+}
+
+// A new scan id (brick stamps) and a new upper-node epoch (up_stamp).  Neither is ever 0: the
+// stamps are cleared to 0, and an id of 0 would make every brick or node look already listed.
+void new_scan_id(Map* m) { if (++m->M.scan_id == 0) m->M.scan_id = 1; }
+void new_up_epoch(Map* m) { if (++m->M.up_epoch == 0) m->M.up_epoch = 1; }
+
+// depth 3 / 4 of the touched bricks from their blocks
+void launch_brick_agg(Map* m)
+{
+	if (m->M.color) k_brick_agg<true><<<m->sm_count * 4, 256, 0, m->stream>>>(m->M);
+	else k_brick_agg<false><<<m->sm_count * 4, 256, 0, m->stream>>>(m->M);
+}
+
+// every derived value of the touched bricks (depth 1 to 4) from their leaves
+void launch_leaf_refresh(Map* m)
+{
+	k_import_refresh<<<m->sm_count * 8, 256, 0, m->stream>>>(m->M);
+	launch_brick_agg(m);
+}
+
+// Runs a pass whose kernels find or create bricks and upper nodes, growing the pools until it
+// completes; `attempt` enqueues the pass's kernels.  Creation is idempotent, so a pass that ran
+// into a full pool is repeated as a whole, keeping what the failed attempt created.  Leaves the
+// final counts in m->n_bricks and m->n_upper.
+template <class F>
+int run_growing(Map* m, const char* what, F&& attempt)
+{
+	for (int k = 0;; ++k) {
+		push_counters(m);
+		attempt();
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(m->h_ctr, m->M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, m->stream));
+		CK(cudaStreamSynchronize(m->stream));
+		keep_created(m);
+		const uint32_t ov = m->h_ctr->overflow;
+		if (!ov) return UFO_B200_OK;
+		if (ov & ~6u) {
+			m->set_error("%s: internal error (overflow flags %u)", what, ov);
+			return UFO_B200_E_NOMEM;
+		}
+		if (k > 16) {
+			m->set_error("%s: device pools keep overflowing", what);
+			return UFO_B200_E_NOMEM;
+		}
+		grow_pools(m, ov, m->h_ctr->n_bricks, m->h_ctr->n_upper);
+	}
+}
+
 size_t layout_stride(int layout)
 {
 	switch (layout) {
@@ -1004,10 +1060,8 @@ void enqueue_write(Map* m, PendingScan& p)
 	DeviceMap& M = m->M;
 	cudaStream_t s = m->stream;
 	WriteArgs a = p.w;
-	M.scan_id++;
-	if (M.scan_id == 0) M.scan_id = 1;
-	M.up_epoch++;
-	if (M.up_epoch == 0) M.up_epoch = 1;
+	new_scan_id(m);
+	new_up_epoch(m);
 	M.dense = 0;
 	M.mask_base = M.miss_mask;
 	ensure_spare(m, m->d_w_seg, (size_t)M.brick_cap * 3 * sizeof(uint32_t), 1 << 12);
@@ -1036,9 +1090,7 @@ void enqueue_write(Map* m, PendingScan& p)
 	if (a.rgb) k_write_apply<true><<<m->sm_count * 16, 64, 0, s>>>(M, a);
 	else k_write_apply<false><<<m->sm_count * 16, 64, 0, s>>>(M, a);
 	CK(cudaEventRecord(m->ev[5], s));
-	k_import_refresh<<<m->sm_count * 8, 256, 0, s>>>(M);
-	if (M.color) k_brick_agg<true><<<m->sm_count * 4, 256, 0, s>>>(M);
-	else k_brick_agg<false><<<m->sm_count * 4, 256, 0, s>>>(M);
+	launch_leaf_refresh(m);
 	m->launches += 6;  // the sort's own launches not counted
 	launch_upper(m);
 	CK(cudaGetLastError());
@@ -1094,10 +1146,8 @@ void enqueue_scan(Map* m, PendingScan& p)
 	DeviceMap& M = m->M;
 	cudaStream_t s = m->stream;
 	ScanArgs& a = p.a;
-	M.scan_id++;
-	if (M.scan_id == 0) M.scan_id = 1;
-	M.up_epoch++;
-	if (M.up_epoch == 0) M.up_epoch = 1;
+	new_scan_id(m);
+	new_up_epoch(m);
 	const bool fused = use_fused(m, p);
 	M.dense = (fused && p.dense) ? 1u : 0u;
 	M.mask_base = M.dense ? M.vol : M.miss_mask;
@@ -1148,8 +1198,7 @@ void enqueue_scan(Map* m, PendingScan& p)
 	if (aliases) {
 		k_alias_apply<<<agrid, 256, 0, s>>>(M, a.miss, 0);
 		k_alias_refresh<<<agrid, 256, 0, s>>>(M);
-		if (M.color) k_brick_agg<true><<<agrid, 256, 0, s>>>(M);
-		else k_brick_agg<false><<<agrid, 256, 0, s>>>(M);
+		launch_brick_agg(m);
 		m->launches += 3;
 	}
 	if (m->profiling) CK(cudaEventRecord(m->ev[5], s));
@@ -1200,25 +1249,20 @@ void finalize_scan(Map* m)
 			throw MapError{(ov & 128u) ? UFO_B200_E_UNSUPPORTED : ((ov & 16u) ? UFO_B200_E_CUDA : UFO_B200_E_NOMEM)};
 		}
 		try {
+			keep_created(m);
 			if (ov == 4u) {
 				// only the upper-node pool overflowed: the leaves are updated, repeat the propagation
-				const uint32_t nu = std::min(m->h_ctr->n_upper, M.up_cap);
 				grow_pools(m, 4u, 0, m->h_ctr->n_upper);
-				M.up_epoch++;
-				k_reset_upper_pass<<<1, 1, 0, m->stream>>>(M.ctr, nu);
+				new_up_epoch(m);
+				k_reset_upper_pass<<<1, 1, 0, m->stream>>>(M.ctr, m->n_upper);
 				launch_upper(m);
 				CK(cudaEventRecord(m->ev[6], m->stream));
 				CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, m->stream));
-			} else if (p.write) {
-				// a brick could not be created while expanding: nothing was applied, grow and repeat
-				m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
-				grow_pools(m, ov & 6u, m->h_ctr->n_bricks, m->h_ctr->n_upper);
-				enqueue_scan(m, p);
 			} else {
-				// an allocation failed while marking: nothing was consumed (K3/K4 backed off).  Grow,
-				// keep the bricks that were created, and run the whole scan again under a new scan id
-				// (marking is idempotent: OR into masks, find-or-create of bricks).
-				m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
+				// an allocation failed while marking a scan or expanding a write batch: nothing was
+				// consumed (every later kernel backed off).  Grow and run the whole pass again under a
+				// new scan id (marking is idempotent: OR into masks, find-or-create of bricks).  Only
+				// scans set the flags other than 2 and 4.
 				if (ov & 64u) {
 					// a mark fell outside the scan volume (cannot happen for rays within max_range; kept
 					// as a safety net): wipe the volume and repeat through the brick hash
@@ -1238,7 +1282,7 @@ void finalize_scan(Map* m)
 				}
 				const bool fused = use_fused(m, p);
 				if (ov & 256u) ensure_early(m, p.a.n, m->h_ctr->e_visits);  // the walks need more ids / table slots
-				if (!fused && !p.simple && !p.has_vol && !p.early) {
+				if (!p.write && !fused && !p.simple && !p.has_vol && !p.early) {
 					ensure_scan_buffers(m, p.a.n, false, true, false);
 					unsigned long long want = std::max<unsigned long long>(m->h_ctr->seg_total + m->h_ctr->seg_total / 4 + 1024,
 					                                                        std::max<unsigned long long>(p.a.n, 1024) * 48ull);
@@ -1303,14 +1347,12 @@ void rebuild_flags(Map* m)
 	if (!m->n_bricks) return;
 	DeviceMap& M = m->M;
 	cudaStream_t s = m->stream;
-	M.scan_id++;
-	if (M.scan_id == 0) M.scan_id = 1;
-	M.up_epoch++;
+	new_scan_id(m);
+	new_up_epoch(m);
 	push_counters(m);
 	k_touch_all<<<m->sm_count, 256, 0, s>>>(M, m->n_bricks);
 	k_reflag<<<m->sm_count * 8, 256, 0, s>>>(M, m->n_bricks);
-	if (M.color) k_brick_agg<true><<<m->sm_count * 4, 256, 0, s>>>(M);
-	else k_brick_agg<false><<<m->sm_count * 4, 256, 0, s>>>(M);
+	launch_brick_agg(m);
 	launch_upper(m);
 	CK(cudaStreamSynchronize(s));
 }
@@ -1574,8 +1616,7 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 	CK(cudaEventRecord(m->ev[0], s));
 	CK(cudaMemcpyAsync(M.route, m->h_route, sizeof(RouteTable), cudaMemcpyHostToDevice, s));
 	if (copied) CK(cudaStreamWaitEvent(s, m->ev_copied, 0));
-	M.scan_id += 1;
-	if (M.scan_id == 0) M.scan_id = 1;
+	new_scan_id(m);
 	push_counters(m);
 	if (p.need_table) {
 		CK(cudaMemsetAsync(m->d_tab_keys.p, 0xff, (size_t)m->tab_size * sizeof(unsigned long long), s));
@@ -1632,15 +1673,13 @@ int do_route_apply(Map* m, uint32_t first, uint32_t count, int last)
 	// every apply call is a scan of its own as far as the touched list goes: the first one starts
 	// from the own bricks that kept local marks (list built by k_outbox under scan id + 1), the
 	// following ones from an empty list
-	M.scan_id += 1;
-	if (M.scan_id == 0) M.scan_id = 1;
+	new_scan_id(m);
 	if (!p.applying) {
 		std::swap(M.touched, M.touched_alt);
 		std::swap(M.touched_mi, M.touched_alt_mi);
 		M.dense = 0;
 		M.mask_base = M.miss_mask;
-		M.up_epoch++;
-		if (M.up_epoch == 0) M.up_epoch = 1;
+		new_up_epoch(m);
 		p.applying = true;
 	} else {
 		CK(cudaMemsetAsync(&M.ctr->n_touched, 0, sizeof(uint32_t), s));
@@ -4031,37 +4070,19 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
 		CK(cudaMemcpyAsync(d_wipe, plan.wipe.data(), n_wipe * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
 	}
 	set_value_floor(m, -INFINITY);  // the stream's values are not clamped to this map's sensor model
-	for (int attempt = 0;; ++attempt) {
-		M.scan_id++;
-		if (M.scan_id == 0) M.scan_id = 1;
-		M.up_epoch++;
+	// writing leaves is idempotent: a grown pool runs the whole import again
+	return run_growing(m, "readData", [&]() {
+		new_scan_id(m);
+		new_up_epoch(m);
 		M.dense = 0;
 		M.mask_base = M.miss_mask;
-		push_counters(m);
 		if (n_wipe && m->n_bricks)
 			k_import_wipe<<<(uint32_t)(((size_t)m->n_bricks * 64 + 255) / 256), 256, 0, s>>>(M, m->n_bricks, d_wipe, (uint32_t)n_wipe);
 		if (n_bricks) k_import_bricks<<<(uint32_t)std::min<size_t>(n_bricks, (size_t)m->sm_count * 16), 64, 0, s>>>(M, d_bricks, (uint32_t)n_bricks);
 		if (n_small) k_import_small<<<m->sm_count * 8, 256, 0, s>>>(M, d_small, (uint32_t)n_small);
-		k_import_refresh<<<m->sm_count * 8, 256, 0, s>>>(M);
-		if (M.color) k_brick_agg<true><<<m->sm_count * 4, 256, 0, s>>>(M);
-		else k_brick_agg<false><<<m->sm_count * 4, 256, 0, s>>>(M);
+		launch_leaf_refresh(m);
 		launch_upper(m);
-		CK(cudaGetLastError());
-		CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
-		CK(cudaStreamSynchronize(s));
-		const uint32_t ov = m->h_ctr->overflow;
-		if (!ov) break;
-		if (attempt > 16) {
-			m->set_error("readData: device pools keep overflowing");
-			return UFO_B200_E_NOMEM;
-		}
-		// writing leaves is idempotent: grow and run the whole import again
-		m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
-		grow_pools(m, ov & 6u, m->h_ctr->n_bricks, m->h_ctr->n_upper);
-	}
-	m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
-	m->n_upper = std::min(m->h_ctr->n_upper, M.up_cap);
-	return UFO_B200_OK;
+	});
 }
 }  // namespace
 
@@ -4505,32 +4526,16 @@ void fill_pool_state(Map* m, uint64_t& bricks, uint64_t& cap, uint64_t& bytes)
 // own depth 1-4 values from their leaves, as an import does.
 void page_propagate(Map* m, const uint32_t* d_slot, uint32_t n, bool derived)
 {
-	DeviceMap& M = m->M;
-	cudaStream_t s = m->stream;
-	for (int attempt = 0;; ++attempt) {
-		M.up_epoch++;
-		push_counters(m);
-		k_page_touch<<<std::max(1u, std::min((n + 255) / 256, (uint32_t)m->sm_count * 4)), 256, 0, s>>>(M, d_slot, n);
-		if (derived) {
-			k_import_refresh<<<m->sm_count * 8, 256, 0, s>>>(M);
-			if (M.color) k_brick_agg<true><<<m->sm_count * 4, 256, 0, s>>>(M);
-			else k_brick_agg<false><<<m->sm_count * 4, 256, 0, s>>>(M);
-		}
+	const int rc = run_growing(m, "upper-node propagation", [&]() {
+		new_up_epoch(m);
+		k_page_touch<<<std::max(1u, std::min((n + 255) / 256, (uint32_t)m->sm_count * 4)), 256, 0, m->stream>>>(m->M, d_slot, n);
+		if (derived) launch_leaf_refresh(m);
 		launch_upper(m);
-		CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
-		CK(cudaStreamSynchronize(s));
-		const uint32_t ov = m->h_ctr->overflow;
-		if (!ov) break;
-		if (attempt > 16 || (ov & ~4u)) {
-			m->set_error("the upper-node pool keeps overflowing (flags %u)", ov);
-			m->poisoned = true;
-			throw MapError{UFO_B200_E_NOMEM};
-		}
-		// every step above is idempotent: keep the nodes that were created, grow and run it again
-		m->n_upper = std::min(m->h_ctr->n_upper, M.up_cap);
-		grow_pools(m, 4u, 0, m->h_ctr->n_upper);
+	});
+	if (rc != UFO_B200_OK) {
+		m->poisoned = true;
+		throw MapError{rc};
 	}
-	m->n_upper = std::min(m->h_ctr->n_upper, M.up_cap);
 }
 
 int retain(Map* m, const Volume& vol, ufo_b200_retain_stats* out)
@@ -4782,22 +4787,11 @@ int page_in(Map* m, const void* blob, size_t size, ufo_b200_retain_stats* out)
 	}
 	// Every brick first, nothing written until all exist: creation is idempotent, so a pass that
 	// ran into a full pool is repeated as a whole after the pool has grown.
-	for (int attempt = 0;; ++attempt) {
-		push_counters(m);
+	const int rc = run_growing(m, "page_in", [&]() {
 		k_page_create<<<(n + 255) / 256, 256, 0, s>>>(M, d_keys, n, d_slot);
-		CK(cudaGetLastError());
 		++m->launches;
-		CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
-		CK(cudaStreamSynchronize(s));
-		const uint32_t ov = m->h_ctr->overflow;
-		m->n_bricks = std::min(m->h_ctr->n_bricks, M.brick_cap);
-		if (!ov) break;
-		if (attempt > 16) {
-			m->set_error("page_in: device pools keep overflowing");
-			return UFO_B200_E_NOMEM;
-		}
-		grow_pools(m, ov & 6u, m->h_ctr->n_bricks, m->h_ctr->n_upper);
-	}
+	});
+	if (rc != UFO_B200_OK) return rc;
 	CK(cudaEventRecord(ev.e[1], s));
 	{
 		PageStage stage;
