@@ -314,6 +314,53 @@ int ufo_b200_write_compressed(ufo_b200_map* m, const double* box6, uint32_t min_
 int ufo_b200_read_data(ufo_b200_map* m, const double* box6, const void* data, size_t size, int compressed,
                        size_t uncompressed_size);
 
+/* The text header of a UFOMap file image (Octree::readHeader, octree.h:1338-1417).  Layout, 96 bytes:
+ *   offset  0  char version[32]                 the version token, NUL-terminated (first 31 bytes)
+ *   offset 32  char id[32]                      the id token (tree type), NUL-terminated (first 31 bytes)
+ *   offset 64  double resolution
+ *   offset 72  uint32_t depth_levels
+ *   offset 76  int32_t compressed               0 or 1
+ *   offset 80  int64_t uncompressed_data_size   -1 when the header has none
+ *   offset 88  uint64_t data_offset             the byte offset of the node stream in the image; 0
+ *                                               when no "data" line was found */
+typedef struct {
+	char version[32];
+	char id[32];
+	double resolution;
+	uint32_t depth_levels;
+	int32_t compressed;
+	int64_t uncompressed_data_size;
+	uint64_t data_offset;
+} ufo_b200_file_header;
+
+/* Octree::readHeader on an image (the whole file, or any prefix that holds its header); needs no
+ * map and no device.  The first line must start with "# UFOMap file"; then whitespace-separated
+ * tokens: a token starting with '#' and an unknown token skip to the end of their line, "data" ends
+ * the header at the end of its line, and version, id, resolution, depth_levels, compressed (0 or 1)
+ * and uncompressed_data_size take the token after them, numbers as an istream reads them.
+ * UFO_B200_E_INVALID, as the reference returns false: a first line without the file mark, no "data"
+ * line, an empty version or id, resolution <= 0, depth_levels 0, a negative or missing
+ * uncompressed_data_size, or a value the stream cannot read.  *out holds what was read either way:
+ * its id is what Octree::readType returns (empty when the first line is not the file mark). */
+int ufo_b200_read_header(const void* image, size_t size, ufo_b200_file_header* out);
+
+/* Octree::read (octree.h:690-729) of a file image -- header, then the node stream -- or of the file
+ * `filename`.  The header's id must be the map's tree type ("occupancy_map" / "occupancy_map_color",
+ * as the writers put it).  A file of another resolution or depth_levels re-creates the map with the
+ * file's (ufo_b200_clear_resize), as the reference's readData does (octree.h:760-762); a file of the
+ * same geometry merges into the map like ufo_b200_read_data.  A compressed file ("compressed 1") is
+ * one LZ4 block, decompressed once (the reference decompresses it a second time and so cannot read
+ * its own compressed files, DESIGN.md section 7).  Every rejection is decided before the map is
+ * touched, so a rejected call changes nothing (the reference clears the map before it parses):
+ * an invalid header, a tree type other than the map's, depth_levels above 21 (UFO_B200_E_INVALID);
+ * depth_levels < 5 (UFO_B200_E_UNSUPPORTED); a file that cannot be opened or read, a failed
+ * decompression, a truncated stream (UFO_B200_E_INVALID); the limits of ufo_b200_read_data.
+ * Routed maps: every rank takes the same call as for ufo_b200_read_data; a file whose geometry
+ * differs from the map's is refused on every rank (UFO_B200_E_UNSUPPORTED), since a rank cannot
+ * re-create a routed map on its own. */
+int ufo_b200_read(ufo_b200_map* m, const void* image, size_t size);
+int ufo_b200_read_file(ufo_b200_map* m, const char* filename);
+
 /* Bounding volumes (ufo::geometry::BoundingVolume, geometry/bounding_volume.h): a union of shapes,
  * each one ufo_b200_volume.  type follows the order of ufo::geometry::BoundingVar
  * (geometry/types.h); v holds the shape's members as the reference stores them:

@@ -550,6 +550,16 @@ class MapFacade
 			throw std::runtime_error("ufomap_b200: no usable CUDA device (there is no CPU fallback)");
 		}
 	}
+	// The file constructors (occupancy_map_base.h:878-886): a map of resolution 0.1 and 16 depth
+	// levels that then reads the file.  A failed read leaves that map and its status in lastStatus().
+	MapFacade(std::string const& filename, bool automatic_pruning = true, double occupied_thres = 0.5,
+	          double free_thres = 0.5, double prob_hit = 0.7, double prob_miss = 0.4,
+	          double clamping_thres_min = 0.1192, double clamping_thres_max = 0.971)
+	    : MapFacade(0.1, 16, automatic_pruning, occupied_thres, free_thres, prob_hit, prob_miss, clamping_thres_min,
+	                clamping_thres_max)
+	{
+		read(filename);
+	}
 	MapFacade(MapFacade const&) = delete;
 	MapFacade& operator=(MapFacade const&) = delete;
 	virtual ~MapFacade() { ufo_b200_destroy(map_); }
@@ -903,6 +913,53 @@ class MapFacade
 		if (UFO_B200_OK != ufo_b200_write_data_bv(map_, bv.data(), bv.size(), min_depth, data.data(), n, &n)) return -1;
 		s.write(data.data(), (std::streamsize)n);
 		return s.good() ? (int)n : -1;
+	}
+
+	// Octree::readType (octree.h:639-688): the id of a file's header, "" when the first line is not
+	// the file mark or the file cannot be opened.  Reads the stream up to the end of its header.
+	static std::string readType(std::string const& filename)
+	{
+		std::ifstream file(filename.c_str(), std::ios_base::in | std::ios_base::binary);
+		return file.is_open() ? readType(file) : std::string();
+	}
+	static std::string readType(std::istream& s)
+	{
+		std::string head;
+		char buf[4096];
+		ufo_b200_file_header h;
+		while (s.good()) {
+			s.read(buf, sizeof buf);
+			head.append(buf, (std::size_t)s.gcount());
+			ufo_b200_read_header(head.data(), head.size(), &h);
+			if (h.data_offset && h.data_offset < head.size()) return h.id;  // the "data" line is complete
+		}
+		ufo_b200_read_header(head.data(), head.size(), &h);
+		return h.id;
+	}
+
+	// Octree::read (octree.h:690-729): the file image (header + node stream) into the map.  A file of
+	// another resolution / depth_levels re-creates the map with the file's (ufo_b200_read); a failed
+	// read changes nothing and leaves its status in lastStatus().
+	bool read(std::string const& filename)
+	{
+		std::ifstream file(filename.c_str(), std::ios_base::in | std::ios_base::binary);
+		if (!file.is_open()) {
+			last_status_ = UFO_B200_E_INVALID;
+			return false;
+		}
+		return read(file);
+	}
+	bool read(std::istream& s)
+	{
+		std::vector<char> image((std::istreambuf_iterator<char>(s)), std::istreambuf_iterator<char>());
+		last_status_ = ufo_b200_read(map_, image.data(), image.size());
+		if (UFO_B200_OK != last_status_) return false;
+		ufo_b200_file_header h;
+		ufo_b200_read_header(image.data(), image.size(), &h);
+		// the geometry getters read params_
+		params_.resolution = h.resolution;
+		params_.depth_levels = h.depth_levels;
+		return true;
 	}
 
 	// Octree::readData with a BoundingVolume (octree.h:751-774; msgToUfo, conversions.h:122-134)

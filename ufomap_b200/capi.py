@@ -92,6 +92,13 @@ class PageHeader(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved"}
 
 
+class FileHeader(C.Structure):
+    """ufo_b200_file_header: the text header of a UFOMap file image."""
+    _fields_ = [("version", C.c_char * 32), ("id", C.c_char * 32), ("resolution", C.c_double),
+                ("depth_levels", C.c_uint32), ("compressed", C.c_int32), ("uncompressed_data_size", C.c_int64),
+                ("data_offset", C.c_uint64)]
+
+
 class PoolCounts(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("bricks", "brick_cap", "upper_nodes", "up_cap", "device_bytes")]
 
@@ -125,6 +132,7 @@ SYMBOLS = [
     "ufo_b200_iterate", "ufo_b200_update_nodes_color",
     "ufo_b200_retain_bv", "ufo_b200_retain", "ufo_b200_page_out_bv", "ufo_b200_page_in", "ufo_b200_page_info",
     "ufo_b200_pool_stats", "ufo_b200_last_update_stats", "ufo_b200_image_part_bv", "ufo_b200_image_assemble",
+    "ufo_b200_read_header", "ufo_b200_read", "ufo_b200_read_file",
 ]
 
 # ufo_b200_volume: one shape of a bounding volume (type in BoundingVar order, members in v)
@@ -315,6 +323,9 @@ def load():
     lib.ufo_b200_write_data_bv.argtypes = [vp, vp, sz, u32, vp, sz, C.POINTER(sz)]
     lib.ufo_b200_write_compressed_bv.argtypes = [vp, vp, sz, u32, i32, i32, i32, vp, sz, C.POINTER(sz), C.POINTER(sz)]
     lib.ufo_b200_read_data_bv.argtypes = [vp, vp, sz, vp, sz, i32, sz]
+    lib.ufo_b200_read_header.argtypes = [vp, sz, C.POINTER(FileHeader)]
+    lib.ufo_b200_read.argtypes = [vp, vp, sz]
+    lib.ufo_b200_read_file.argtypes = [vp, C.c_char_p]
     lib.ufo_b200_image_part_bv.argtypes = [vp, vp, sz, u32, i32, vp, sz, C.POINTER(sz)]
     lib.ufo_b200_image_assemble.argtypes = [C.POINTER(vp), C.POINTER(sz), sz, i32, i32, i32, i32, vp, sz,
                                             C.POINTER(sz), C.POINTER(sz)]
@@ -363,6 +374,20 @@ def pack_points(xyz, rgb=None, dtype=np.float64):
     buf[:, :12] = np.ascontiguousarray(xyz, dtype=np.float32).reshape(n, 3).view(np.uint8).reshape(n, 12)
     buf[:, 12:15] = rgb
     return buf, XYZRGB_F32
+
+
+def read_header(image):
+    """Octree::readHeader of a file image (bytes, or a prefix holding the header): (ok, fields).
+    fields: version, id, resolution, depth_levels, compressed, uncompressed_data_size and
+    data_offset (the node stream's first byte), as far as they were read; id is what
+    Octree::readType returns."""
+    buf = np.frombuffer(image, np.uint8)
+    h = FileHeader()
+    rc = load().ufo_b200_read_header(buf.ctypes.data if len(buf) else None, len(buf), C.byref(h))
+    fields = dict(version=h.version.decode(), id=h.id.decode(), resolution=h.resolution,
+                  depth_levels=int(h.depth_levels), compressed=bool(h.compressed),
+                  uncompressed_data_size=int(h.uncompressed_data_size), data_offset=int(h.data_offset))
+    return rc == OK, fields
 
 
 class Map:
@@ -599,6 +624,41 @@ class Map:
         self._check(self.lib.ufo_b200_read_data(self.h, None if b is None else b.ctypes.data,
                                                 buf.ctypes.data if len(buf) else None, len(buf), int(compressed),
                                                 int(uncompressed_size)))
+
+    def read(self, image):
+        """Octree::read of a file image (bytes): a file of another resolution / depth_levels
+        re-creates the map with the file's, one of the same merges into it."""
+        buf = np.frombuffer(image, np.uint8)
+        self._check(self.lib.ufo_b200_read(self.h, buf.ctypes.data if len(buf) else None, len(buf)))
+        self._geometry_from(image[:1 << 16])
+
+    def read_file(self, filename):
+        """Octree::read(filename)."""
+        self._check(self.lib.ufo_b200_read_file(self.h, os.fsencode(filename)))
+        with open(filename, "rb") as f:
+            self._geometry_from(f.read(1 << 16))
+
+    def _geometry_from(self, head):
+        ok, h = read_header(head)
+        if ok:
+            self.resolution, self.depth_levels = h["resolution"], h["depth_levels"]
+
+    @classmethod
+    def open(cls, filename, device=-1, **kwargs):
+        """A new map of the file's tree type, read from the file (the file constructors
+        OccupancyMap(filename) / OccupancyMapColor(filename))."""
+        with open(filename, "rb") as f:
+            ok, h = read_header(f.read(1 << 16))
+        if h["id"] not in ("occupancy_map", "occupancy_map_color"):
+            raise ValueError("%s: not a UFOMap file of a known tree type" % filename)
+        m = cls(h["resolution"] if ok else 0.1, h["depth_levels"] if ok and 5 <= h["depth_levels"] <= 21 else 16,
+                color=h["id"] == "occupancy_map_color", device=device, **kwargs)
+        try:
+            m.read_file(filename)
+        except Exception:
+            m.close()
+            raise
+        return m
 
     def write_file(self, filename, expanded=False, box=None, min_depth=0):
         b = self._box6(box)

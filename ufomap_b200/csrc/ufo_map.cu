@@ -17,11 +17,13 @@
 
 #include <algorithm>
 #include <numeric>
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <string>
 #include <utility>
@@ -3907,61 +3909,120 @@ int ufo_b200_volume_intersects(const ufo_b200_volume* bv, size_t n_bv, const dou
 
 namespace
 {
+// the events of one call
+struct Events {
+	cudaEvent_t e[4] = {};
+	Events()
+	{
+		for (auto& x : e) CK(cudaEventCreate(&x));
+	}
+	Events(const Events&) = delete;
+	Events& operator=(const Events&) = delete;
+	~Events()
+	{
+		for (auto& x : e)
+			if (x) cudaEventDestroy(x);
+	}
+};
+
+// Pinned staging for the sections of a page: two chunks of a bounded size on each side, so that the
+// host's copy of one chunk overlaps the device's work on the next and a page of any size needs
+// 2 x kPageChunk of pinned memory.
+constexpr size_t kPageChunk = 16u << 20;
+struct PageStage {
+	uint8_t* pin[2] = {};
+	DevBuf dev_buf[2];
+	uint8_t* dev[2] = {};
+	cudaEvent_t ev[2] = {};
+	PageStage()
+	{
+		for (int b = 0; b < 2; ++b) {
+			CK(cudaHostAlloc(reinterpret_cast<void**>(&pin[b]), kPageChunk, cudaHostAllocDefault));
+			dev[b] = dev_buf[b].alloc<uint8_t>(kPageChunk);
+			CK(cudaEventCreateWithFlags(&ev[b], cudaEventDisableTiming));
+		}
+	}
+	PageStage(const PageStage&) = delete;
+	PageStage& operator=(const PageStage&) = delete;
+	~PageStage()
+	{
+		for (int b = 0; b < 2; ++b) {
+			if (pin[b]) cudaFreeHost(pin[b]);
+			if (ev[b]) cudaEventDestroy(ev[b]);
+		}
+	}
+};
+
 struct StreamReader {
 	const uint8_t* p;
 	size_t n, at = 0;
 	bool ok = true;
-	bool get(void* out, size_t len)
+	bool skip(size_t len)
 	{
 		if (at + len > n) {
 			ok = false;
-			std::memset(out, 0, len);
 			at = n + 1;
 			return false;
 		}
-		std::memcpy(out, p + at, len);
 		at += len;
+		return true;
+	}
+	bool get(void* out, size_t len)
+	{
+		const size_t from = at;
+		if (!skip(len)) {
+			std::memset(out, 0, len);
+			return false;
+		}
+		std::memcpy(out, p + from, len);
 		return true;
 	}
 };
 
+// a depth-4 node with children: its bytes in the stream
+struct SubStream {
+	unsigned long long code;
+	size_t at;
+	uint32_t len;
+};
+
 struct ImportPlan {
-	std::vector<ImportRec> small, bricks, wipe;  // depth <= 2, depth 4, depth >= 5
-	const Geometry* g = nullptr;
+	std::vector<ImportRec> bricks, wipe;  // depth 4, depth >= 5
+	std::vector<SubStream> subs;          // of the bricks this map owns, in stream order
+	std::vector<size_t> cuts;             // upload chunk k holds subs[cuts[k], cuts[k + 1])
+	Geometry g{};
 	Volume vol{nullptr, 0, {}, {}};  // host records
 	uint32_t P = 4;
 	uint64_t budget = 1ull << 20;  // bricks a stream may create through collapsed nodes above the brick level
 	bool too_big = false;
+	bool none = false;  // the volume misses the root: nothing to read
 	uint32_t route_world = 1, route_rank = 0;  // a routed rank expands only the bricks it owns
+	bool owns(uint64_t brick_key) const { return route_world <= 1 || brick_owner(brick_key, route_world) == route_rank; }
 };
 
+// a leaf at depth >= 4 (the walk hands the levels below to k_import_parse)
 void import_leaf(ImportPlan& plan, uint64_t code, uint32_t depth, float occ, uint32_t rgb)
 {
 	const ImportRec r{code, depth, occ, rgb, 0u};
-	if (depth <= 2) {
-		plan.small.push_back(r);
-	} else if (depth == 3) {
-		for (uint64_t i = 0; i < 8; ++i) plan.small.push_back(ImportRec{code + (i << 6), 2u, occ, rgb, 0u});
-	} else if (depth == 4) {
+	if (depth == 4) {
 		plan.bricks.push_back(r);
-	} else {
-		// existing bricks below the node take the payload; if it is not the default, the bricks that
-		// do not exist yet have to be created as well (the value field has no collapsed nodes).  The
-		// budget counts every brick of the node on every rank, so that all ranks of a routed map
-		// reach the same decision.
-		plan.wipe.push_back(r);
-		if (occ != 0.0f || rgb != 0u) {
-			const uint64_t nb = depth >= 11 ? ~0ull : 1ull << (3 * (depth - 4));
-			if (nb > plan.budget) {
-				plan.too_big = true;
-				return;
-			}
-			plan.budget -= nb;
-			for (uint64_t i = 0; i < nb; ++i) {
-				const uint64_t c = code + (i << 12);
-				if (plan.route_world <= 1 || brick_owner(record_brick(c), plan.route_world) == plan.route_rank)
-					plan.bricks.push_back(ImportRec{c, 4u, occ, rgb, 0u});
-			}
+		return;
+	}
+	// existing bricks below the node take the payload; if it is not the default, the bricks that
+	// do not exist yet have to be created as well (the value field has no collapsed nodes).  The
+	// budget counts every brick of the node on every rank, so that all ranks of a routed map
+	// reach the same decision.
+	plan.wipe.push_back(r);
+	if (occ != 0.0f || rgb != 0u) {
+		const uint64_t nb = depth >= 11 ? ~0ull : 1ull << (3 * (depth - 4));
+		if (nb > plan.budget) {
+			plan.too_big = true;
+			return;
+		}
+		plan.budget -= nb;
+		for (uint64_t i = 0; i < nb; ++i) {
+			const uint64_t c = code + (i << 12);
+			if (plan.owns(record_brick(c))) plan.bricks.push_back(ImportRec{c, 4u, occ, rgb, 0u});
 		}
 	}
 }
@@ -3974,11 +4035,70 @@ void read_payload(StreamReader& in, uint32_t P, float& occ, uint32_t& rgb)
 	rgb = P == 7 ? ((uint32_t)b[4] | ((uint32_t)b[5] << 8) | ((uint32_t)b[6] << 16)) : 0u;
 }
 
-// readNodesRecurs (occupancy_map_base.h:1403-1456): `code` = first voxel of the node of depth `depth`
+// The bytes of the depth-4 node with children at in.at (first voxel `code`, centre c): reads its
+// children bytes only and steps over the payloads, whose number the children bytes and the volume
+// decide (readNodesRecurs reads no bytes for a child whose cube misses the volume).  Without a
+// volume no cube is tested and a depth-2 node costs one step.
+void walk_brick(ImportPlan& plan, StreamReader& in, uint64_t code, const double c[3])
+{
+	const size_t at0 = in.at;
+	const uint32_t P = plan.P;
+	const bool filtered = plan.vol.n != 0;
+	const double* hs = plan.g.half_size;
+	auto hits = [&](const double* pc, uint32_t d, uint32_t i, double out[3]) {
+		if (!filtered) return true;
+		child_center(pc, hs[d], i, out);
+		return vol_hits(plan.vol, out, hs[d]);
+	};
+	uint8_t c4 = 0;
+	if (!in.get(&c4, 1)) return;
+	for (uint32_t j = 0; j < 8; ++j) {
+		double c3c[3];
+		if (!hits(c, 3, j, c3c)) continue;
+		if (!((c4 >> j) & 1u)) {
+			in.skip(P);
+			continue;
+		}
+		uint8_t c3 = 0;
+		if (!in.get(&c3, 1)) return;
+		for (uint32_t k = 0; k < 8; ++k) {
+			double c2c[3];
+			if (!hits(c3c, 2, k, c2c)) continue;
+			if (!((c3 >> k) & 1u)) {
+				in.skip(P);
+				continue;
+			}
+			uint8_t c2 = 0;
+			if (!in.get(&c2, 1)) return;
+			if (!filtered) {
+				in.skip((size_t)P * (8 + 7 * __builtin_popcount(c2)));
+				continue;
+			}
+			for (uint32_t o = 0; o < 8; ++o) {
+				double c1c[3];
+				if (!hits(c2c, 1, o, c1c)) continue;
+				if (!((c2 >> o) & 1u)) {
+					in.skip(P);
+					continue;
+				}
+				uint32_t nv = 0;
+				for (uint32_t v = 0; v < 8; ++v) {
+					double c0c[3];
+					nv += hits(c1c, 0, v, c0c) ? 1u : 0u;
+				}
+				in.skip((size_t)P * nv);
+			}
+		}
+	}
+	if (in.ok && plan.owns(record_brick(code))) plan.subs.push_back(SubStream{code, at0, (uint32_t)(in.at - at0)});
+}
+
+// readNodesRecurs (occupancy_map_base.h:1403-1456) above the brick level: `code` = first voxel of
+// the node of depth `depth` (> 4)
 void import_rec(ImportPlan& plan, StreamReader& in, uint64_t code, uint32_t depth, const double c[3])
 {
 	const uint32_t cd = depth - 1;
-	const double chs = plan.g->half_size[cd];
+	const double chs = plan.g.half_size[cd];
 	uint8_t children = 0;
 	if (!in.get(&children, 1)) return;
 	for (uint32_t i = 0; i < 8 && in.ok; ++i) {
@@ -3987,19 +4107,8 @@ void import_rec(ImportPlan& plan, StreamReader& in, uint64_t code, uint32_t dept
 		if (!vol_hits(plan.vol, cc, chs)) continue;
 		const uint64_t ccode = code + ((uint64_t)i << (3 * cd));
 		if ((children >> i) & 1u) {
-			if (1 == cd) {
-				for (uint32_t j = 0; j < 8; ++j) {
-					double gc[3];
-					child_center(cc, plan.g->half_size[0], j, gc);
-					if (!vol_hits(plan.vol, gc, plan.g->half_size[0])) continue;
-					float occ;
-					uint32_t rgb;
-					read_payload(in, plan.P, occ, rgb);
-					import_leaf(plan, ccode + j, 0, occ, rgb);
-				}
-			} else {
-				import_rec(plan, in, ccode, cd, cc);
-			}
+			if (cd == 4) walk_brick(plan, in, ccode, cc);
+			else import_rec(plan, in, ccode, cd, cc);
 		} else {
 			float occ;
 			uint32_t rgb;
@@ -4009,28 +4118,32 @@ void import_rec(ImportPlan& plan, StreamReader& in, uint64_t code, uint32_t dept
 	}
 }
 
-int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
+// Upload chunks: records, then the sub-streams, and the 16 bytes k_import_parse may read past the
+// last one (it copies whole 16-byte words), within one staging chunk.
+void cut_chunks(ImportPlan& plan)
 {
-	DeviceMap& M = m->M;
-	if (M.g.depth_levels < 5) {
-		m->set_error("readData needs depth_levels >= 5");
-		return UFO_B200_E_UNSUPPORTED;
+	plan.cuts.assign(1, 0);
+	size_t bytes = 16;
+	for (size_t i = 0; i < plan.subs.size(); ++i) {
+		const size_t add = sizeof(ImportSub) + plan.subs[i].len;
+		if (bytes + add > kPageChunk) {
+			plan.cuts.push_back(i);
+			bytes = 16;
+		}
+		bytes += add;
 	}
-	if (M.shard_world > 1) {
-		m->set_error("readData on a sharded map is not supported");
-		return UFO_B200_E_UNSUPPORTED;
-	}
-	// the stream is parsed and every rejection decided before any device work, so that the ranks
-	// of a routed map, which take the same call, reach the same status and a rejected call changes
-	// nothing
-	ImportPlan plan;
-	plan.g = &M.g;
-	plan.P = M.color ? 7 : 4;
-	plan.vol = vol;
-	plan.route_world = M.route_world;
-	plan.route_rank = M.route_rank;
+	if (!plan.subs.empty()) plan.cuts.push_back(plan.subs.size());
+}
+
+// The host part of readData: walks the stream with plan.g, plan.vol, plan.P and the routing set,
+// deciding every rejection before any device work.
+int plan_import(Map* m, ImportPlan& plan, const uint8_t* data, size_t size)
+{
 	const double c0[3] = {0.0, 0.0, 0.0};
-	if (!vol_hits(plan.vol, c0, M.g.half_size[M.g.depth_levels])) return UFO_B200_OK;  // no node intersects
+	if (!vol_hits(plan.vol, c0, plan.g.half_size[plan.g.depth_levels])) {  // no node intersects
+		plan.none = true;
+		return UFO_B200_OK;
+	}
 	StreamReader in{data, size};
 	uint8_t children = 0;
 	in.get(&children, 1);
@@ -4038,9 +4151,9 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
 		float occ;
 		uint32_t rgb;
 		read_payload(in, plan.P, occ, rgb);
-		import_leaf(plan, 0, M.g.depth_levels, occ, rgb);
+		import_leaf(plan, 0, plan.g.depth_levels, occ, rgb);
 	} else {
-		import_rec(plan, in, 0, M.g.depth_levels, c0);
+		import_rec(plan, in, 0, plan.g.depth_levels, c0);
 	}
 	if (!in.ok) {
 		m->set_error("readData: the node stream is truncated");
@@ -4050,17 +4163,41 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
 		m->set_error("readData: a collapsed node above the brick level would expand into more than 2^20 bricks");
 		return UFO_B200_E_UNSUPPORTED;
 	}
+	cut_chunks(plan);
+	return UFO_B200_OK;
+}
+
+// the checks of readData that need no stream; plan set up for this map
+int import_allowed(Map* m, uint32_t depth_levels, ImportPlan& plan, const Volume& vol)
+{
+	if (depth_levels < 5) {
+		m->set_error("readData needs depth_levels >= 5");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (m->M.shard_world > 1) {
+		m->set_error("readData on a sharded map is not supported");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	plan.P = m->M.color ? 7 : 4;
+	plan.vol = vol;
+	plan.route_world = m->M.route_world;
+	plan.route_rank = m->M.route_rank;
+	return UFO_B200_OK;
+}
+
+// The device part of readData.  The sub-streams travel in pinned chunks on the copy stream while
+// the map's stream parses the chunk before; writing leaves is idempotent, so a grown pool runs the
+// whole import again.
+int apply_import(Map* m, const ImportPlan& plan, const uint8_t* data)
+{
+	if (plan.none) return UFO_B200_OK;
+	DeviceMap& M = m->M;
 	CK(cudaSetDevice(m->device));
 	finalize_scan(m);
-	// the codes of a tree of L levels use 3L bits; the pools must hold the bricks the stream creates
 	cudaStream_t s = m->stream;
-	const size_t n_small = plan.small.size(), n_bricks = plan.bricks.size(), n_wipe = plan.wipe.size();
-	DevBuf b_small, b_bricks, b_wipe;
-	ImportRec *d_small = nullptr, *d_bricks = nullptr, *d_wipe = nullptr;
-	if (n_small) {
-		d_small = b_small.alloc<ImportRec>(n_small);
-		CK(cudaMemcpyAsync(d_small, plan.small.data(), n_small * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
-	}
+	const size_t n_bricks = plan.bricks.size(), n_wipe = plan.wipe.size();
+	DevBuf b_bricks, b_wipe;
+	ImportRec *d_bricks = nullptr, *d_wipe = nullptr;
 	if (n_bricks) {
 		d_bricks = b_bricks.alloc<ImportRec>(n_bricks);
 		CK(cudaMemcpyAsync(d_bricks, plan.bricks.data(), n_bricks * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
@@ -4069,8 +4206,20 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
 		d_wipe = b_wipe.alloc<ImportRec>(n_wipe);
 		CK(cudaMemcpyAsync(d_wipe, plan.wipe.data(), n_wipe * sizeof(ImportRec), cudaMemcpyHostToDevice, s));
 	}
+	Volume hv = plan.vol;
+	const bool general = volume_is_general(hv);
+	DeviceVolume dvol;
+	const Volume dv = dvol.upload(hv, s);
+	std::unique_ptr<PageStage> st;
+	Events ev;  // e[0..1]: chunk copied to the device, e[2..3]: chunk parsed
+	if (!plan.subs.empty()) st.reset(new PageStage());
+	auto parse = [&](uint32_t grid, const ImportSub* subs, uint32_t n, const uint8_t* bytes) {
+		if (M.color && general) k_import_parse<true, true><<<grid, 64, 0, s>>>(M, dv, subs, n, bytes);
+		else if (M.color) k_import_parse<true, false><<<grid, 64, 0, s>>>(M, dv, subs, n, bytes);
+		else if (general) k_import_parse<false, true><<<grid, 64, 0, s>>>(M, dv, subs, n, bytes);
+		else k_import_parse<false, false><<<grid, 64, 0, s>>>(M, dv, subs, n, bytes);
+	};
 	set_value_floor(m, -INFINITY);  // the stream's values are not clamped to this map's sensor model
-	// writing leaves is idempotent: a grown pool runs the whole import again
 	return run_growing(m, "readData", [&]() {
 		new_scan_id(m);
 		new_up_epoch(m);
@@ -4079,10 +4228,230 @@ int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
 		if (n_wipe && m->n_bricks)
 			k_import_wipe<<<(uint32_t)(((size_t)m->n_bricks * 64 + 255) / 256), 256, 0, s>>>(M, m->n_bricks, d_wipe, (uint32_t)n_wipe);
 		if (n_bricks) k_import_bricks<<<(uint32_t)std::min<size_t>(n_bricks, (size_t)m->sm_count * 16), 64, 0, s>>>(M, d_bricks, (uint32_t)n_bricks);
-		if (n_small) k_import_small<<<m->sm_count * 8, 256, 0, s>>>(M, d_small, (uint32_t)n_small);
+		for (size_t k = 0; k + 1 < plan.cuts.size(); ++k) {
+			const int b = (int)(k & 1);
+			const size_t first = plan.cuts[k], n = plan.cuts[k + 1] - first;
+			if (k >= 2) CK(cudaEventSynchronize(ev.e[b]));  // the pinned chunk has gone to the device
+			ImportSub* recs = reinterpret_cast<ImportSub*>(st->pin[b]);
+			uint8_t* bytes = st->pin[b] + n * sizeof(ImportSub);
+			uint32_t off = 0;
+			for (size_t i = 0; i < n; ++i) {
+				const SubStream& sub = plan.subs[first + i];
+				recs[i] = ImportSub{sub.code, off, sub.len};
+				memcpy(bytes + off, data + sub.at, sub.len);
+				off += sub.len;
+			}
+			if (k >= 2) CK(cudaStreamWaitEvent(m->copy_stream, ev.e[2 + b], 0));  // the device chunk is parsed
+			CK(cudaMemcpyAsync(st->dev[b], st->pin[b], n * sizeof(ImportSub) + off, cudaMemcpyHostToDevice, m->copy_stream));
+			CK(cudaEventRecord(ev.e[b], m->copy_stream));
+			CK(cudaStreamWaitEvent(s, ev.e[b], 0));
+			parse((uint32_t)std::min<size_t>(n, (size_t)m->sm_count * 7), reinterpret_cast<const ImportSub*>(st->dev[b]),
+			      (uint32_t)n, st->dev[b] + n * sizeof(ImportSub));
+			CK(cudaEventRecord(ev.e[2 + b], s));
+		}
 		launch_leaf_refresh(m);
 		launch_upper(m);
 	});
+}
+
+int import_stream(Map* m, const uint8_t* data, size_t size, const Volume& vol)
+{
+	// the stream is parsed and every rejection decided before any device work, so that the ranks
+	// of a routed map, which take the same call, reach the same status and a rejected call changes
+	// nothing
+	ImportPlan plan;
+	plan.g = m->M.g;
+	int rc = import_allowed(m, m->M.g.depth_levels, plan, vol);
+	if (rc == UFO_B200_OK) rc = plan_import(m, plan, data, size);
+	return rc == UFO_B200_OK ? apply_import(m, plan, data) : rc;
+}
+
+// the node stream of a compressed input: one LZ4 block of uncompressed_size bytes
+int decompress_stream(Map* m, const void* data, size_t size, size_t uncompressed_size, std::vector<uint8_t>& raw)
+{
+	if (!lz4().ok) {
+		m->set_error("liblz4.so.1 not found: compressed input is unavailable");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	if (size > (size_t)INT_MAX || uncompressed_size > (size_t)INT_MAX) {
+		m->set_error("readData: an LZ4 block is at most 2^31 - 1 bytes");
+		return UFO_B200_E_INVALID;
+	}
+	raw.resize(std::max<size_t>(uncompressed_size, 1));
+	const int n = lz4().decompress(static_cast<const char*>(data), reinterpret_cast<char*>(raw.data()), (int)size, (int)uncompressed_size);
+	if (n < 0) {
+		m->set_error("readData: LZ4 decompression failed");
+		return UFO_B200_E_INVALID;
+	}
+	raw.resize((size_t)n);
+	return UFO_B200_OK;
+}
+
+// ---- file images: readHeader (octree.h:1338-1417) ----
+const char kFileHeader[] = "# UFOMap file";
+
+// The token loop of an istream over the image: operator>> skips whitespace and reads up to the next
+// one; numbers are the longest prefix of the token num_get would take.
+struct HeaderReader {
+	const char* p;
+	size_t n, at = 0;
+	bool good = true;
+	static bool space(char c) { return c == ' ' || c == '\t' || c == '\n' || c == '\v' || c == '\f' || c == '\r'; }
+	bool skip_space()
+	{
+		while (at < n && space(p[at])) ++at;
+		if (at == n) good = false;
+		return good;
+	}
+	std::string token()
+	{
+		if (!skip_space()) return std::string();
+		const size_t from = at;
+		while (at < n && !space(p[at])) ++at;
+		if (at == n) good = false;  // eof while reading: the token stands, the stream is no longer good
+		return std::string(p + from, at - from);
+	}
+	void skip_line()
+	{
+		while (at < n && p[at++] != '\n') {}
+		if (at == n && (n == 0 || p[n - 1] != '\n')) good = false;
+	}
+	// [+-]digits[.digits][e[+-]digits] with at least one digit; false (and not good) otherwise
+	bool number(std::string& out, bool fraction)
+	{
+		if (!skip_space()) return false;
+		const size_t from = at;
+		auto digits = [&]() {
+			size_t k = 0;
+			while (at < n && p[at] >= '0' && p[at] <= '9') ++at, ++k;
+			return k;
+		};
+		if (at < n && (p[at] == '+' || p[at] == '-')) ++at;
+		size_t nd = digits();
+		if (fraction && at < n && p[at] == '.') {
+			++at;
+			nd += digits();
+		}
+		if (fraction && nd && at < n && (p[at] == 'e' || p[at] == 'E')) {
+			const size_t e = at++;
+			if (at < n && (p[at] == '+' || p[at] == '-')) ++at;
+			if (!digits()) at = e;
+		}
+		if (!nd) {
+			good = false;
+			return false;
+		}
+		out.assign(p + from, at - from);
+		if (at == n) good = false;
+		return true;
+	}
+};
+
+// readHeader without the tree-type test; `id` in full.  Returns OK or E_INVALID, and fills `out`
+// with what it read either way.
+int parse_header(const void* image, size_t size, ufo_b200_file_header* out, std::string& id)
+{
+	memset(out, 0, sizeof(*out));
+	out->uncompressed_data_size = -1;
+	id.clear();
+	const char* p = static_cast<const char*>(image);
+	size_t eol = 0;
+	while (eol < size && p[eol] != '\n') ++eol;
+	if (eol < sizeof kFileHeader - 1 || memcmp(p, kFileHeader, sizeof kFileHeader - 1) != 0) return UFO_B200_E_INVALID;
+	HeaderReader s{p, size, eol < size ? eol + 1 : size};
+	if (s.at == size) s.good = false;
+	std::string version;
+	bool header_read = false;
+	while (s.good && !header_read) {
+		const std::string token = s.token();
+		std::string num;
+		if (token.empty()) break;
+		if (token == "data") {
+			header_read = true;
+			s.skip_line();
+			out->data_offset = s.at;
+		} else if (token[0] == '#') {
+			s.skip_line();
+		} else if (token == "version") {
+			version = s.token();
+		} else if (token == "id") {
+			id = s.token();
+		} else if (token == "resolution") {
+			if (s.number(num, true)) out->resolution = strtod(num.c_str(), nullptr);
+		} else if (token == "depth_levels") {
+			if (s.number(num, false)) {
+				const long long v = strtoll(num.c_str(), nullptr, 10);
+				if (v > (long long)UINT32_MAX || v < -(long long)UINT32_MAX) s.good = false;
+				else out->depth_levels = (uint32_t)v;
+			}
+		} else if (token == "compressed") {
+			if (s.number(num, false)) {
+				const long long v = strtoll(num.c_str(), nullptr, 10);
+				if (v != 0 && v != 1) s.good = false;
+				else out->compressed = (int32_t)v;
+			}
+		} else if (token == "uncompressed_data_size") {
+			if (s.number(num, false)) {
+				const long long v = strtoll(num.c_str(), nullptr, 10);
+				if (v > INT_MAX || v < INT_MIN) s.good = false;
+				else out->uncompressed_data_size = v;
+			}
+		} else {
+			s.skip_line();
+		}
+	}
+	snprintf(out->version, sizeof out->version, "%s", version.c_str());
+	snprintf(out->id, sizeof out->id, "%s", id.c_str());
+	if (!header_read || version.empty() || id.empty() || !(out->resolution > 0.0) || out->depth_levels == 0 ||
+	    out->uncompressed_data_size < 0)
+		return UFO_B200_E_INVALID;
+	return UFO_B200_OK;
+}
+
+// Octree::read (octree.h:700-729) of a file image
+int read_image(Map* m, const uint8_t* image, size_t size)
+{
+	ufo_b200_file_header h;
+	std::string id;
+	if (parse_header(image, size, &h, id) != UFO_B200_OK) {
+		m->set_error("read: not a valid UFOMap file header");
+		return UFO_B200_E_INVALID;
+	}
+	const char* type = m->M.color ? "occupancy_map_color" : "occupancy_map";
+	if (id != type) {
+		m->set_error("read: a file of type '%s' does not go into an %s", h.id, type);
+		return UFO_B200_E_INVALID;
+	}
+	if (h.depth_levels > 21) {
+		m->set_error("read: depth_levels %u (at most 21)", h.depth_levels);
+		return UFO_B200_E_INVALID;
+	}
+	ImportPlan plan;
+	plan.g = make_geometry(h.resolution, h.depth_levels);
+	int rc = import_allowed(m, h.depth_levels, plan, Volume{nullptr, 0, {}, {}});
+	if (rc != UFO_B200_OK) return rc;
+	const bool resize = h.resolution != m->M.g.resolution || h.depth_levels != m->M.g.depth_levels;
+	if (resize && m->M.route_world > 1) {
+		m->set_error("read: a routed map cannot be re-created with the file's resolution / depth_levels");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	const uint8_t* body = image + h.data_offset;
+	size_t body_size = size - h.data_offset;
+	std::vector<uint8_t> raw;
+	if (h.compressed) {
+		// decompressed once: the reference decompresses a second time in readData (DESIGN.md section 7)
+		rc = decompress_stream(m, body, body_size, (size_t)h.uncompressed_data_size, raw);
+		if (rc != UFO_B200_OK) return rc;
+		body = raw.data();
+		body_size = raw.size();
+	}
+	rc = plan_import(m, plan, body, body_size);
+	if (rc != UFO_B200_OK) return rc;
+	if (resize) {
+		rc = ufo_b200_clear_resize(m, h.resolution, h.depth_levels);
+		if (rc != UFO_B200_OK) return rc;
+	}
+	return apply_import(m, plan, body);
 }
 }  // namespace
 
@@ -4100,17 +4469,9 @@ int ufo_b200_read_data_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_b
 	return guarded(m, [&]() {
 		const Volume vol{as_records(bv), (uint32_t)n_bv};
 		if (!compressed) return import_stream(m, static_cast<const uint8_t*>(data), size, vol);
-		if (!lz4().ok) {
-			m->set_error("liblz4.so.1 not found: compressed input is unavailable");
-			return (int)UFO_B200_E_UNSUPPORTED;
-		}
-		std::vector<uint8_t> raw(std::max<size_t>(uncompressed_size, 1));
-		const int n = lz4().decompress(static_cast<const char*>(data), reinterpret_cast<char*>(raw.data()), (int)size, (int)uncompressed_size);
-		if (n < 0) {
-			m->set_error("readData: LZ4 decompression failed");
-			return (int)UFO_B200_E_INVALID;
-		}
-		return import_stream(m, raw.data(), (size_t)n, vol);
+		std::vector<uint8_t> raw;
+		const int rc = decompress_stream(m, data, size, uncompressed_size, raw);
+		return rc != UFO_B200_OK ? rc : import_stream(m, raw.data(), raw.size(), vol);
 	});
 }
 
@@ -4120,6 +4481,53 @@ int ufo_b200_read_data(ufo_b200_map* m, const double* box6, const void* data, si
 	const VolRec r = box6 ? aabb_record(box6) : VolRec{};
 	return ufo_b200_read_data_bv(m, reinterpret_cast<const ufo_b200_volume*>(&r), box6 ? 1 : 0, data, size, compressed,
 	                             uncompressed_size);
+}
+
+int ufo_b200_read_header(const void* image, size_t size, ufo_b200_file_header* out)
+{
+	if (!out || (!image && size)) return UFO_B200_E_INVALID;
+	std::string id;
+	return parse_header(image, size, out, id);
+}
+
+int ufo_b200_read(ufo_b200_map* m, const void* image, size_t size)
+{
+	if (!m || (!image && size)) return UFO_B200_E_INVALID;
+	if (m->route_stage == 1) {
+		m->set_error("read between ufo_b200_route_mark and the last ufo_b200_route_apply of the pass");
+		return UFO_B200_E_INVALID;
+	}
+	return guarded(m, [&]() { return read_image(m, static_cast<const uint8_t*>(image), size); });
+}
+
+int ufo_b200_read_file(ufo_b200_map* m, const char* filename)
+{
+	if (!m || !filename) return UFO_B200_E_INVALID;
+	if (m->route_stage == 1) {
+		m->set_error("read between ufo_b200_route_mark and the last ufo_b200_route_apply of the pass");
+		return UFO_B200_E_INVALID;
+	}
+	return guarded(m, [&]() {
+		FILE* f = fopen(filename, "rb");
+		if (!f) {
+			m->set_error("cannot open %s", filename);
+			return (int)UFO_B200_E_INVALID;
+		}
+		std::vector<uint8_t> image;
+		bool ok = fseeko(f, 0, SEEK_END) == 0;
+		const off_t n = ok ? ftello(f) : -1;
+		ok = ok && n >= 0 && fseeko(f, 0, SEEK_SET) == 0;
+		if (ok) {
+			image.resize((size_t)n);
+			ok = fread(image.data(), 1, image.size(), f) == image.size();
+		}
+		fclose(f);
+		if (!ok) {
+			m->set_error("cannot read %s", filename);
+			return (int)UFO_B200_E_INVALID;
+		}
+		return read_image(m, image.data(), image.size());
+	});
 }
 
 }  // extern "C"
@@ -4389,50 +4797,6 @@ int ufo_b200_insert_rays(ufo_b200_map* m, const double* origins, const double* e
 // ---------------------------------------------------------------------------
 namespace
 {
-// the events of one call
-struct Events {
-	cudaEvent_t e[4] = {};
-	Events()
-	{
-		for (auto& x : e) CK(cudaEventCreate(&x));
-	}
-	Events(const Events&) = delete;
-	Events& operator=(const Events&) = delete;
-	~Events()
-	{
-		for (auto& x : e)
-			if (x) cudaEventDestroy(x);
-	}
-};
-
-// Pinned staging for the sections of a page: two chunks of a bounded size on each side, so that the
-// host's copy of one chunk overlaps the device's work on the next and a page of any size needs
-// 2 x kPageChunk of pinned memory.
-constexpr size_t kPageChunk = 16u << 20;
-struct PageStage {
-	uint8_t* pin[2] = {};
-	DevBuf dev_buf[2];
-	uint8_t* dev[2] = {};
-	cudaEvent_t ev[2] = {};
-	PageStage()
-	{
-		for (int b = 0; b < 2; ++b) {
-			CK(cudaHostAlloc(reinterpret_cast<void**>(&pin[b]), kPageChunk, cudaHostAllocDefault));
-			dev[b] = dev_buf[b].alloc<uint8_t>(kPageChunk);
-			CK(cudaEventCreateWithFlags(&ev[b], cudaEventDisableTiming));
-		}
-	}
-	PageStage(const PageStage&) = delete;
-	PageStage& operator=(const PageStage&) = delete;
-	~PageStage()
-	{
-		for (int b = 0; b < 2; ++b) {
-			if (pin[b]) cudaFreeHost(pin[b]);
-			if (ev[b]) cudaEventDestroy(ev[b]);
-		}
-	}
-};
-
 // One section of a page-out: gather(device chunk, first brick, bricks) fills a device chunk, which
 // goes to pinned memory and from there into the caller's buffer.
 template <class Gather>
