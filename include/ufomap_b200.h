@@ -526,7 +526,7 @@ typedef struct {
 	uint64_t regrows;         /* pool growth events during this insert     */
 	uint64_t launches;        /* kernels launched by this insert           */
 	uint64_t result_bytes;    /* bytes of per-scan counters copied device -> host by this insert */
-	uint64_t touched_lines;   /* 128-byte lines of leaf data the update read (HBM moves whole lines): lines holding a touched octet, less those whose touched octets all sit in saturated pairs (ufo_b200_last_update_stats) */
+	uint64_t touched_lines;   /* 128-byte lines of leaf data the update read (HBM moves whole lines): lines holding a touched octet, less saturated lines (ufo_b200_last_update_stats) */
 	float ms_total;           /* CUDA-event time of the whole insert (device work) */
 	float ms_h2d;
 	float ms_points;          /* K1: discretise + hit marking              */
@@ -556,12 +556,12 @@ int ufo_b200_last_walk_stats(ufo_b200_map* m, ufo_b200_walk_stats* out);
 
 /* What the leaf update of the most recent insert left out (waits for it to finish).  Counted at
  * profiling level 2 only; all zero otherwise, and always zero on colour maps, which read and write
- * every touched pair.  A saturated pair is a pair of initialised octets
- * (a 64 B half line) that the scan only marked free and whose 16 voxels already sit at
- * clamping_thres_min: the update would not change it, so it is neither read nor written. */
+ * every touched line.  A saturated line is a 128 B leaf line of four initialised octets that the
+ * scan only marked free and whose 32 voxels already sit at clamping_thres_min: the update would
+ * not change it, so it is neither read nor written. */
 typedef struct {
-	uint64_t saturated_octets; /* touched octets in saturated pairs (part of touched_octets)          */
-	uint64_t saturated_lines;  /* 128 B leaf lines with touched voxels that were not read because of them */
+	uint64_t saturated_octets; /* touched octets in saturated lines (part of touched_octets)          */
+	uint64_t saturated_lines;  /* saturated lines with touched voxels: not read                        */
 	uint64_t clean_sectors;    /* 32 B leaf sectors read and updated but left unchanged: not written back */
 } ufo_b200_update_stats;
 int ufo_b200_last_update_stats(ufo_b200_map* m, ufo_b200_update_stats* out);

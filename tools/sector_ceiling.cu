@@ -16,9 +16,12 @@
 // (touched_lines / D_2 = 1.14), and 81 % of the 4 octets of a touched line are touched
 // (D_1 / touched_lines = 3.2); k3_all adds, per brick, the depth-1 sector of every marked block
 // (own region), the mask / meta slab (1280 B) and the depth-2 aggregates (512 B) -- the metadata of
-// the layout with per-octet maxima; k3_pairs is today's layout: the leaf sectors, the untouched
+// the layout with per-octet maxima; k3_pairs the layout with pair maxima: the leaf sectors, the untouched
 // partner (2k, 2k+1) of every touched octet (read-modify-written here, only read by K3: an upper
-// bound), the mask / meta slab and the brick's pair maxima (1 KB).
+// bound), the mask / meta slab and the brick's pair maxima (1 KB); k3_lines is the layout with one
+// maximum per 128 B line: the leaf sectors, every other octet of each touched line (again
+// read-modify-written), the mask / meta slab and the brick's line maxima (512 B).  The "_ro"
+// variants of the last two only read the untouched partners / line-mates, as K3 does.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -37,6 +40,8 @@
 		}                                                                              \
 	} while (0)
 
+constexpr uint32_t kReadOnly = 0x80000000u;  // list flag (mode 0): load the sector, do not write it back
+
 template <int MODE>  // 0 rmw, 1 read
 __global__ void __launch_bounds__(256) k_sectors(float4* __restrict__ pool, const uint32_t* __restrict__ list, uint32_t n, float* sink)
 {
@@ -54,14 +59,17 @@ __global__ void __launch_bounds__(256) k_sectors(float4* __restrict__ pool, cons
 #pragma unroll
 		for (int u = 0; u < U; ++u) {
 			if (s[u] != 0xffffffffu) {
-				a[u] = pool[(size_t)s[u] * 2];
-				b[u] = pool[(size_t)s[u] * 2 + 1];
+				const size_t q = s[u] & ~kReadOnly;
+				a[u] = pool[q * 2];
+				b[u] = pool[q * 2 + 1];
 			}
 		}
 #pragma unroll
 		for (int u = 0; u < U; ++u) {
 			if (s[u] == 0xffffffffu) continue;
-			if (MODE == 0) {
+			if (MODE == 0 && (s[u] & kReadOnly)) {
+				acc += a[u].y + b[u].z;
+			} else if (MODE == 0) {
 				a[u].x += 1.f; a[u].y += 1.f; a[u].z += 1.f; a[u].w += 1.f;
 				b[u].x += 1.f; b[u].y += 1.f; b[u].z += 1.f; b[u].w += 1.f;
 				pool[(size_t)s[u] * 2] = a[u];
@@ -71,7 +79,7 @@ __global__ void __launch_bounds__(256) k_sectors(float4* __restrict__ pool, cons
 			}
 		}
 	}
-	if (MODE == 1 && acc == 123.456f) *sink = acc;
+	if (acc == 123.456f) *sink = acc;
 }
 
 int main(int argc, char** argv)
@@ -132,12 +140,14 @@ int main(int argc, char** argv)
 		const double pb = argc > 3 ? atof(argv[3]) : 0.53, p_both = argc > 4 ? atof(argv[4]) : 0.14, po = argc > 5 ? atof(argv[5]) : 0.81;
 		std::uniform_real_distribution<double> uni(0.0, 1.0);
 		// regions inside the pool, in 32 B sectors: leaves [0, T*512), depth-1 [T*512, T*576), slab + depth-2
-		// [T*576, T*632); k3_pairs: slab + pair maxima [T*576, T*648)
+		// [T*576, T*632); k3_pairs: slab + pair maxima [T*576, T*648); k3_lines: slab + line maxima [T*576, T*632)
 		const uint32_t T = std::min(touched, (uint32_t)((size_t)pool_bricks * 512 / 648));
+		const char* names[] = {"k3_leaf", "k3_all", "k3_pairs", "k3_lines", "k3_pairs_ro", "k3_lines_ro"};
 		std::vector<uint32_t> pt(T);
 		for (uint32_t i = 0; i < T; ++i) pt[i] = i;
 		std::shuffle(pt.begin(), pt.end(), rng);
-		for (int all = 0; all < 3; ++all) {  // k3_leaf, k3_all, k3_pairs
+		for (int all = 0; all < 6; ++all) {
+			const bool pairs = all == 2 || all == 4, lines_ = all == 3 || all == 5, ro = all >= 4;
 			std::vector<uint32_t> list;
 			size_t leaf_sectors = 0, lines = 0;
 			for (uint32_t t = 0; t < T; ++t) {
@@ -155,19 +165,28 @@ int main(int argc, char** argv)
 						if (!l4) l4 = 1u << (blk & 3);
 						t8 |= l4 << (4 * h);
 					}
-					const uint32_t ld = all == 2 ? t8 | ((t8 & 0x55u) << 1) | ((t8 & 0xaau) >> 1) : t8;
+					const uint32_t ld = pairs    ? t8 | ((t8 & 0x55u) << 1) | ((t8 & 0xaau) >> 1)
+					                    : lines_ ? ((t8 & 0x0fu) ? 0x0fu : 0u) | ((t8 & 0xf0u) ? 0xf0u : 0u)
+					                             : t8;
 					for (uint32_t o = 0; o < 8; ++o)
-						if ((ld >> o) & 1u) list.push_back(brick * 512u + blk * 8u + o);
+						if ((ld >> o) & 1u) list.push_back((brick * 512u + blk * 8u + o) | (ro && !((t8 >> o) & 1u) ? kReadOnly : 0u));
 					leaf_sectors += __builtin_popcount(t8);
 					lines += ((t8 & 0x0f) ? 1 : 0) + ((t8 & 0xf0) ? 1 : 0);
 					if (all == 1) list.push_back(T * 512u + brick * 64u + blk);
 				}
 				if (all == 1)
 					for (uint32_t q = 0; q < 56; ++q) list.push_back(T * 576u + brick * 56u + q);
-				if (all == 2)
+				if (pairs)
 					for (uint32_t q = 0; q < 72; ++q) list.push_back(T * 576u + brick * 72u + q);
+				if (lines_)
+					for (uint32_t q = 0; q < 56; ++q) list.push_back(T * 576u + brick * 56u + q);
 			}
 			const uint32_t n = (uint32_t)list.size();
+			for (uint32_t e : list)
+				if ((e & ~kReadOnly) >= pool_bricks * 512u) {
+					fprintf(stderr, "%s: sector %u outside the pool\n", names[all], e & ~kReadOnly);
+					return 1;
+				}
 			uint32_t* dl;
 			CK(cudaMalloc(&dl, (size_t)n * 4));
 			CK(cudaMemcpy(dl, list.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
@@ -182,7 +201,7 @@ int main(int argc, char** argv)
 				if (rep >= 1) best = std::min(best, ms);
 			}
 			printf("{\"pattern\": \"%s\", \"bricks\": %u, \"p_block\": %.2f, \"p_both_lines\": %.2f, \"p_octet_in_line\": %.2f, \"sectors\": %u, \"leaf_sectors\": %zu, \"leaf_lines_128B\": %zu, \"ms\": %.4f, \"GBps\": %.1f}\n",
-			       all == 2 ? "k3_pairs" : all ? "k3_all" : "k3_leaf", T, pb, p_both, po, n, leaf_sectors, lines, best, (double)n * 64.0 / (best * 1e-3) / 1e9);
+			       names[all], T, pb, p_both, po, n, leaf_sectors, lines, best, (double)n * 64.0 / (best * 1e-3) / 1e9);
 			CK(cudaFree(dl));
 		}
 	}

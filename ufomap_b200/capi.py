@@ -515,7 +515,7 @@ class Map:
 
     def update_stats(self):
         """What the leaf update of the last insert left out (profiling level 2): touched octets of
-        saturated pairs, leaf lines not read because of them, sectors not written back."""
+        saturated lines, leaf lines not read because of them, sectors not written back."""
         st = UpdateStats()
         self._check(self.lib.ufo_b200_last_update_stats(self.h, C.byref(st)))
         return st.as_dict()

@@ -166,10 +166,11 @@ struct DeviceMap {
 	unsigned long long* hit_mask;   // [b] per-scan hit bits
 	unsigned long long* chg_mask;   // [b] voxels changed since the last reset (allocated by enableChangeDetection)
 	uint32_t* meta;                 // [b] bits 0..15: flags of the 8 octets, bits 16..23: octet initialised
-	// [b] pair maxima: component k = max of the depth-1 nodes (octets) 2k and 2k+1, an uninitialised
-	// octet counting as 0.0.  The depth-2 value is their max (block_occ), the depth-2 flags follow
-	// from meta (block_flags), a depth-1 value is the max of the octet's 32 B leaf sector (octet_occ).
-	float4* pair_max;
+	// [b] line maxima: component h = max of the depth-1 nodes (octets) 4h..4h+3, the octets of the
+	// block's 128 B leaf line h, an uninitialised octet counting as 0.0.  The depth-2 value is their
+	// max (block_occ), the depth-2 flags follow from meta (block_flags), a depth-1 value is the max of
+	// the octet's 32 B leaf sector (octet_occ).
+	float2* line_max;
 	uint32_t* rgb2;                 // colour maps: [b]
 	uint32_t* sum1_rgb;             // colour maps: [b][8]
 	// Keys outside [0, 2^L) (a coordinate exactly on the + face of the map, or a walk that
@@ -468,8 +469,13 @@ __device__ __forceinline__ float octet_occ(const float* lp)
 	const float4 a = reinterpret_cast<const float4*>(lp)[0], c = reinterpret_cast<const float4*>(lp)[1];
 	return fmaxf(fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w)), fmaxf(fmaxf(c.x, c.y), fmaxf(c.z, c.w)));
 }
-// depth-2 value of a block from its pair maxima
-__device__ __forceinline__ float block_occ(float4 q) { return fmaxf(fmaxf(q.x, q.y), fmaxf(q.z, q.w)); }
+// depth-2 value of a block from its line maxima
+__device__ __forceinline__ float block_occ(float2 q) { return fmaxf(q.x, q.y); }
+// line maxima of a block from the maxima of its 8 octets
+__device__ __forceinline__ float2 line_maxima(const float (&om)[8])
+{
+	return make_float2(fmaxf(fmaxf(om[0], om[1]), fmaxf(om[2], om[3])), fmaxf(fmaxf(om[4], om[5]), fmaxf(om[6], om[7])));
+}
 // depth-2 flags of a block from its meta word: an uninitialised octet is unknown space
 __device__ __forceinline__ uint32_t block_flags(const DeviceMap& M, uint32_t mt)
 {
@@ -480,15 +486,15 @@ __device__ __forceinline__ uint32_t block_flags(const DeviceMap& M, uint32_t mt)
 }
 
 // float add + float clamp (occupancy_map_base.h:1139-1145).
-// Saturated pairs.  Let c = clamp_min be nonzero with c <= clamp_max, and let no leaf of the map lie
+// Saturated lines.  Let c = clamp_min be nonzero with c <= clamp_max, and let no leaf of the map lie
 // below c (DeviceMap::sat_skip; the voxels of an initialised octet that no update has reached hold
-// 0.0, so this needs c < 0).  If both octets of a pair are initialised and the pair maximum is c
-// bit for bit, every one of its 16 leaves is >= c and <= c, so it equals c, and being nonzero it has
-// c's bits.  For a miss u <= 0 (and not NaN), v + u <= c, so fmaxf(v + u, c) = c and fminf(c,
+// 0.0, so this needs c < 0).  If all four octets of a leaf line are initialised and the line maximum
+// is c bit for bit, every one of its 32 leaves is >= c and <= c, so it equals c, and being nonzero it
+// has c's bits.  For a miss u <= 0 (and not NaN), v + u <= c, so fmaxf(v + u, c) = c and fminf(c,
 // clamp_max) = c: every marked voxel keeps its bits, the reference's updateOccupancy reports no
-// change, and leaves, octet flags, pair maximum, colours, change mask and every aggregate above stay
+// change, and leaves, octet flags, line maximum, colours, change mask and every aggregate above stay
 // as they are.  c = 0 is left out because -0.0 and +0.0 compare equal but differ in their bits.  Hits
-// are applied before misses and can raise a voxel, so a pair with a hit bit is updated as usual.
+// are applied before misses and can raise a voxel, so a line with a hit bit is updated as usual.
 __device__ __forceinline__ float apply_update(const DeviceMap& M, float v, float u)
 {
 	return fminf(fmaxf(__fadd_rn(v, u), M.clamp_min), M.clamp_max);

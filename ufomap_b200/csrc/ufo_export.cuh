@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(64) k_brick_stream(DeviceMap M, uint32_t n_bri
 	s_blk_has[t] = blk_has ? 1 : 0;
 	s_blk_size[t] = blk_size;
 	// payload when the block is written as a leaf: its value, or its depth-2 aggregate
-	s_blk_occ[t] = blk_has ? block_occ(M.pair_max[b]) : oocc[0];
+	s_blk_occ[t] = blk_has ? block_occ(M.line_max[b]) : oocc[0];
 	s_blk_rgb[t] = blk_has ? (COLOR ? M.rgb2[b] : 0u) : orgb[0];
 	__syncthreads();
 	if (t < 8) {
@@ -442,7 +442,7 @@ __global__ void __launch_bounds__(64) k_brick_iter(DeviceMap M, uint32_t n_brick
 		}
 	}
 	const bool blk_has = keeps_children(oct_has != 0, oocc, orgb);
-	const float blk_v = blk_has ? block_occ(M.pair_max[b]) : oocc[0];
+	const float blk_v = blk_has ? block_occ(M.line_max[b]) : oocc[0];
 	const uint32_t blk_rgb = blk_has ? (COLOR ? M.rgb2[b] : 0u) : orgb[0];
 	s_blk_has[t] = blk_has ? 1 : 0;
 	s_blk_occ[t] = blk_v;
@@ -648,7 +648,7 @@ __global__ void __launch_bounds__(256) k_export_nodes(DeviceMap M, uint32_t n_br
 	const uint32_t meta = M.meta[blk];
 	const bool init = (meta >> 16) != 0;
 	if (d == 2) {
-		node_emit<CHAIN>(M, f, x0, y0, z0, init ? block_occ(M.pair_max[blk]) : 0.0f, (init && M.color) ? M.rgb2[blk] : 0u, codes, occ, rgbs, cap, count);
+		node_emit<CHAIN>(M, f, x0, y0, z0, init ? block_occ(M.line_max[blk]) : 0.0f, (init && M.color) ? M.rgb2[blk] : 0u, codes, occ, rgbs, cap, count);
 		return;
 	}
 	for (uint32_t o = 0; o < 8; ++o) {

@@ -300,7 +300,7 @@ __global__ void __launch_bounds__(256) k_import_wipe(DeviceMap M, uint32_t n_bri
 	}
 }
 
-// pair maxima, octet flags and depth-1 / depth-2 colours of every block of the touched bricks from
+// line maxima, octet flags and depth-1 / depth-2 colours of every block of the touched bricks from
 // the leaves (initialised octets only); one thread per (touched brick, block)
 __global__ void __launch_bounds__(256) k_import_refresh(DeviceMap M)
 {
@@ -328,7 +328,7 @@ __global__ void __launch_bounds__(256) k_import_refresh(DeviceMap M)
 				}
 			}
 		}
-		M.pair_max[b] = make_float4(fmaxf(om[0], om[1]), fmaxf(om[2], om[3]), fmaxf(om[4], om[5]), fmaxf(om[6], om[7]));
+		M.line_max[b] = line_maxima(om);
 		if (M.color) M.rgb2[b] = rms_rgb(oc, 8);
 		M.meta[b] = (mt & 0xff0000u) | fl16 | (M.scan_id << 24);
 	}

@@ -1164,7 +1164,7 @@ __global__ void __launch_bounds__(256) k_alias_refresh(DeviceMap M)
 			meta |= ofl << (2 * o);
 		}
 		// every octet now holds real values; several sources refreshing one target write the same
-		M.pair_max[tb] = make_float4(fmaxf(om[0], om[1]), fmaxf(om[2], om[3]), fmaxf(om[4], om[5]), fmaxf(om[6], om[7]));
+		M.line_max[tb] = line_maxima(om);
 		M.meta[tb] = meta | 0xff0000u | (M.scan_id << 24);
 		if (M.color) {
 			// the wrapped leaves' colours changed too (k_wrapped_colors): depth 1 and 2 colours
@@ -1486,7 +1486,7 @@ __device__ __forceinline__ void node_value(const DeviceMap& M, Key3 k, uint32_t 
 		const uint32_t meta = M.meta[slot];
 		if (!(meta >> 16)) return;
 		if (d == 2) {
-			o = block_occ(M.pair_max[slot]);
+			o = block_occ(M.line_max[slot]);
 			f = block_flags(M, meta);
 			if (M.color) c = M.rgb2[slot];
 		} else if (d == 1) {

@@ -254,7 +254,7 @@ namespace
 {
 using Map = ufo_b200_map;
 
-// Scans may skip saturated pairs (apply_update) while no leaf lies below clamp_min: the floor only
+// Scans may skip saturated leaf lines (apply_update) while no leaf lies below clamp_min: the floor only
 // falls (a lowered clamp_min, unclamped values), so once clamp_min is raised above it the skip stays
 // off until the map is cleared.  The floor is at most 0.0, so a positive clamp_min never skips.
 void set_value_floor(Map* m, float floor)
@@ -409,7 +409,7 @@ const PoolArray kPool[] = {
 	{UFO_POOL_ARRAY(M.miss_mask), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
 	{UFO_POOL_ARRAY(M.hit_mask), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
 	{UFO_POOL_ARRAY(M.meta), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
-	{UFO_POOL_ARRAY(M.pair_max), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.line_max), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
 	{UFO_POOL_ARRAY(M.brick_parent), 1, 0xff, Pool::Brick, Have::Always, Retain::Renew},
 	{UFO_POOL_ARRAY(chg_mask), 64, 0, Pool::Brick, Have::Changes, Retain::Compact},
 	{UFO_POOL_ARRAY(M.alias_miss), 64, 0, Pool::Brick, Have::Aliases, Retain::Compact},
@@ -3158,7 +3158,7 @@ int ufo_b200_clear(ufo_b200_map* m)
 		CK(cudaMemsetAsync(M.leaf, 0, nb * 64 * 4, s));
 		CK(cudaMemsetAsync(M.miss_mask, 0, nb * 8, s));
 		CK(cudaMemsetAsync(M.hit_mask, 0, nb * 8, s));
-		CK(cudaMemsetAsync(M.pair_max, 0, nb * sizeof(float4), s));
+		CK(cudaMemsetAsync(M.line_max, 0, nb * sizeof(float2), s));
 		CK(cudaMemsetAsync(M.meta, 0, nb * 4, s));
 		if (M.color) CK(cudaMemsetAsync(M.leaf_rgb, 0, nb * 64 * 4, s));
 		if (M.alias_miss) {
@@ -5172,7 +5172,7 @@ int page_in(Map* m, const void* blob, size_t size, ufo_b200_retain_stats* out)
 		});
 	}
 	CK(cudaEventRecord(ev.e[2], s));
-	// pair maxima, flags, inner colours, depth 3 / 4 and the levels above, under the current sensor model
+	// line maxima, flags, inner colours, depth 3 / 4 and the levels above, under the current sensor model
 	page_propagate(m, d_slot, n, true);
 	CK(cudaEventRecord(ev.e[3], s));
 	CK(cudaStreamSynchronize(s));

@@ -120,6 +120,8 @@ __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gmem_src, 
 	             "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
 	             : "memory");
 }
+// the octets of every leaf line (octets 4h..4h+3) that holds an octet of o8
+__device__ __forceinline__ uint32_t line_octets(uint32_t o8) { return ((o8 & 0x0fu) ? 0x0fu : 0u) | ((o8 & 0xf0u) ? 0xf0u : 0u); }
 __device__ __forceinline__ void fence_proxy_async()
 {
 	asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -143,15 +145,11 @@ struct __align__(128) WarpSlab {
 	unsigned long long mm[64];
 	unsigned long long hm[64];
 	uint32_t meta[64];
-	float4 q[64];  // pair maxima
+	float2 q[64];  // line maxima
 };
 // list entry of a loaded octet: (block << 3) | octet, plus
 constexpr uint32_t kEntInit = 1u << 9;      // the octet is initialised (its leaves are loaded; otherwise 0.0)
 constexpr uint32_t kEntTouched = 1u << 10;  // the scan marked a voxel of it (otherwise only its max is needed)
-// colour maps keep one entry in flight per lane, so a partner does not get an entry of its own: the
-// lane of the touched octet folds it into the octet's max (the slot then carries the pair's max)
-constexpr uint32_t kEntPartner = 1u << 11;      // untouched, initialised partner: loaded with the octet
-constexpr uint32_t kEntPartnerZero = 1u << 12;  // untouched, uninitialised partner: 0.0
 
 // K3: one WARP per brick of the scan's TOUCHED LIST (the cost of a scan does not depend on the size
 // of the map), no CTA-wide barrier at all: a warp waiting for its leaf sectors never holds others at
@@ -159,21 +157,21 @@ constexpr uint32_t kEntPartnerZero = 1u << 12;  // untouched, uninitialised part
 //  * warps claim their bricks from a work cursor (the cost of a brick varies by more than 10x);
 //  * lane 0 stages the header slab of the warp's NEXT brick -- miss masks 512 B, hit masks 512 B
 //    (only for a brick with a hit this scan: most bricks are crossed by free space only), meta
-//    256 B, pair maxima 1 KB -- with bulk copies (cp.async.bulk) on a per-warp mbarrier, two stages;
+//    256 B, line maxima 512 B -- with bulk copies (cp.async.bulk) on a per-warp mbarrier, two stages;
 //  * lane = block (twice: 64 blocks): masks from shared memory, list of the octets to load of the
-//    WHOLE brick by warp prefix sums: the touched octets and the initialised partners of touched
-//    octets (the pair (2k, 2k+1) is one 64 B-aligned piece of the block, so the partner's sector
-//    comes with the same DRAM access; colour maps: touched octets only, whose lane also reads the
-//    partner, see kEntPartner); built one brick EARLY, right after the previous brick's leaf
+//    WHOLE brick by warp prefix sums: the touched octets and the initialised untouched octets of
+//    every leaf line with a touched octet (a line, octets 4h..4h+3, is one 128 B-aligned piece of
+//    the block that HBM delivers whole, so its other sectors come with the same DRAM access, and
+//    the block keeps one maximum per line instead of one per octet); built one brick EARLY, right after the previous brick's leaf
 //    loop, so that the brick's leaf sectors can be pulled into the L2 (prefetch.global.L2, no
 //    registers) while the previous brick's aggregates are still being written;
 //  * colour maps: the old depth-1 / depth-2 colours the block lanes need at the end travel by
 //    cp.async into shared memory behind the leaf loop (no registers held across it);
 //  * lanes then own list entries = 32 B leaf sectors, UFO_UB_INFLIGHT requested per lane before the
 //    first is used (an uninitialised octet is not loaded: its leaves are 0.0): v = clamp(v + hit),
-//    then v = clamp(v + miss) (float, order fixed), written back in place; a partner is only read;
+//    then v = clamp(v + miss) (float, order fixed), written back in place; an untouched octet is only read;
 //    octet maxima / flags return through warp-private shared memory (__syncwarp only);
-//  * block lanes write the pair maxima and the meta word, clear the masks; depth-3 / depth-4
+//  * block lanes write the line maxima and the meta word, clear the masks; depth-3 / depth-4
 //    aggregates by shuffles.
 // Alternatives that were slower on the bench workload: a list per half brick (latency exposed twice
 // per brick); 2 sectors in flight at 6 CTAs of 80 registers; no L2 prefetch; more shared memory per
@@ -206,7 +204,7 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 #ifndef UFO_UB_MINBLOCKS_COLOR
 #define UFO_UB_MINBLOCKS_COLOR 7
 #endif
-// One warp's shared memory.  Kept small on purpose: 5 CTAs per SM (35.3 KB each + 1 KB reserved) fit
+// One warp's shared memory.  Kept small on purpose: 5 CTAs per SM (30.5 KB each + 1 KB reserved) fit
 // the 196 KB carve-out of the SM's 256 KB of L1 + shared memory; one step more (228 KB) leaves 28 KB
 // of L1, too little for the leaf sectors the warps keep in flight.
 template <bool COLOR>
@@ -256,11 +254,11 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 		}
 		const bool hits = !(mi & kMiNoHits);
 		fence_proxy_async();
-		mbar_expect_tx(&S.bar[stage], 512u + (hits ? 512u : 0u) + 256u + 1024u);
+		mbar_expect_tx(&S.bar[stage], 512u + (hits ? 512u : 0u) + 256u + 512u);
 		bulk_load(S.slab[stage].mm, M.mask_base + (size_t)(mi & ~kMiNoHits) * 64, 512u, &S.bar[stage]);
 		if (hits) bulk_load(S.slab[stage].hm, M.hit_mask + (size_t)brick * 64, 512u, &S.bar[stage]);
 		bulk_load(S.slab[stage].meta, M.meta + (size_t)brick * 64, 256u, &S.bar[stage]);
-		bulk_load(S.slab[stage].q, M.pair_max + (size_t)brick * 64, 1024u, &S.bar[stage]);
+		bulk_load(S.slab[stage].q, M.line_max + (size_t)brick * 64, 512u, &S.bar[stage]);
 	};
 	// all lanes, before the stage's list is built (a __syncwarp in between)
 	auto zero_hits = [&](uint32_t stage) {
@@ -284,16 +282,16 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 	__syncwarp();
 
 	unsigned int s_vox = 0, s_hit = 0, s_oct = 0, s_blk = 0, s_new = 0, s_lin = 0;
-	// saturated pairs (see apply_update): a miss-only pair whose 16 voxels all sit at clamp_min is
+	// saturated lines (see apply_update): a miss-only leaf line whose 32 voxels all sit at clamp_min is
 	// left as it is, so it is neither loaded nor written.  Exact only when the map holds no value below
 	// clamp_min (M.sat_skip, kept by the host) and the marks land in the tree (fold).  Mono maps only:
 	// on colour maps (config #3) the skip's extra code cost more K3 time than the lines it saved, so
-	// the colour kernel still reads every touched pair
+	// the colour kernel still reads every touched line
 	const bool sat = !COLOR && !SET && fold && M.sat_skip && miss <= 0.0f;
 
 	// lane = block lane of either half: touched octets of the brick in `slab` and the octets to load
-	// (touched, and initialised partners of touched ones), list by warp prefix sums.  t8 = the touched
-	// octets that are loaded | the touched octets of saturated pairs << 8 (not loaded)
+	// (touched, and the initialised octets of their lines), list by warp prefix sums.  t8 = the touched
+	// octets that are loaded | the touched octets of saturated lines << 8 (not loaded)
 	auto build_list = [&](const WarpSlab& slab, uint16_t* list, uint32_t (&t8)[2], uint32_t (&excl)[2], uint32_t& total) {
 		total = 0;
 #pragma unroll
@@ -314,19 +312,18 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				}
 				init = (slab.meta[blk] >> 16) & 0xffu;
 				if (sat) {
-					const float4 q = slab.q[blk];
-					const float qk[4] = {q.x, q.y, q.z, q.w};
+					const float2 q = slab.q[blk];
+					const float qh[2] = {q.x, q.y};
 #pragma unroll
-					for (uint32_t k = 0; k < 4; ++k) {
-						// pair k = octets 2k, 2k+1: x 0..3, y and z from the bits of k (linear mask order)
-						const unsigned long long pm = 0x00ff00ffull << (8 * (k & 1u) + 32 * (k >> 1));
-						const bool s = ((init >> (2 * k)) & 3u) == 3u && !(hm & pm) &&
-						               __float_as_uint(qk[k]) == __float_as_uint(M.clamp_min);
-						sk |= s ? t & (3u << (2 * k)) : 0u;
+					for (uint32_t k = 0; k < 2; ++k) {
+						// line k = octets 4k..4k+3 = voxels with z in {2k, 2k+1}: bits 32k..32k+31 (linear mask order)
+						const bool s = ((init >> (4 * k)) & 15u) == 15u && !((hm >> (32 * k)) & 0xffffffffull) &&
+						               __float_as_uint(qh[k]) == __float_as_uint(M.clamp_min);
+						sk |= s ? t & (15u << (4 * k)) : 0u;
 					}
 					t &= ~sk;
 				}
-				ld = t | (COLOR ? 0u : (((t & 0x55u) << 1) | ((t & 0xaau) >> 1)) & init);
+				ld = t | (line_octets(t) & init);
 				// out-of-tree hits (k_alias_apply, before this kernel) may have written an octet whose
 				// initialised bit is still clear: touched octets are then loaded all the same
 				if (!fold) init |= t;
@@ -344,9 +341,7 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				while (bits) {
 					const uint32_t o = __ffs(bits) - 1;
 					bits &= bits - 1;
-					uint32_t pf = 0;
-					if (COLOR && !((t >> (o ^ 1u)) & 1u)) pf = ((init >> (o ^ 1u)) & 1u) ? kEntPartner : kEntPartnerZero;
-					list[at++] = (uint16_t)((blk << 3) | o | (((init >> o) & 1u) ? kEntInit : 0u) | (((t >> o) & 1u) ? kEntTouched : 0u) | pf);
+					list[at++] = (uint16_t)((blk << 3) | o | (((init >> o) & 1u) ? kEntInit : 0u) | (((t >> o) & 1u) ? kEntTouched : 0u));
 				}
 			}
 			total += __shfl_sync(FULL, incl, 31);
@@ -393,7 +388,7 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 		// requested per lane before the first is used
 		constexpr int NF = COLOR ? UFO_UB_INFLIGHT_COLOR : UFO_UB_INFLIGHT;
 		for (uint32_t i = lane; i < total; i += 32 * NF) {
-			float4 a0[NF], a1[NF], p0[COLOR ? NF : 1], p1[COLOR ? NF : 1];
+			float4 a0[NF], a1[NF];
 			uint4 x0[COLOR ? NF : 1], x1[COLOR ? NF : 1];
 			uint32_t en[NF];
 #pragma unroll
@@ -413,18 +408,13 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 						x0[COLOR ? f : 0] = cp[0];
 						x1[COLOR ? f : 0] = cp[1];
 					}
-					if (COLOR && (en[f] & kEntPartner)) {
-						const float4* pp = reinterpret_cast<const float4*>(M.leaf + (off ^ 8u));
-						p0[COLOR ? f : 0] = pp[0];
-						p1[COLOR ? f : 0] = pp[1];
-					}
 				}
 			}
 #pragma unroll
 			for (int f = 0; f < NF; ++f) {
 				if (en[f] == 0xffffffffu) continue;
 				const uint32_t idx = i + 32 * f, t = (en[f] >> 3) & 63u, o = en[f] & 7u;
-				if (!(en[f] & kEntTouched)) {  // partner of a touched octet: its max only
+				if (!(en[f] & kEntTouched)) {  // line-mate of a touched octet: its max only
 					const float4 p = a0[f], q = a1[f];
 					S.omax[idx] = fmaxf(fmaxf(fmaxf(p.x, p.y), fmaxf(p.z, p.w)), fmaxf(fmaxf(q.x, q.y), fmaxf(q.z, q.w)));
 					continue;
@@ -434,11 +424,6 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				uint32_t ofl;
 				const bool clean = update_octet<SET, !COLOR>(M, miss, M.leaf + (b0 + t) * 64 + 8 * o, m8, h8, a0[f], a1[f], omax, ofl,
 				                                     b0 + t, o, (en[f] & kEntInit) != 0u);
-				if (COLOR && (en[f] & kEntPartner)) {
-					const float4 p = p0[COLOR ? f : 0], q = p1[COLOR ? f : 0];
-					omax = fmaxf(omax, fmaxf(fmaxf(fmaxf(p.x, p.y), fmaxf(p.z, p.w)), fmaxf(fmaxf(q.x, q.y), fmaxf(q.z, q.w))));
-				}
-				if (COLOR && (en[f] & kEntPartnerZero)) omax = fmaxf(omax, 0.0f);
 				S.omax[idx] = omax;
 				// the entry has been consumed: the slot carries the flags back (bit 2: not written back)
 				S.list[st][idx] = (uint16_t)(ofl | (clean ? 4u : 0u));
@@ -466,14 +451,13 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			for (uint32_t i = lane; i < totaln; i += 32) {
 				const uint32_t en = S.list[st ^ 1u][i], off = ((en >> 3) & 63u) * 64 + 8 * (en & 7u);
 				if (en & kEntInit) prefetch_l2(leaf_n + off);
-				if (COLOR && (en & kEntPartner)) prefetch_l2(leaf_n + (off ^ 8u));
 				if (COLOR && (en & kEntTouched)) prefetch_l2(M.leaf_rgb + (size_t)brick_n * 64 * 64 + off);
 			}
 #endif
 		}
 		if (COLOR) cp_async_wait_all();
 		__syncwarp();
-		// block lanes: pair maxima, meta, mask clearing
+		// block lanes: line maxima, meta, mask clearing
 		float agg_occ[2];
 		uint32_t agg_fl[2], agg_rgb[2];
 		uint32_t n_clean = 0;  // profiling level 2: this lane's sectors that were not written back
@@ -487,8 +471,8 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			float my_occ = 0.0f;
 			uint32_t my_fl = M.default_flags, my_rgb = 0;
 			if (marked) {
-				// t: the touched octets that were loaded.  An octet of a saturated pair (t8 bits 8..15) is
-				// treated like an untouched initialised one: flags from meta, old colour, old pair max
+				// t: the touched octets that were loaded.  An octet of a saturated line (t8 bits 8..15) is
+				// treated like an untouched initialised one: flags from meta, old colour, old line max
 				const uint32_t t = t8[h] & 0xffu, init = (mt >> 16) & 0xffu;
 				uint4 q0 = make_uint4(0u, 0u, 0u, 0u), q1 = q0;
 				if (COLOR && t != 0xffu) {
@@ -496,18 +480,15 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 					q1 = S.c1hi[COLOR ? blk : 0];
 				}
 				const uint32_t oldc[8] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w};
-				const float4 oq = slab.q[blk];
-				const float oldq[4] = {oq.x, oq.y, oq.z, oq.w};
-				const uint32_t ld = t | (COLOR ? 0u : (((t & 0x55u) << 1) | ((t & 0xaau) >> 1)) & init);
-				float om[8], nq[4];
+				const float2 oq = slab.q[blk];
+				const uint32_t ld = t | (line_octets(t) & init);
+				float om[8];
 				uint32_t newc[8];
 				uint32_t bfl = 0, newmeta = 0, at = excl[h];
 #pragma unroll
 				for (uint32_t o = 0; o < 8; ++o) {
 					uint32_t fl = M.default_flags, oc = 0;
-					// mono: an uninitialised partner of a touched octet; colour: the partner is already in
-					// the touched octet's slot
-					om[o] = COLOR ? -3.402823466e+38f : 0.0f;
+					om[o] = 0.0f;  // an uninitialised octet (only used in a loaded line)
 					if ((ld >> o) & 1u) {
 						om[o] = S.omax[at];
 						if ((t >> o) & 1u) {
@@ -528,11 +509,10 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 					bfl |= fl;
 					newmeta |= (fl << (2 * o)) | (((t >> o) & 1u) << (16 + o));
 				}
-#pragma unroll
-				for (uint32_t k = 0; k < 4; ++k) nq[k] = ((t >> (2 * k)) & 3u) ? fmaxf(om[2 * k], om[2 * k + 1]) : oldq[k];
-				const float4 q = make_float4(nq[0], nq[1], nq[2], nq[3]);
+				// a line without a loaded touched octet keeps its maximum
+				const float2 nq = line_maxima(om), q = make_float2((t & 0x0fu) ? nq.x : oq.x, (t & 0xf0u) ? nq.y : oq.y);
 				const float bmax = block_occ(q);
-				M.pair_max[b] = q;
+				M.line_max[b] = q;
 				if (COLOR) {
 					uint4* cp = reinterpret_cast<uint4*>(M.sum1_rgb + b * 8);
 					cp[0] = make_uint4(newc[0], newc[1], newc[2], newc[3]);
@@ -615,8 +595,8 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			}
 		}
 		if (!COLOR && M.k3_stat) {
-			// profiling level 2: octets of saturated pairs, leaf lines that were not read because of
-			// them, sectors not written back
+			// profiling level 2: touched octets of saturated lines, leaf lines that were not read because
+			// of them, sectors not written back
 			uint32_t n_sat = 0, n_lin = 0;
 #pragma unroll
 			for (uint32_t h = 0; h < 2; ++h) {
@@ -679,7 +659,7 @@ __global__ void __launch_bounds__(256) k_brick_agg(DeviceMap M)
 		}
 		const size_t b = (size_t)brick * 64 + 2 * lane;
 		const uint2 mt = *reinterpret_cast<const uint2*>(&M.meta[b]);
-		Agg c0 = {block_occ(M.pair_max[b]), block_flags(M, mt.x)}, c1 = {block_occ(M.pair_max[b + 1]), block_flags(M, mt.y)};
+		Agg c0 = {block_occ(M.line_max[b]), block_flags(M, mt.x)}, c1 = {block_occ(M.line_max[b + 1]), block_flags(M, mt.y)};
 		if (!(mt.x & 0xff0000u)) c0 = {0.0f, M.default_flags};  // never written: unknown space
 		if (!(mt.y & 0xff0000u)) c1 = {0.0f, M.default_flags};
 		const uint32_t tag = M.scan_id & 0xffu;
