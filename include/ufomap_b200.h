@@ -753,6 +753,48 @@ typedef struct {
 } ufo_b200_pool_counts;
 int ufo_b200_pool_stats(ufo_b200_map* m, ufo_b200_pool_counts* out);
 
+/* ---- copies and tree size ----
+ * ufo_b200_clone      a new map on the source's device holding the source's content, made on the
+ *                     device without serialisation (the reference's copy constructor writes and reads
+ *                     the map, occupancy_map_base.h:888-897).  Carried over: resolution, depth_levels,
+ *                     colour mode, the six stored sensor-model log-odds bit for bit, every leaf, leaf
+ *                     colour and octet-initialised bit, the values derived from them, and the alias state
+ *                     of a map that has seen out-of-tree keys: the same later calls give the same
+ *                     results on both maps.  Not carried over (a fresh map's defaults): change detection
+ *                     and its changes, the min/max change box, the early-stopping opt-in, profiling and
+ *                     a stream set with ufo_b200_set_stream (the copy has its own).  The brick pool's
+ *                     capacity is max(initial capacity, 2 x bricks), as after ufo_b200_retain.  Waits for
+ *                     a pending scan; the source is not changed.  Refused with nothing allocated: routed
+ *                     maps (ufo_b200_route_setup) and sharded maps (UFO_B200_E_UNSUPPORTED), a map whose
+ *                     scan failed half-way (UFO_B200_E_INVALID).  A device that cannot hold the copy gives
+ *                     UFO_B200_E_NOMEM and *out = NULL.
+ * ufo_b200_tree_info  the reference's node counters and getKnownBBX() of the pruned tree (the tree
+ *                     ufo_b200_iterate and the file writer walk), computed on the device.  A node has
+ *                     children iff it is not a leaf of that tree, so num_leaf_nodes = 8 x depth-1 nodes
+ *                     with children and num_inner_nodes = 1 + 8 x nodes with children at depth >= 2
+ *                     (getNumInnerNodes(): inner and inner-leaf nodes; the empty map has 1).  The known
+ *                     box is the per-axis min / max of centre -/+ half_size over the leaves of
+ *                     beginLeaves(occupied, free, !unknown), centres accumulated from the root as the
+ *                     iterators accumulate them; AABB((0,0,0), 0) when there is none (known = 0).  A map
+ *                     created with automatic_pruning = 0 reports the counters of the pruned tree.  A
+ *                     routed or sharded map reports its own part: the counts of the ranks do not add up
+ *                     to those of the union, whose upper levels and collapses differ.  Needs
+ *                     depth_levels >= 5 (UFO_B200_E_UNSUPPORTED). */
+int ufo_b200_clone(ufo_b200_map* src, ufo_b200_map** out);
+
+typedef struct {
+	uint64_t num_leaf_nodes;    /* getNumLeafNodes() */
+	uint64_t num_inner_nodes;   /* getNumInnerNodes() */
+	uint64_t with_children[22]; /* [d]: nodes of depth d that have children (d = 1 .. depth_levels) */
+	int32_t known;              /* 1: the map has a free or occupied leaf */
+	int32_t reserved;
+	double known_min[3], known_max[3];  /* getKnownBBX() */
+	float ms_device;            /* CUDA-event time of the brick pass on the map's stream */
+	float reserved2;
+} ufo_b200_tree_stats;
+/* (a type cannot share the function's name in C) */
+int ufo_b200_tree_info(ufo_b200_map* m, ufo_b200_tree_stats* out);
+
 const char* ufo_b200_version(void);
 
 #ifdef __cplusplus

@@ -560,8 +560,29 @@ class MapFacade
 	{
 		read(filename);
 	}
-	MapFacade(MapFacade const&) = delete;
-	MapFacade& operator=(MapFacade const&) = delete;
+	// The copy constructor (occupancy_map_base.h:888-897) without its file round trip: the map is
+	// copied on its device (ufo_b200_clone).  As in the reference, whose copy passes the source's
+	// probability getters to its constructor, the copy's sensor model is toLogit(toProb(x)) of the
+	// source's.  Change detection, min/max change detection, the early-stopping opt-in and a stream set
+	// on the source start as on a new map.  Throws std::runtime_error when the device copy fails.
+	MapFacade(MapFacade const& other) : map_(copyOf(other)), params_(other.params_) {}
+	// Copy assignment, an extension: the reference's is deleted (its map holds a std::future,
+	// occupancy_map_base.h:1553).  Same meaning as the copy constructor; when the copy fails this map is
+	// unchanged and the error is thrown.
+	MapFacade& operator=(MapFacade const& other)
+	{
+		if (this != &other) {
+			MapFacade copy(other);
+			std::swap(map_, copy.map_);
+			params_ = copy.params_;
+			changes_.clear();
+			change_enabled_ = false;
+			change_depth_ = 0;
+			minmax_enabled_ = false;
+			last_status_ = 0;
+		}
+		return *this;
+	}
 	virtual ~MapFacade() { ufo_b200_destroy(map_); }
 
 	virtual std::string getTreeType() const noexcept { return COLOR ? "occupancy_map_color" : "occupancy_map"; }
@@ -810,6 +831,33 @@ class MapFacade
 		last_status_ = ufo_b200_page_in(map_, blob.data(), blob.size(), stats);
 		return UFO_B200_OK == last_status_;
 	}
+	// getKnownBBX() (occupancy_map_base.h:828-852) and the node counters of octree.h:411-443 for the
+	// pruned tree, computed on the device (ufo_b200_tree_info).  The memoryUsage members apply the
+	// reference's formula to the sizes of ITS node types on LP64 (inner / leaf: 16 / 4 bytes, colour
+	// 24 / 8): they say what the reference would hold for this map, not what this library holds, which
+	// poolStats() reports.  A routed or sharded map reports its own part.
+	ufo::geometry::AABB getKnownBBX() const
+	{
+		const ufo_b200_tree_stats t = treeStats();
+		if (!t.known) return ufo::geometry::AABB(Point3(0, 0, 0), 0);
+		return ufo::geometry::AABB(Point3(t.known_min[0], t.known_min[1], t.known_min[2]),
+		                           Point3(t.known_max[0], t.known_max[1], t.known_max[2]));
+	}
+	std::size_t getNumInnerNodes() const { return treeStats().num_inner_nodes; }
+	std::size_t getNumLeafNodes() const { return treeStats().num_leaf_nodes; }
+	std::size_t memoryUsageInnerNode() const noexcept { return COLOR ? 24 : 16; }
+	std::size_t memoryUsageLeafNode() const noexcept { return COLOR ? 8 : 4; }
+	std::size_t memoryUsage() const
+	{
+		const ufo_b200_tree_stats t = treeStats();
+		return t.num_inner_nodes * memoryUsageInnerNode() + t.num_leaf_nodes * memoryUsageLeafNode();
+	}
+	std::size_t size() const
+	{
+		const ufo_b200_tree_stats t = treeStats();
+		return t.num_inner_nodes + t.num_leaf_nodes;
+	}
+
 	// live bricks / upper nodes, pool capacities and device bytes of the map right now
 	ufo_b200_pool_counts poolStats()
 	{
@@ -1273,6 +1321,27 @@ class MapFacade
 	{
 		ufo_b200_sensor_model_logit(map_, model_);
 		return model_;
+	}
+	ufo_b200_tree_stats treeStats() const
+	{
+		ufo_b200_tree_stats t{};
+		if (UFO_B200_OK != ufo_b200_tree_info(map_, &t)) throw std::runtime_error("ufomap_b200: " + lastError());
+		return t;
+	}
+	static ufo_b200_map* copyOf(MapFacade const& other)
+	{
+		ufo_b200_map* m = nullptr;
+		if (UFO_B200_OK != ufo_b200_clone(other.map_, &m))
+			throw std::runtime_error("ufomap_b200: the map could not be copied on its device: " + other.lastError());
+		const double p[6] = {other.getOccupiedThres(), other.getFreeThres(),         other.getProbHit(),
+		                     other.getProbMiss(),      other.getClampingThresMin(), other.getClampingThresMax()};
+		// one call for all six: the flags are rebuilt once
+		if (UFO_B200_OK != ufo_b200_set_sensor_model(m, p)) {
+			const std::string why = ufo_b200_last_error(m);
+			ufo_b200_destroy(m);
+			throw std::runtime_error("ufomap_b200: the copy's sensor model could not be set: " + why);
+		}
+		return m;
 	}
 
 	template <typename T>

@@ -1,0 +1,31 @@
+# oracle/info.mk -- builds the TEST-ONLY CPU checker of the tree counters, the known box and the copy
+# constructor.
+#
+#   _ref/libufo_ref_info.so  ref_info.cpp (which includes ref_color_writes.cpp, ref_writes.cpp and
+#                            ref_harness.cpp) against the UNMODIFIED reference under $(REF) (only present
+#                            in the build container); output in oracle/_ref/ only.
+#
+# Same compilers and flags as oracle/iterate.mk.  The library may not be linked or loaded by the product
+# path (ufomap_b200/).
+
+REF      ?= /root/reference
+CXX      ?= g++
+CXXFLAGS ?= -std=c++17 -O3 -DNDEBUG -fPIC -w
+REF_CXX  ?= $(shell if [ -x /usr/bin/g++ ]; then echo /usr/bin/g++; else echo $(CXX); fi)
+
+REF_SRCS = $(REF)/ufomap/src/map/occupancy_map.cpp \
+           $(REF)/ufomap/src/map/occupancy_map_color.cpp \
+           $(REF)/ufomap/src/geometry/bounding_volume.cpp \
+           $(REF)/ufomap/src/geometry/collision_checks.cpp
+
+all: ref
+
+ref:
+	@if [ -d $(REF)/ufomap/include ]; then $(MAKE) -f info.mk _ref/libufo_ref_info.so; \
+	 else echo "oracle: $(REF) absent -- using prebuilt _ref/libufo_ref_info.so if present"; fi
+
+_ref/libufo_ref_info.so: ref_info.cpp ref_color_writes.cpp ref_writes.cpp ref_harness.cpp
+	mkdir -p _ref
+	$(REF_CXX) $(CXXFLAGS) -shared -I$(REF)/ufomap/include -Istub -o $@ ref_info.cpp $(REF_SRCS) -lpthread -ldl
+
+.PHONY: all ref

@@ -106,6 +106,13 @@ class PoolCounts(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class TreeStats(C.Structure):
+    """ufo_b200_tree_stats: the reference's node counters and known box of the pruned tree."""
+    _fields_ = [("num_leaf_nodes", C.c_uint64), ("num_inner_nodes", C.c_uint64), ("with_children", C.c_uint64 * 22),
+                ("known", C.c_int32), ("reserved", C.c_int32), ("known_min", C.c_double * 3),
+                ("known_max", C.c_double * 3), ("ms_device", C.c_float), ("reserved2", C.c_float)]
+
+
 # every symbol include/ufomap_b200.h declares
 SYMBOLS = [
     "ufo_b200_default_params", "ufo_b200_create", "ufo_b200_destroy", "ufo_b200_last_error",
@@ -132,7 +139,7 @@ SYMBOLS = [
     "ufo_b200_iterate", "ufo_b200_update_nodes_color",
     "ufo_b200_retain_bv", "ufo_b200_retain", "ufo_b200_page_out_bv", "ufo_b200_page_in", "ufo_b200_page_info",
     "ufo_b200_pool_stats", "ufo_b200_last_update_stats", "ufo_b200_image_part_bv", "ufo_b200_image_assemble",
-    "ufo_b200_read_header", "ufo_b200_read", "ufo_b200_read_file",
+    "ufo_b200_read_header", "ufo_b200_read", "ufo_b200_read_file", "ufo_b200_clone", "ufo_b200_tree_info",
 ]
 
 # ufo_b200_volume: one shape of a bounding volume (type in BoundingVar order, members in v)
@@ -346,6 +353,8 @@ def load():
     lib.ufo_b200_page_in.argtypes = [vp, vp, sz, C.POINTER(RetainStats)]
     lib.ufo_b200_page_info.argtypes = [vp, sz, C.POINTER(PageHeader)]
     lib.ufo_b200_pool_stats.argtypes = [vp, C.POINTER(PoolCounts)]
+    lib.ufo_b200_clone.argtypes = [vp, C.POINTER(vp)]
+    lib.ufo_b200_tree_info.argtypes = [vp, C.POINTER(TreeStats)]
     lib.ufo_b200_version.restype = C.c_char_p
     _lib = lib
     return lib
@@ -868,6 +877,28 @@ class Map:
         st = PoolCounts()
         self._check(self.lib.ufo_b200_pool_stats(self.h, C.byref(st)))
         return st.as_dict()
+
+    def clone(self):
+        """A new Map on the same device holding this map's content (ufo_b200_clone): sensor model,
+        leaves, colours and everything derived; change detection, the change box, the early-stopping
+        opt-in, profiling and a set stream start as on a new map."""
+        h = C.c_void_p()
+        self._check(self.lib.ufo_b200_clone(self.h, C.byref(h)))
+        other = Map.__new__(Map)
+        other.lib, other.h = self.lib, h
+        other.color, other.resolution, other.depth_levels = self.color, self.resolution, self.depth_levels
+        return other
+
+    def tree_info(self):
+        """The reference's counters and known box of the pruned tree (ufo_b200_tree_info): dict with
+        num_leaf_nodes, num_inner_nodes, size, with_children (list by depth), known (bool), known_min,
+        known_max (getKnownBBX()'s min / max; zeros when nothing is known) and ms_device."""
+        st = TreeStats()
+        self._check(self.lib.ufo_b200_tree_info(self.h, C.byref(st)))
+        return dict(num_leaf_nodes=st.num_leaf_nodes, num_inner_nodes=st.num_inner_nodes,
+                    size=st.num_leaf_nodes + st.num_inner_nodes, with_children=list(st.with_children),
+                    known=bool(st.known), known_min=np.array(st.known_min[:]), known_max=np.array(st.known_max[:]),
+                    ms_device=st.ms_device)
 
     # -- state ----------------------------------------------------------------
     def value_field(self, sort=True):

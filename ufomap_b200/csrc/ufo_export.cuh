@@ -355,21 +355,21 @@ __device__ __forceinline__ bool iter_visit(const IterArgs& a, const double c[3],
 	return true;
 }
 
-// The records of one depth-2 node (block b) and its subtree, its parent being descended into;
-// written to dst when dst != nullptr.  oct_has / oocc / orgb: the block's octets as the canonical
+// The records of one depth-2 node (block b) and its subtree, its parent being descended into.  oct_has / oocc / orgb: the block's octets as the canonical
 // shape sees them.
-template <bool COLOR, bool G>
+// emit(n, record, centre, depth) receives the n-th record of the block.
+template <bool COLOR, bool G, class Emit>
 __device__ __forceinline__ uint32_t block_records(const DeviceMap& M, const IterArgs& a, size_t b, uint32_t meta,
                                                   uint32_t oct_has, const float oocc[8], const uint32_t orgb[8],
                                                   bool blk_has, float blk_v, uint32_t blk_rgb, const double blkc[3],
-                                                  unsigned long long code, IterRec* dst)
+                                                  unsigned long long code, Emit&& emit)
 {
 	const uint32_t blk_fl = (meta >> 16) ? block_flags(M, meta) : M.default_flags;
 	uint32_t n = 0;
 	bool ret;
 	if (!iter_visit<G>(a, blkc, M.g.half_size[2], 2, blk_v, blk_fl, !blk_has, &ret)) return 0;
 	if (ret) {
-		if (dst) dst[n] = iter_rec(code, blk_v, blk_rgb, 2, blk_fl, !blk_has);
+		emit(n, iter_rec(code, blk_v, blk_rgb, 2, blk_fl, !blk_has), blkc, 2u);
 		++n;
 	}
 	if (a.min_depth >= 2 || !blk_has) return n;
@@ -383,7 +383,7 @@ __device__ __forceinline__ uint32_t block_records(const DeviceMap& M, const Iter
 		child_center(blkc, M.g.half_size[1], o, oc);
 		if (!iter_visit<G>(a, oc, M.g.half_size[1], 1, ov, ofl, !oh, &ret)) continue;
 		if (ret) {
-			if (dst) dst[n] = iter_rec(ocode, ov, orv, 1, ofl, !oh);
+			emit(n, iter_rec(ocode, ov, orv, 1, ofl, !oh), oc, 1u);
 			++n;
 		}
 		if (a.min_depth >= 1 || !oh) continue;
@@ -393,23 +393,135 @@ __device__ __forceinline__ uint32_t block_records(const DeviceMap& M, const Iter
 			double vc[3];
 			child_center(oc, M.g.half_size[0], j, vc);
 			if (!iter_visit<G>(a, vc, M.g.half_size[0], 0, v, fl, true, &ret) || !ret) continue;
-			if (dst) dst[n] = iter_rec(ocode | j, v, COLOR ? M.leaf_rgb[b * 64 + 8 * o + j] : 0u, 0, fl, true);
+			emit(n, iter_rec(ocode | j, v, COLOR ? M.leaf_rgb[b * 64 + 8 * o + j] : 0u, 0, fl, true), vc, 0u);
 			++n;
 		}
 	}
 	return n;
 }
 
+// Shared memory of one brick's CTA in brick_descend: the canonical shape of the brick's subtree down to
+// the blocks and the iterator's decisions on its depth-4 and depth-3 nodes.
+struct BrickWalk {
+	float blk_occ[64], d3_occ[8];
+	uint32_t blk_rgb[64], d3_rgb[8];
+	uint8_t blk_has[64], d3_has[8], desc3[8], ret3[8];
+	IterRec rec4, rec3[8];
+	uint8_t has4, desc4, ret4;
+	double center[3];
+};
+
+// This thread's block (t = Morton index of the block in the brick) as the canonical shape sees it.
+struct BlockShape {
+	size_t b;
+	uint32_t meta, oct_has;
+	float oocc[8];
+	uint32_t orgb[8];
+	bool blk_has;
+	float blk_v;
+	uint32_t blk_rgb;
+	double blkc[3];
+};
+
+// The descent k_brick_iter and k_brick_info share: one CTA of 64 threads per brick (an in-tree one), one
+// thread per 4^3 block.  Fills S and B with the canonical shape (as k_brick_stream, pruned) and with
+// validNode / validReturnNode of the brick node and its depth-3 nodes, assuming the brick's parent is
+// descended into.  Ends with the CTA synchronised.
+template <bool COLOR, bool G>
+__device__ __forceinline__ void brick_descend(const DeviceMap& M, uint32_t brick, const IterArgs& a, BrickWalk& S, BlockShape& B)
+{
+	const uint32_t t = threadIdx.x;
+	uint32_t kx, ky, kz;
+	unpack_key(M.brick_key[brick], kx, ky, kz);
+	const unsigned long long code4 = key_to_code({kx << 4, ky << 4, kz << 4});
+	if (t == 0) brick_center(M.g, kx, ky, kz, S.center);
+	const size_t b = (size_t)brick * 64 + t;
+	B.b = b;
+	const uint32_t meta = M.meta[b];
+	B.meta = meta;
+	uint32_t oct_has = 0;
+#pragma unroll
+	for (uint32_t o = 0; o < 8; ++o) {
+		B.oocc[o] = 0.0f;
+		B.orgb[o] = 0u;
+		if (!((meta >> (16 + o)) & 1u)) continue;
+		const float* lp = M.leaf + b * 64 + 8 * o;
+		const uint32_t* cp = COLOR ? M.leaf_rgb + b * 64 + 8 * o : nullptr;
+		if (keeps_children(false, lp, cp)) {
+			oct_has |= 1u << o;
+		} else {
+			B.oocc[o] = lp[0];
+			B.orgb[o] = COLOR ? cp[0] : 0u;
+		}
+	}
+	B.oct_has = oct_has;
+	B.blk_has = keeps_children(oct_has != 0, B.oocc, B.orgb);
+	B.blk_v = B.blk_has ? block_occ(M.line_max[b]) : B.oocc[0];
+	B.blk_rgb = B.blk_has ? (COLOR ? M.rgb2[b] : 0u) : B.orgb[0];
+	S.blk_has[t] = B.blk_has ? 1 : 0;
+	S.blk_occ[t] = B.blk_v;
+	S.blk_rgb[t] = B.blk_rgb;
+	__syncthreads();
+	const uint32_t j3 = t >> 3, k3 = t & 7u;
+	const double bc[3] = {S.center[0], S.center[1], S.center[2]};
+	double d3c[3];
+	child_center(bc, M.g.half_size[3], j3, d3c);
+	child_center(d3c, M.g.half_size[2], k3, B.blkc);
+	if (t < 8) {
+		bool any = false;
+		for (int k = 0; k < 8; ++k) any = any || S.blk_has[8 * t + k];
+		const bool has = keeps_children(any, S.blk_occ + 8 * t, S.blk_rgb + 8 * t);
+		S.d3_has[t] = has ? 1 : 0;
+		S.d3_occ[t] = has ? M.brick_sum3[(size_t)brick * 8 + t].occ : S.blk_occ[8 * t];
+		S.d3_rgb[t] = has ? (COLOR ? M.brick_rgb3[(size_t)brick * 8 + t] : 0u) : S.blk_rgb[8 * t];
+	}
+	__syncthreads();
+	if (t == 0) {
+		bool any = false;
+		for (int j = 0; j < 8; ++j) any = any || S.d3_has[j];
+		const bool has = keeps_children(any, S.d3_occ, S.d3_rgb);
+		const float v = has ? M.brick_sum4[brick].occ : S.d3_occ[0];
+		const uint32_t rgb = has ? (COLOR ? M.brick_rgb4[brick] : 0u) : S.d3_rgb[0];
+		const uint32_t fl = M.brick_sum4[brick].flags;
+		bool ret;
+		const bool vis = a.min_depth <= 4 && iter_visit<G>(a, bc, M.g.half_size[4], 4, v, fl, !has, &ret);
+		S.has4 = has ? 1 : 0;
+		S.desc4 = (vis && a.min_depth < 4 && has) ? 1 : 0;
+		S.ret4 = (vis && ret) ? 1 : 0;
+		S.rec4 = iter_rec(code4, v, rgb, 4, fl, !has);
+	}
+	__syncthreads();
+	if (t < 8) {
+		const bool has = S.d3_has[t];
+		const float v = S.d3_occ[t];
+		const uint32_t fl = M.brick_sum3[(size_t)brick * 8 + t].flags;
+		double c3[3];
+		child_center(bc, M.g.half_size[3], t, c3);
+		bool ret = false;
+		const bool vis = S.desc4 && iter_visit<G>(a, c3, M.g.half_size[3], 3, v, fl, !has, &ret);
+		S.desc3[t] = (vis && a.min_depth < 3 && has) ? 1 : 0;
+		S.ret3[t] = (vis && ret) ? 1 : 0;
+		S.rec3[t] = iter_rec(code4 | ((unsigned long long)t << 9), v, S.d3_rgb[t], 3, fl, !has);
+	}
+	__syncthreads();
+}
+
+// the records of this thread's block and its subtree (block_records) when its depth-3 node is descended into
+template <bool COLOR, bool G, class Emit>
+__device__ __forceinline__ uint32_t block_walk(const DeviceMap& M, const IterArgs& a, const BrickWalk& S, const BlockShape& B,
+                                               unsigned long long blk_code, Emit&& emit)
+{
+	if (!S.desc3[threadIdx.x >> 3]) return 0;
+	return block_records<COLOR, G>(M, a, B.b, B.meta, B.oct_has, B.oocc, B.orgb, B.blk_has, B.blk_v, B.blk_rgb, B.blkc, blk_code,
+	                               emit);
+}
+
 template <bool COLOR, bool G>
 __global__ void __launch_bounds__(64) k_brick_iter(DeviceMap M, uint32_t n_bricks, IterArgs a, BrickInfo* info,
                                                    const unsigned long long* offsets, IterRec* out)
 {
-	__shared__ float s_blk_occ[64], s_d3_occ[8];
-	__shared__ uint32_t s_blk_rgb[64], s_d3_rgb[8], s_warp[2];
-	__shared__ uint8_t s_blk_has[64], s_d3_has[8], s_desc3[8], s_ret3[8];
-	__shared__ IterRec s_rec4, s_rec3[8];
-	__shared__ uint8_t s_desc4, s_ret4;
-	__shared__ double s_center[3];
+	__shared__ BrickWalk S;
+	__shared__ uint32_t s_warp[2];
 	const uint32_t brick = blockIdx.x, t = threadIdx.x;
 	if (brick >= n_bricks) return;
 	if (offsets && offsets[brick] == ~0ull) return;  // not reached by the walk above the bricks
@@ -419,82 +531,14 @@ __global__ void __launch_bounds__(64) k_brick_iter(DeviceMap M, uint32_t n_brick
 		if (!offsets && t == 0) info[brick] = {0u, 2u, 0.0f, 0u};
 		return;
 	}
-	const unsigned long long code4 = key_to_code({kx << 4, ky << 4, kz << 4});
-	if (t == 0) brick_center(M.g, kx, ky, kz, s_center);
-	// canonical shape of the block (as k_brick_stream, pruned)
-	const size_t b = (size_t)brick * 64 + t;
-	const uint32_t meta = M.meta[b];
-	uint32_t oct_has = 0;
-	float oocc[8];
-	uint32_t orgb[8];
-#pragma unroll
-	for (uint32_t o = 0; o < 8; ++o) {
-		oocc[o] = 0.0f;
-		orgb[o] = 0u;
-		if (!((meta >> (16 + o)) & 1u)) continue;
-		const float* lp = M.leaf + b * 64 + 8 * o;
-		const uint32_t* cp = COLOR ? M.leaf_rgb + b * 64 + 8 * o : nullptr;
-		if (keeps_children(false, lp, cp)) {
-			oct_has |= 1u << o;
-		} else {
-			oocc[o] = lp[0];
-			orgb[o] = COLOR ? cp[0] : 0u;
-		}
-	}
-	const bool blk_has = keeps_children(oct_has != 0, oocc, orgb);
-	const float blk_v = blk_has ? block_occ(M.line_max[b]) : oocc[0];
-	const uint32_t blk_rgb = blk_has ? (COLOR ? M.rgb2[b] : 0u) : orgb[0];
-	s_blk_has[t] = blk_has ? 1 : 0;
-	s_blk_occ[t] = blk_v;
-	s_blk_rgb[t] = blk_rgb;
-	__syncthreads();
-	const uint32_t j3 = t >> 3, k3 = t & 7u;
-	const double bc[3] = {s_center[0], s_center[1], s_center[2]};
-	double d3c[3], blkc[3];
-	child_center(bc, M.g.half_size[3], j3, d3c);
-	child_center(d3c, M.g.half_size[2], k3, blkc);
-	if (t < 8) {
-		bool any = false;
-		for (int k = 0; k < 8; ++k) any = any || s_blk_has[8 * t + k];
-		const bool has = keeps_children(any, s_blk_occ + 8 * t, s_blk_rgb + 8 * t);
-		s_d3_has[t] = has ? 1 : 0;
-		s_d3_occ[t] = has ? M.brick_sum3[(size_t)brick * 8 + t].occ : s_blk_occ[8 * t];
-		s_d3_rgb[t] = has ? (COLOR ? M.brick_rgb3[(size_t)brick * 8 + t] : 0u) : s_blk_rgb[8 * t];
-	}
-	__syncthreads();
-	if (t == 0) {
-		bool any = false;
-		for (int j = 0; j < 8; ++j) any = any || s_d3_has[j];
-		const bool has = keeps_children(any, s_d3_occ, s_d3_rgb);
-		const float v = has ? M.brick_sum4[brick].occ : s_d3_occ[0];
-		const uint32_t rgb = has ? (COLOR ? M.brick_rgb4[brick] : 0u) : s_d3_rgb[0];
-		const uint32_t fl = M.brick_sum4[brick].flags;
-		bool ret;
-		const bool vis = a.min_depth <= 4 && iter_visit<G>(a, bc, M.g.half_size[4], 4, v, fl, !has, &ret);
-		s_desc4 = (vis && a.min_depth < 4 && has) ? 1 : 0;
-		s_ret4 = (vis && ret) ? 1 : 0;
-		s_rec4 = iter_rec(code4, v, rgb, 4, fl, !has);
-		if (!offsets) info[brick] = {0u, has ? 1u : 0u, v, rgb};  // size: below
-	}
-	__syncthreads();
-	if (t < 8) {
-		const bool has = s_d3_has[t];
-		const float v = s_d3_occ[t];
-		const uint32_t fl = M.brick_sum3[(size_t)brick * 8 + t].flags;
-		double c3[3];
-		child_center(bc, M.g.half_size[3], t, c3);
-		bool ret = false;
-		const bool vis = s_desc4 && iter_visit<G>(a, c3, M.g.half_size[3], 3, v, fl, !has, &ret);
-		s_desc3[t] = (vis && a.min_depth < 3 && has) ? 1 : 0;
-		s_ret3[t] = (vis && ret) ? 1 : 0;
-		s_rec3[t] = iter_rec(code4 | ((unsigned long long)t << 9), v, s_d3_rgb[t], 3, fl, !has);
-	}
-	__syncthreads();
+	BlockShape B;
+	brick_descend<COLOR, G>(M, brick, a, S, B);
+	if (!offsets && t == 0) info[brick] = {0u, S.has4, S.rec4.occ, S.rec4.meta & 0xffffffu};  // size: below
 	// this thread's records, in pre-order: the brick node (t == 0), the depth-3 node (k3 == 0), the block
-	const unsigned long long blk_code = code4 | ((unsigned long long)t << 6);
-	const uint32_t head = (t == 0 ? s_ret4 : 0u) + (k3 == 0 ? s_ret3[j3] : 0u);
-	const uint32_t mine =
-	    head + (s_desc3[j3] ? block_records<COLOR, G>(M, a, b, meta, oct_has, oocc, orgb, blk_has, blk_v, blk_rgb, blkc, blk_code, nullptr) : 0u);
+	const uint32_t j3 = t >> 3, k3 = t & 7u;
+	const unsigned long long blk_code = S.rec4.code | ((unsigned long long)t << 6);
+	const uint32_t head = (t == 0 ? S.ret4 : 0u) + (k3 == 0 ? S.ret3[j3] : 0u);
+	const uint32_t mine = head + block_walk<COLOR, G>(M, a, S, B, blk_code, [](uint32_t, const IterRec&, const double*, uint32_t) {});
 	const uint32_t lane = t & 31u, warp = t >> 5;
 	uint32_t incl = mine;
 #pragma unroll
@@ -509,9 +553,85 @@ __global__ void __launch_bounds__(64) k_brick_iter(DeviceMap M, uint32_t n_brick
 		return;
 	}
 	IterRec* dst = out + offsets[brick] + (incl - mine) + (warp ? s_warp[0] : 0u);
-	if (t == 0 && s_ret4) *dst++ = s_rec4;
-	if (k3 == 0 && s_ret3[j3]) *dst++ = s_rec3[j3];
-	if (mine > head) block_records<COLOR, G>(M, a, b, meta, oct_has, oocc, orgb, blk_has, blk_v, blk_rgb, blkc, blk_code, dst);
+	if (t == 0 && S.ret4) *dst++ = S.rec4;
+	if (k3 == 0 && S.ret3[j3]) *dst++ = S.rec3[j3];
+	if (mine > head)
+		block_walk<COLOR, G>(M, a, S, B, blk_code, [dst](uint32_t n, const IterRec& r, const double*, uint32_t) { dst[n] = r; });
+}
+
+// Tree size of the live bricks (ufo_b200_tree_info): per brick the size-pass info of k_brick_iter, with
+// size = 1 when the brick node is itself a returned leaf (the host places it, as it is reached or not);
+// into out, the nodes with children at depth 1..4 and the known box of the leaves below the brick nodes
+// that have children, which the walk above always reaches.  `a` is beginLeaves(occupied, free, !unknown).
+struct TreeTotals {
+	unsigned long long with_children[4];  // [d - 1]
+	unsigned long long box[6];            // encode_ordered: min xyz (atomicMin), max xyz (atomicMax)
+};
+
+template <bool COLOR>
+__global__ void __launch_bounds__(64) k_brick_info(DeviceMap M, uint32_t n_bricks, IterArgs a, BrickInfo* info, TreeTotals* out)
+{
+	__shared__ BrickWalk S;
+	__shared__ unsigned long long s_part[2][10];
+	const uint32_t brick = blockIdx.x, t = threadIdx.x;
+	if (brick >= n_bricks) return;
+	uint32_t kx, ky, kz;
+	unpack_key(M.brick_key[brick], kx, ky, kz);
+	if ((kx | ky | kz) & ~(M.g.key_mask >> 4)) {  // collects out-of-tree marks, owns no voxels
+		if (t == 0) info[brick] = {0u, 2u, 0.0f, 0u};
+		return;
+	}
+	BlockShape B;
+	brick_descend<COLOR, false>(M, brick, a, S, B);
+	if (t == 0) info[brick] = {S.ret4 && !S.has4 ? 1u : 0u, S.has4, S.rec4.occ, S.rec4.meta & 0xffffffu};
+	if (!S.has4) return;
+	double lo[3] = {DBL_MAX, DBL_MAX, DBL_MAX}, hi[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX};
+	auto grow = [&](const double c[3], double hs) {
+		for (int i = 0; i < 3; ++i) {
+			lo[i] = fmin(lo[i], dop::sub(c[i], hs));
+			hi[i] = fmax(hi[i], dop::add(c[i], hs));
+		}
+	};
+	const uint32_t j3 = t >> 3;
+	if ((t & 7u) == 0 && S.ret3[j3]) {
+		double c3[3];
+		const double bc[3] = {S.center[0], S.center[1], S.center[2]};
+		child_center(bc, M.g.half_size[3], j3, c3);
+		grow(c3, M.g.half_size[3]);
+	}
+	block_walk<COLOR, false>(M, a, S, B, 0ull, [&](uint32_t, const IterRec&, const double* c, uint32_t d) { grow(c, M.g.half_size[d]); });
+	// per warp, then the two warps, then one atomic per value and brick
+	unsigned long long v[10];
+	v[0] = __popc(B.oct_has);
+	v[1] = B.blk_has ? 1u : 0u;
+	v[2] = t < 8 ? S.d3_has[t] : 0u;
+	v[3] = t == 0 ? 1u : 0u;
+	for (int i = 0; i < 3; ++i) {
+		v[4 + i] = lo[i] <= hi[i] ? encode_ordered(lo[i]) : ~0ull;
+		v[7 + i] = lo[i] <= hi[i] ? encode_ordered(hi[i]) : 0ull;
+	}
+#pragma unroll
+	for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+		for (int i = 0; i < 10; ++i) {
+			const unsigned long long y = __shfl_xor_sync(0xffffffffu, v[i], o);
+			v[i] = i < 4 ? v[i] + y : (i < 7 ? (y < v[i] ? y : v[i]) : (y > v[i] ? y : v[i]));
+		}
+	if ((t & 31u) == 0)
+		for (int i = 0; i < 10; ++i) s_part[t >> 5][i] = v[i];
+	__syncthreads();
+	if (t < 10) {
+		const unsigned long long x = s_part[0][t], y = s_part[1][t];
+		if (t < 4) {
+			if (x + y) atomicAdd(&out->with_children[t], x + y);
+		} else if (t < 7) {
+			const unsigned long long m = y < x ? y : x;
+			if (m != ~0ull) atomicMin(&out->box[t - 4], m);
+		} else {
+			const unsigned long long m = y > x ? y : x;
+			if (m) atomicMax(&out->box[t - 4], m);
+		}
+	}
 }
 
 // ---------------------------------------------------------------------------

@@ -89,6 +89,22 @@ struct DevBuf {
 	}
 };
 
+// the events of one call
+struct Events {
+	cudaEvent_t e[4] = {};
+	Events()
+	{
+		for (auto& x : e) CK(cudaEventCreate(&x));
+	}
+	Events(const Events&) = delete;
+	Events& operator=(const Events&) = delete;
+	~Events()
+	{
+		for (auto& x : e)
+			if (x) cudaEventDestroy(x);
+	}
+};
+
 double to_logit(double p) { return std::log(p / (1.0 - p)); }
 }  // namespace
 
@@ -436,21 +452,24 @@ uint32_t pool_cap(const Map* m, Pool pool) { return pool == Pool::Brick ? m->M.b
 
 // Replaces pool array `a` of old_cap bricks / nodes by one of new_cap (0: frees it).  The first
 // `kept` entries come from the old array, entries 0..kept or, with `src`, entries src[0..kept); the
-// others get the array's fill.  With nothing to keep the old array goes first.
-void reshape(Map* m, const PoolArray& a, uint32_t old_cap, uint32_t new_cap, uint32_t kept, const uint32_t* src)
+// others get the array's fill.  With `from` they come from that map's array instead (a copy on the
+// same device).  With nothing to keep from the old array it goes first.
+void reshape(Map* m, const PoolArray& a, uint32_t old_cap, uint32_t new_cap, uint32_t kept, const uint32_t* src,
+             Map* from = nullptr)
 {
 	cudaStream_t s = m->stream;
 	void*& p = *a.owner(m);
 	const size_t per = a.per * a.elem;
 	void* old = p;
-	if (!kept) {
+	if (!kept || from) {
 		p = nullptr;
 		map_realloc(m, old, (size_t)old_cap * per, 0);
 		old = nullptr;
 	}
+	const void* in = from ? *a.owner(from) : old;
 	void* q = map_realloc(m, nullptr, 0, (size_t)new_cap * per);
-	if (kept && src) launch_page_move<false>(m, q, old, src, kept, per);
-	else if (kept) CK(cudaMemcpyAsync(q, old, (size_t)kept * per, cudaMemcpyDeviceToDevice, s));
+	if (kept && src) launch_page_move<false>(m, q, in, src, kept, per);
+	else if (kept) CK(cudaMemcpyAsync(q, in, (size_t)kept * per, cudaMemcpyDeviceToDevice, s));
 	if (q) CK(cudaMemsetAsync(static_cast<uint8_t*>(q) + (size_t)kept * per, a.fill, (size_t)(new_cap - kept) * per, s));
 	if (old) {
 		CK(cudaStreamSynchronize(s));
@@ -1762,6 +1781,62 @@ void ufo_b200_default_params(ufo_b200_params* p)
 	p->device = -1;
 }
 
+}  // extern "C"
+
+namespace
+{
+// Everything of a new map on a device but its pools: device, streams, events, the counters' pinned
+// mirror, geometry and sensor model (ufo_b200_create, clone).
+void init_map(Map* m, const ufo_b200_params* p)
+{
+	int dev = p->device;
+	if (dev < 0) CK(cudaGetDevice(&dev));
+	CK(cudaSetDevice(dev));
+	m->device = dev;
+	cudaDeviceProp prop;
+	CK(cudaGetDeviceProperties(&prop, dev));
+	m->sm_count = prop.multiProcessorCount;
+	CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m->ray_blocks_per_sm, k_rays<0, false>, kRayThreads, 0));
+	if (m->ray_blocks_per_sm < 1) m->ray_blocks_per_sm = 1;
+	CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m->walk_blocks_per_sm, k_walk_mark<0, false, false, true>, kWalkThreads, 0));
+	if (m->walk_blocks_per_sm < 1) m->walk_blocks_per_sm = 1;
+	// the rounds kernel is cooperative: every CTA of its grid must be resident
+	CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m->early_blocks_per_sm, k_early_rounds, kEarlyThreads, 0));
+	if (m->early_blocks_per_sm < 1) m->early_blocks_per_sm = 1;
+	{
+		const char* e = getenv("UFO_B200_MARK");
+		m->force_records = e && !strcmp(e, "records");
+		m->no_dense = e && !strcmp(e, "probe");
+		// resident CTAs per SM of the two long kernels (tuning / co-residency experiments)
+		const char* kb = getenv("UFO_B200_K3_BLOCKS");
+		if (kb && atoi(kb) > 0) m->k3_blocks = atoi(kb);
+		const char* wb = getenv("UFO_B200_WALK_BLOCKS");
+		if (wb && atoi(wb) > 0) m->walk_blocks_per_sm = std::min(m->walk_blocks_per_sm, atoi(wb));
+	}
+	m->params = *p;
+	CK(cudaStreamCreateWithFlags(&m->own_stream, cudaStreamNonBlocking));
+	CK(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
+	CK(cudaEventCreate(&m->ev_copy0));
+	CK(cudaEventCreate(&m->ev_copied));
+	m->stream = m->own_stream;
+	for (auto& e : m->ev) CK(cudaEventCreate(&e));
+	CK(cudaHostAlloc(reinterpret_cast<void**>(&m->h_ctr), sizeof(Counters), cudaHostAllocDefault));
+	m->M.g = make_geometry(p->resolution, p->depth_levels);
+	m->M.color = p->color ? 1u : 0u;
+	m->M.shard_rank = 0;
+	m->M.shard_world = 1;
+	m->occ_thr_log = to_logit(p->occupied_thres);
+	m->free_thr_log = to_logit(p->free_thres);
+	m->hit_log = to_logit(p->prob_hit);
+	m->miss_log = to_logit(p->prob_miss);
+	m->cmin_log = to_logit(p->clamping_thres_min);
+	m->cmax_log = to_logit(p->clamping_thres_max);
+	refresh_model(m);
+}
+}  // namespace
+
+extern "C" {
+
 int ufo_b200_create(const ufo_b200_params* p, ufo_b200_map** out)
 {
 	if (!p || !out) return UFO_B200_E_INVALID;
@@ -1785,49 +1860,7 @@ int ufo_b200_create(const ufo_b200_params* p, ufo_b200_map** out)
 		return UFO_B200_OK;
 	}
 	int rc = guarded(m, [&]() {
-		int dev = p->device;
-		if (dev < 0) CK(cudaGetDevice(&dev));
-		CK(cudaSetDevice(dev));
-		m->device = dev;
-		cudaDeviceProp prop;
-		CK(cudaGetDeviceProperties(&prop, dev));
-		m->sm_count = prop.multiProcessorCount;
-		CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m->ray_blocks_per_sm, k_rays<0, false>, kRayThreads, 0));
-		if (m->ray_blocks_per_sm < 1) m->ray_blocks_per_sm = 1;
-		CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m->walk_blocks_per_sm, k_walk_mark<0, false, false, true>, kWalkThreads, 0));
-		if (m->walk_blocks_per_sm < 1) m->walk_blocks_per_sm = 1;
-		// the rounds kernel is cooperative: every CTA of its grid must be resident
-		CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&m->early_blocks_per_sm, k_early_rounds, kEarlyThreads, 0));
-		if (m->early_blocks_per_sm < 1) m->early_blocks_per_sm = 1;
-		{
-			const char* e = getenv("UFO_B200_MARK");
-			m->force_records = e && !strcmp(e, "records");
-			m->no_dense = e && !strcmp(e, "probe");
-			// resident CTAs per SM of the two long kernels (tuning / co-residency experiments)
-			const char* kb = getenv("UFO_B200_K3_BLOCKS");
-			if (kb && atoi(kb) > 0) m->k3_blocks = atoi(kb);
-			const char* wb = getenv("UFO_B200_WALK_BLOCKS");
-			if (wb && atoi(wb) > 0) m->walk_blocks_per_sm = std::min(m->walk_blocks_per_sm, atoi(wb));
-		}
-		m->params = *p;
-		CK(cudaStreamCreateWithFlags(&m->own_stream, cudaStreamNonBlocking));
-		CK(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
-		CK(cudaEventCreate(&m->ev_copy0));
-		CK(cudaEventCreate(&m->ev_copied));
-		m->stream = m->own_stream;
-		for (auto& e : m->ev) CK(cudaEventCreate(&e));
-		CK(cudaHostAlloc(reinterpret_cast<void**>(&m->h_ctr), sizeof(Counters), cudaHostAllocDefault));
-		m->M.g = make_geometry(p->resolution, p->depth_levels);
-		m->M.color = p->color ? 1u : 0u;
-		m->M.shard_rank = 0;
-		m->M.shard_world = 1;
-		m->occ_thr_log = to_logit(p->occupied_thres);
-		m->free_thr_log = to_logit(p->free_thres);
-		m->hit_log = to_logit(p->prob_hit);
-		m->miss_log = to_logit(p->prob_miss);
-		m->cmin_log = to_logit(p->clamping_thres_min);
-		m->cmax_log = to_logit(p->clamping_thres_max);
-		refresh_model(m);
+		init_map(m, p);
 		uint32_t bricks, upper;
 		initial_caps(*p, bricks, upper);
 		alloc_pools(m, bricks, upper);
@@ -3659,53 +3692,33 @@ void iter_walk(IterWalk& w, int32_t idx, uint32_t d, unsigned long long code, co
 	}
 }
 
-int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, float* logodds, uint8_t* flags, uint8_t* rgb, size_t cap,
-            size_t* n)
+// What iterate and tree_info share: `pass(d_info)` enqueues the size pass over the live bricks; their
+// info and keys come back, the bricks of the tree are sorted into Morton order, the shape above them is
+// built (build_upper), its nodes get their values (ufo_b200_query's) and iter_walk walks w.a over it.
+// w.plan must point at plan.
+template <class Pass>
+void walk_above_bricks(Map* m, IterWalk& w, ExportPlan& plan, std::vector<BrickInfo>& info, std::vector<unsigned long long>& keys,
+                       std::vector<unsigned long long>& brick_codes, Pass&& pass)
 {
-	*n = 0;
-	if (m->M.g.depth_levels < 5) {
-		m->set_error("iteration needs depth_levels >= 5");
-		return UFO_B200_E_UNSUPPORTED;
-	}
-	CK(cudaSetDevice(m->device));
-	sync_map(m);
-	const uint32_t L = m->M.g.depth_levels;
-	const double c0[3] = {0.0, 0.0, 0.0};
-	if (args.min_depth > L || !vol_hits(args.vol, c0, m->M.g.half_size[L])) return UFO_B200_OK;  // octree.h:200-208
 	cudaStream_t s = m->stream;
 	const uint32_t nb = m->n_bricks;
+	const uint32_t L = m->M.g.depth_levels;
 	const bool color = m->M.color != 0;
-	ExportPlan plan;
+	const double c0[3] = {0.0, 0.0, 0.0};
 	plan.levels = L;
 	plan.pruned = true;
 	plan.g = &m->M.g;
-	std::vector<BrickInfo> info(nb);
-	std::vector<unsigned long long> brick_codes;
+	info.assign(nb, BrickInfo{});
 	plan.info = info.data();
-	IterWalk w;
-	w.plan = &plan;
-	w.a = args;
 	w.a.occ_thr = m->M.occ_thr;
 	w.a.free_thr = m->M.free_thr;
 	w.default_flags = m->M.default_flags;
 	w.offs.assign(nb, ~0ull);
-	DevBuf b_info, b_offs, b_out, b_qcodes, b_qdepths, b_qocc, b_qflags, b_qrgb;
-	BrickInfo* d_info = nullptr;
-	DeviceVolume dvol;
-	Volume hv = args.vol;
-	const bool general = volume_is_general(hv);
-	IterArgs da = w.a;
-	da.vol = dvol.upload(hv, s);
-	auto brick_iter = [&](const unsigned long long* offs, IterRec* out) {
-		if (color && general) k_brick_iter<true, true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
-		else if (color) k_brick_iter<true, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
-		else if (general) k_brick_iter<false, true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
-		else k_brick_iter<false, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
-	};
-	std::vector<unsigned long long> keys(nb);
+	DevBuf b_info, b_qcodes, b_qdepths, b_qocc, b_qflags, b_qrgb;
+	keys.assign(nb, 0ull);
 	if (nb) {
-		d_info = b_info.alloc<BrickInfo>(nb);
-		brick_iter(nullptr, nullptr);
+		BrickInfo* d_info = b_info.alloc<BrickInfo>(nb);
+		pass(d_info);
 		CK(cudaGetLastError());
 		CK(cudaMemcpyAsync(info.data(), d_info, sizeof(BrickInfo) * nb, cudaMemcpyDeviceToHost, s));
 		CK(cudaMemcpyAsync(keys.data(), m->M.brick_key, 8ull * nb, cudaMemcpyDeviceToHost, s));
@@ -3732,32 +3745,71 @@ int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, floa
 	plan.codes = brick_codes.data();
 	if (sorted.empty()) {
 		iter_walk(w, -1, L, 0ull, c0, 0.0f, w.default_flags, 0u, true);
-	} else {
-		build_upper(plan, L, 0, sorted.size(), c0);
-		// values of the nodes above the bricks: ufo_b200_query's, one batch
-		const size_t nu = plan.nodes.size();
-		std::vector<unsigned long long> qc(nu);
-		std::vector<uint32_t> qd(nu), qrgb(nu, 0u);
-		upper_codes(plan, 0, L, 0ull, qc, qd);
-		w.occ.resize(nu);
-		w.flags.resize(nu);
-		unsigned long long* d_qcodes = b_qcodes.alloc<unsigned long long>(nu);
-		uint32_t* d_qdepths = b_qdepths.alloc<uint32_t>(nu);
-		float* d_qocc = b_qocc.alloc<float>(nu);
-		uint8_t* d_qflags = b_qflags.alloc<uint8_t>(nu);
-		uint32_t* d_qrgb = color ? b_qrgb.alloc<uint32_t>(nu) : nullptr;
-		CK(cudaMemcpyAsync(d_qcodes, qc.data(), 8 * nu, cudaMemcpyHostToDevice, s));
-		CK(cudaMemcpyAsync(d_qdepths, qd.data(), 4 * nu, cudaMemcpyHostToDevice, s));
-		k_query<<<(uint32_t)((nu + 255) / 256), 256, 0, s>>>(m->M, d_qcodes, d_qdepths, (uint32_t)nu, d_qocc, d_qflags, d_qrgb);
-		CK(cudaGetLastError());
-		CK(cudaMemcpyAsync(w.occ.data(), d_qocc, 4 * nu, cudaMemcpyDeviceToHost, s));
-		CK(cudaMemcpyAsync(w.flags.data(), d_qflags, nu, cudaMemcpyDeviceToHost, s));
-		if (color) CK(cudaMemcpyAsync(qrgb.data(), d_qrgb, 4 * nu, cudaMemcpyDeviceToHost, s));
-		CK(cudaStreamSynchronize(s));
-		w.rgb = std::move(qrgb);
-		const UpNode& r = plan.nodes[0];
-		iter_walk(w, 0, L, 0ull, c0, r.has ? w.occ[0] : r.occ, w.flags[0], r.has ? w.rgb[0] : r.rgb, !r.has);
+		return;
 	}
+	build_upper(plan, L, 0, sorted.size(), c0);
+	// values of the nodes above the bricks: ufo_b200_query's, one batch
+	const size_t nu = plan.nodes.size();
+	std::vector<unsigned long long> qc(nu);
+	std::vector<uint32_t> qd(nu), qrgb(nu, 0u);
+	upper_codes(plan, 0, L, 0ull, qc, qd);
+	w.occ.resize(nu);
+	w.flags.resize(nu);
+	unsigned long long* d_qcodes = b_qcodes.alloc<unsigned long long>(nu);
+	uint32_t* d_qdepths = b_qdepths.alloc<uint32_t>(nu);
+	float* d_qocc = b_qocc.alloc<float>(nu);
+	uint8_t* d_qflags = b_qflags.alloc<uint8_t>(nu);
+	uint32_t* d_qrgb = color ? b_qrgb.alloc<uint32_t>(nu) : nullptr;
+	CK(cudaMemcpyAsync(d_qcodes, qc.data(), 8 * nu, cudaMemcpyHostToDevice, s));
+	CK(cudaMemcpyAsync(d_qdepths, qd.data(), 4 * nu, cudaMemcpyHostToDevice, s));
+	k_query<<<(uint32_t)((nu + 255) / 256), 256, 0, s>>>(m->M, d_qcodes, d_qdepths, (uint32_t)nu, d_qocc, d_qflags, d_qrgb);
+	CK(cudaGetLastError());
+	CK(cudaMemcpyAsync(w.occ.data(), d_qocc, 4 * nu, cudaMemcpyDeviceToHost, s));
+	CK(cudaMemcpyAsync(w.flags.data(), d_qflags, nu, cudaMemcpyDeviceToHost, s));
+	if (color) CK(cudaMemcpyAsync(qrgb.data(), d_qrgb, 4 * nu, cudaMemcpyDeviceToHost, s));
+	CK(cudaStreamSynchronize(s));
+	w.rgb = std::move(qrgb);
+	const UpNode& r = plan.nodes[0];
+	iter_walk(w, 0, L, 0ull, c0, r.has ? w.occ[0] : r.occ, w.flags[0], r.has ? w.rgb[0] : r.rgb, !r.has);
+}
+
+int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, float* logodds, uint8_t* flags, uint8_t* rgb, size_t cap,
+            size_t* n)
+{
+	*n = 0;
+	if (m->M.g.depth_levels < 5) {
+		m->set_error("iteration needs depth_levels >= 5");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	CK(cudaSetDevice(m->device));
+	sync_map(m);
+	const uint32_t L = m->M.g.depth_levels;
+	const double c0[3] = {0.0, 0.0, 0.0};
+	if (args.min_depth > L || !vol_hits(args.vol, c0, m->M.g.half_size[L])) return UFO_B200_OK;  // octree.h:200-208
+	cudaStream_t s = m->stream;
+	const uint32_t nb = m->n_bricks;
+	const bool color = m->M.color != 0;
+	ExportPlan plan;
+	std::vector<BrickInfo> info;
+	std::vector<unsigned long long> keys, brick_codes;
+	IterWalk w;
+	w.plan = &plan;
+	w.a = args;
+	DevBuf b_offs, b_out;
+	DeviceVolume dvol;
+	Volume hv = args.vol;
+	const bool general = volume_is_general(hv);
+	IterArgs da = args;
+	da.occ_thr = m->M.occ_thr;
+	da.free_thr = m->M.free_thr;
+	da.vol = dvol.upload(hv, s);
+	auto brick_iter = [&](BrickInfo* d_info, const unsigned long long* offs, IterRec* out) {
+		if (color && general) k_brick_iter<true, true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+		else if (color) k_brick_iter<true, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+		else if (general) k_brick_iter<false, true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+		else k_brick_iter<false, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, offs, out);
+	};
+	walk_above_bricks(m, w, plan, info, keys, brick_codes, [&](BrickInfo* d_info) { brick_iter(d_info, nullptr, nullptr); });
 	*n = (size_t)w.total;
 	if (codes && w.total && w.total <= cap) {
 		std::vector<IterRec> packed(w.packed);
@@ -3765,7 +3817,7 @@ int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, floa
 			unsigned long long* d_offs = b_offs.alloc<unsigned long long>(nb);
 			IterRec* d_out = b_out.alloc<IterRec>(w.packed);
 			CK(cudaMemcpyAsync(d_offs, w.offs.data(), 8ull * nb, cudaMemcpyHostToDevice, s));
-			brick_iter(d_offs, d_out);
+			brick_iter(nullptr, d_offs, d_out);
 			CK(cudaGetLastError());
 			CK(cudaMemcpyAsync(packed.data(), d_out, sizeof(IterRec) * w.packed, cudaMemcpyDeviceToHost, s));
 			CK(cudaStreamSynchronize(s));
@@ -3794,6 +3846,115 @@ int iterate(Map* m, const IterArgs& args, uint64_t* codes, uint8_t* depths, floa
 	}
 	return UFO_B200_OK;
 }
+
+// nodes with children at depth >= 5 of the shape above the bricks (a collapsed node has none below it)
+void count_upper(const ExportPlan& plan, int32_t idx, uint32_t d, uint64_t* with_children)
+{
+	const UpNode& n = plan.nodes[idx];
+	if (!n.has) return;
+	++with_children[d];
+	if (d == 5) return;
+	for (uint32_t i = 0; i < 8; ++i)
+		if (n.child[i] >= 0) count_upper(plan, n.child[i], d - 1, with_children);
+}
+
+// centre of the node `code` of depth d, accumulated from the root as the iterators accumulate it
+void node_center(const Geometry& g, unsigned long long code, uint32_t d, double c[3])
+{
+	c[0] = c[1] = c[2] = 0.0;
+	for (uint32_t l = g.depth_levels; l > d; --l) {
+		double n[3];
+		child_center(c, g.half_size[l - 1], (uint32_t)(code >> (3 * (l - 1))) & 7u, n);
+		c[0] = n[0];
+		c[1] = n[1];
+		c[2] = n[2];
+	}
+}
+
+// getNumLeafNodes / getNumInnerNodes / getKnownBBX of the pruned tree: k_brick_info over the live
+// bricks, the levels above them as iterate walks them (beginLeaves(occupied, free, !unknown)).
+int tree_info(Map* m, ufo_b200_tree_stats* out)
+{
+	*out = ufo_b200_tree_stats{};
+	if (m->M.g.depth_levels < 5) {
+		m->set_error("tree_info needs depth_levels >= 5");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	CK(cudaSetDevice(m->device));
+	sync_map(m);
+	cudaStream_t s = m->stream;
+	const uint32_t nb = m->n_bricks;
+	const Geometry& g = m->M.g;
+	ExportPlan plan;
+	std::vector<BrickInfo> info;
+	std::vector<unsigned long long> keys, brick_codes;
+	IterWalk w;
+	w.plan = &plan;
+	w.a.leaves_only = 1;
+	w.a.occupied = 1;
+	w.a.free_ = 1;
+	IterArgs da = w.a;
+	da.occ_thr = m->M.occ_thr;
+	da.free_thr = m->M.free_thr;
+	TreeTotals tot{};
+	for (int i = 0; i < 3; ++i) tot.box[i] = ~0ull;
+	DevBuf b_tot;
+	TreeTotals* d_tot = b_tot.alloc<TreeTotals>(1);
+	Events ev;
+	CK(cudaMemcpyAsync(d_tot, &tot, sizeof(tot), cudaMemcpyHostToDevice, s));
+	walk_above_bricks(m, w, plan, info, keys, brick_codes, [&](BrickInfo* d_info) {
+		CK(cudaEventRecord(ev.e[0], s));
+		if (m->M.color) k_brick_info<true><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, d_tot);
+		else k_brick_info<false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, d_tot);
+		CK(cudaEventRecord(ev.e[1], s));
+		++m->launches;
+	});
+	CK(cudaMemcpyAsync(&tot, d_tot, sizeof(tot), cudaMemcpyDeviceToHost, s));
+	CK(cudaStreamSynchronize(s));
+	if (nb) CK(cudaEventElapsedTime(&out->ms_device, ev.e[0], ev.e[1]));
+
+	const uint32_t L = g.depth_levels;
+	for (uint32_t d = 1; d <= 4; ++d) out->with_children[d] = tot.with_children[d - 1];
+	if (!plan.nodes.empty()) count_upper(plan, 0, L, out->with_children);
+	uint64_t inner = 0;
+	for (uint32_t d = 2; d <= L; ++d) inner += out->with_children[d];
+	out->num_leaf_nodes = 8 * out->with_children[1];
+	out->num_inner_nodes = 1 + 8 * inner;
+
+	// occupancy_map_base.h:828-852: nothing but unknown space gives AABB((0,0,0), 0)
+	const bool root_has = !plan.nodes.empty() && plan.nodes[0].has;
+	const float root_v = plan.nodes.empty() ? 0.0f : (root_has ? w.occ[0] : plan.nodes[0].occ);
+	const uint32_t root_fl = plan.nodes.empty() ? m->M.default_flags : w.flags[0];
+	out->known = iter_contains(w.a, root_v, root_fl) ? 1 : 0;
+	if (!out->known) return UFO_B200_OK;
+	double lo[3], hi[3];
+	for (int i = 0; i < 3; ++i) {
+		lo[i] = tot.box[i] != ~0ull ? decode_ordered(tot.box[i]) : DBL_MAX;
+		hi[i] = tot.box[3 + i] != 0ull ? decode_ordered(tot.box[3 + i]) : -DBL_MAX;
+	}
+	// the leaves above the brick level and the bricks that are leaves themselves
+	for (const auto& p : w.pieces) {
+		double c[3];
+		uint32_t d = 4;
+		if (p.second == kNone) {
+			d = (p.first.meta >> 24) & 31u;
+			node_center(g, p.first.code, d, c);
+		} else {
+			uint32_t x, y, z;
+			unpack_key(keys[p.second], x, y, z);
+			brick_center(g, x, y, z, c);
+		}
+		for (int i = 0; i < 3; ++i) {
+			lo[i] = std::min(lo[i], dop::sub(c[i], g.half_size[d]));
+			hi[i] = std::max(hi[i], dop::add(c[i], g.half_size[d]));
+		}
+	}
+	for (int i = 0; i < 3; ++i) {
+		out->known_min[i] = lo[i];
+		out->known_max[i] = hi[i];
+	}
+	return UFO_B200_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -3817,6 +3978,12 @@ int ufo_b200_iterate(ufo_b200_map* m, int leaves_only, int occupied, int free_sp
 		a.contains = contains != 0;
 		return iterate(m, a, codes, depths, logodds, flags, rgb, cap, n);
 	});
+}
+
+int ufo_b200_tree_info(ufo_b200_map* m, ufo_b200_tree_stats* out)
+{
+	if (!m || !out) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() { return tree_info(m, out); });
 }
 
 }  // extern "C"
@@ -3909,22 +4076,6 @@ int ufo_b200_volume_intersects(const ufo_b200_volume* bv, size_t n_bv, const dou
 
 namespace
 {
-// the events of one call
-struct Events {
-	cudaEvent_t e[4] = {};
-	Events()
-	{
-		for (auto& x : e) CK(cudaEventCreate(&x));
-	}
-	Events(const Events&) = delete;
-	Events& operator=(const Events&) = delete;
-	~Events()
-	{
-		for (auto& x : e)
-			if (x) cudaEventDestroy(x);
-	}
-};
-
 // Pinned staging for the sections of a page: two chunks of a bounded size on each side, so that the
 // host's copy of one chunk overlaps the device's work on the next and a page of any size needs
 // 2 x kPageChunk of pinned memory.
@@ -5186,9 +5337,91 @@ int page_in(Map* m, const void* blob, size_t size, ufo_b200_retain_stats* out)
 	if (out) *out = st;
 	return UFO_B200_OK;
 }
+
+// A device copy of src, built the way retain rebuilds a map after its compaction: the first n_bricks
+// entries of every Compact brick array copied (every slot below n_bricks is live), the Renew arrays at
+// their fill, the change masks left out, the brick hash and the levels above the bricks rebuilt.
+void clone_into(Map* m, Map* src)
+{
+	ufo_b200_params p = src->params;
+	p.device = src->device;
+	init_map(m, &p);
+	m->params = src->params;
+	m->occ_thr_log = src->occ_thr_log;
+	m->free_thr_log = src->free_thr_log;
+	m->hit_log = src->hit_log;
+	m->miss_log = src->miss_log;
+	m->cmin_log = src->cmin_log;
+	m->cmax_log = src->cmax_log;
+	m->value_floor = src->value_floor;
+	refresh_model(m);
+	m->no_dense = src->no_dense;
+	m->M.scan_id = src->M.scan_id;  // the copied brick stamps hold scan ids of the source
+	reset_bbox(m);
+	DeviceMap& M = m->M;
+	const uint32_t n = src->n_bricks;
+	uint32_t cap0, up0;
+	initial_caps(m->params, cap0, up0);
+	M.brick_cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(cap0, 2ull * n), 0x3ffffffull);
+	M.up_cap = std::max(up0, M.brick_cap / 2);
+	for (const Pool pool : {Pool::Brick, Pool::Upper})
+		each_array(src, pool, [&](const PoolArray& a) {
+			if (a.have == Have::Changes) return;
+			const uint32_t keep = (pool == Pool::Brick && a.retain == Retain::Compact) ? n : 0u;
+			reshape(m, a, 0, pool_cap(m, pool), keep, nullptr, src);
+		});
+	m->ctr.ensure(m, sizeof(Counters), 0);
+	M.ctr = m->ctr.p;
+	brick_hash(m, n);
+	upper_hash(m, 0);
+	m->n_blocks = src->n_blocks;
+	m->n_bricks = n;
+	m->n_upper = 0;
+	page_propagate(m, nullptr, n, false);
+	CK(cudaStreamSynchronize(m->stream));
+}
+
+int clone(Map* src, Map** out)
+{
+	if (src->M.route_world > 1 || src->route_inbox.p || src->M.shard_world > 1) {
+		src->set_error("ufo_b200_clone: a routed or sharded map holds one rank's part and cannot be copied");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	CK(cudaSetDevice(src->device));
+	sync_map(src);
+	if (src->poisoned) {
+		src->set_error("an earlier scan failed half-way; ufo_b200_clear() the map first");
+		return UFO_B200_E_INVALID;
+	}
+	Map* m = new Map;
+	try {
+		clone_into(m, src);
+	} catch (...) {
+		// a failed cudaMalloc is the runtime's last error: read and clear it, so that later calls on the
+		// source do not report it
+		const bool oom = cudaGetLastError() == cudaErrorMemoryAllocation;
+		const std::string why = m->err;
+		ufo_b200_destroy(m);
+		if (oom) {
+			src->set_error("ufo_b200_clone: the device cannot hold the copy");
+			return UFO_B200_E_NOMEM;
+		}
+		if (!why.empty()) src->err = why;
+		throw;
+	}
+	*out = m;
+	return UFO_B200_OK;
+}
 }  // namespace
 
 extern "C" {
+
+int ufo_b200_clone(ufo_b200_map* src, ufo_b200_map** out)
+{
+	if (out) *out = nullptr;
+	if (!src || !out) return UFO_B200_E_INVALID;
+	return guarded(src, [&]() { return clone(src, out); });
+}
 
 int ufo_b200_retain_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, ufo_b200_retain_stats* out)
 {
