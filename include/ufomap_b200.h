@@ -795,6 +795,38 @@ typedef struct {
 /* (a type cannot share the function's name in C) */
 int ufo_b200_tree_info(ufo_b200_map* m, ufo_b200_tree_stats* out);
 
+/* ---- nearest-first iteration ----
+ * ufo_b200_nearest  one distance shell of beginNNLeaves (leaves_only != 0) / beginNNTree
+ *                   (occupancy_map_base.h:169-245) from point[3]: the nodes that ufo_b200_iterate
+ *                   returns for the same filters, contains, min_depth and volume, whose squared distance
+ *                   d2 from the point satisfies d2_from <= d2 < hi, in non-decreasing d2; equal distances
+ *                   keep ufo_b200_iterate's order (code ascending, depth descending).  d2 is the
+ *                   reference's squaredDistance (iterator/octree_nearest.h:198-202): the point minus the
+ *                   point clamped to the node's cube, (x*x + y*y) + z*z in doubles.  hi is chosen so that
+ *                   at least `want` nodes come back, or all that remain; it never splits a group of equal
+ *                   distances.  *d2_next = hi, where the next shell starts, or +inf when nothing is left.
+ *                   Arrays as ufo_b200_iterate, plus d2[i]; *n is always the shell's size, the arrays are
+ *                   filled when it is <= cap.  The shape of the tree above the bricks is kept on the map
+ *                   and rebuilt by the first call after the map changed.  A non-finite point or a NaN
+ *                   d2_from is UFO_B200_E_INVALID; depth_levels < 5 UFO_B200_E_UNSUPPORTED.  Waits for a
+ *                   pending scan.  A sharded or routed map searches the part its own rank holds.
+ * ufo_b200_last_nearest_stats  the work of the last ufo_b200_nearest call. */
+int ufo_b200_nearest(ufo_b200_map* m, const double point[3], const ufo_b200_volume* bv, size_t n_bv, int leaves_only,
+                     int occupied, int free_space, int unknown, int contains, uint32_t min_depth, double d2_from,
+                     size_t want, uint64_t* codes, uint8_t* depths, float* logodds, uint8_t* flags, uint8_t* rgb,
+                     double* d2, size_t cap, size_t* n, double* d2_next);
+
+typedef struct {
+	uint64_t bricks_visited;  /* CTAs of the brick kernel, summed over the shells tried */
+	uint64_t upper_visited;   /* nodes above the bricks the host search visited */
+	uint32_t shells;          /* brick kernel launches (a shell too small for `want` is doubled) */
+	int32_t rebuilt;          /* 1: this call rebuilt the cached tree shape */
+	uint64_t revision;        /* the map revision the call answered for; every write changes it */
+	float ms_device;          /* CUDA-event time of the brick kernels and the sort */
+	float ms_rebuild;         /* host time of the shape rebuild (0 when none) */
+} ufo_b200_nearest_stats;
+int ufo_b200_last_nearest_stats(ufo_b200_map* m, ufo_b200_nearest_stats* out);
+
 const char* ufo_b200_version(void);
 
 #ifdef __cplusplus

@@ -734,6 +734,203 @@ class MapFacade
 	Iterator endLeaves() const noexcept { return Iterator(); }
 
 	//
+	// Nearest-first iteration (occupancy_map_base.h:169-245) with the intended semantics (DESIGN §8):
+	// the nodes of beginTree / beginLeaves with the same arguments, in non-decreasing squared distance
+	// from a point, equal distances in beginTree / beginLeaves order.  The iterator fetches the sequence
+	// lazily in distance shells (ufo_b200_nearest): the first holds at least 8 nodes, each next one at
+	// least twice as many as the one before.  A map changed after begin*() ends the iteration at the next
+	// shell fetch and sets lastStatus() to UFO_B200_E_INVALID: it never mixes two states of the map.
+	// Forward iterator; copies share the fetched shells.  The map must outlive it.
+	//
+	class NNIterator
+	{
+	 public:
+		using value_type = std::conditional_t<COLOR, ColorOccupancyValue, OccupancyValue>;
+		using difference_type = std::ptrdiff_t;
+		using pointer = value_type const*;
+		using reference = value_type const&;
+		using iterator_category = std::forward_iterator_tag;
+
+		NNIterator() {}  // the end iterator
+
+		// as Iterator: equal when both are exhausted, or at the same node of the same sequence
+		bool operator==(NNIterator const& o) const
+		{
+			return (atEnd() && o.atEnd()) || (!atEnd() && !o.atEnd() && s_ == o.s_ && i_ == o.i_);
+		}
+		bool operator!=(NNIterator const& o) const { return !(*this == o); }
+		NNIterator& operator++()
+		{
+			++i_;
+			load();
+			return *this;
+		}
+		NNIterator operator++(int)
+		{
+			NNIterator r = *this;
+			++(*this);
+			return r;
+		}
+		reference operator*() const { return value_; }
+		pointer operator->() const { return &value_; }
+
+		double getDistance() const { return std::sqrt(getSquaredDistance()); }
+		double getSquaredDistance() const { return s_->d2[i_]; }
+		// an extension: the reference's nearest iterators have no getCode
+		Code getCode() const { return Code(s_->codes[i_], getDepth()); }
+		DepthType getDepth() const { return s_->depths[i_]; }
+		Point3 getCenter() const { return center_; }
+		double getX() const { return center_.x(); }
+		double getY() const { return center_.y(); }
+		double getZ() const { return center_.z(); }
+		double getSize() const { return 2.0 * getHalfSize(); }
+		double getHalfSize() const { return s_->half_size[getDepth()]; }
+		ufo::geometry::AABB getAABB() const { return ufo::geometry::AABB(center_, getHalfSize()); }
+		bool isLeaf() const { return s_->flags[i_] & 4u; }
+		bool isPureLeaf() const { return 0 == getDepth(); }
+		bool hasChildren() const { return !isLeaf(); }
+		bool isOccupied() const { return s_->occupied_thres_log < value_.occupancy; }
+		bool isFree() const { return s_->free_thres_log > value_.occupancy; }
+		bool isUnknown() const { return !isOccupied() && !isFree(); }
+		bool containsOccupied() const { return isOccupied(); }
+		bool containsFree() const { return s_->flags[i_] & 1u; }
+		bool containsUnknown() const { return s_->flags[i_] & 2u; }
+		double getOccupancy() const { return toProb(value_.occupancy); }
+
+	 private:
+		friend class MapFacade;
+		struct State {
+			MapFacade const* map;
+			double point[3];
+			std::vector<ufo_b200_volume> bv;
+			bool leaves, occupied, free_space, unknown, contains;
+			DepthType min_depth;
+			std::uint64_t revision = 0;
+			double d2_next = 0.0;  // where the next shell starts; +inf: none left
+			std::size_t want = 8;
+			std::vector<std::uint64_t> codes;
+			std::vector<std::uint8_t> depths, flags, rgb;
+			std::vector<float> logodds;
+			std::vector<double> d2;
+			double half_size[22];
+			DepthType levels;
+			double occupied_thres_log, free_thres_log;
+
+			// appends the next shell; false when none is left, the map changed or the call failed
+			bool fetch()
+			{
+				if (!(d2_next < HUGE_VAL)) return false;
+				ufo_b200_map* m = map->map_;
+				auto call = [&](std::size_t at, std::size_t cap, std::size_t* n, double* next) {
+					return ufo_b200_nearest(m, point, bv.data(), bv.size(), leaves, occupied, free_space, unknown, contains,
+					                        min_depth, d2_next, want, cap ? codes.data() + at : nullptr,
+					                        cap ? depths.data() + at : nullptr, cap ? logodds.data() + at : nullptr,
+					                        cap ? flags.data() + at : nullptr, cap && COLOR ? rgb.data() + 3 * at : nullptr,
+					                        cap ? d2.data() + at : nullptr, cap, n, next);
+				};
+				auto fail = [&](int status) {
+					map->last_status_ = status;
+					d2_next = HUGE_VAL;
+					return false;
+				};
+				std::size_t n = 0;
+				double next = HUGE_VAL;
+				int rc = call(0, 0, &n, &next);
+				ufo_b200_nearest_stats st{};
+				if (UFO_B200_OK != rc) return fail(rc);
+				ufo_b200_last_nearest_stats(m, &st);
+				if (0 == revision) revision = st.revision;
+				if (st.revision != revision) return fail(UFO_B200_E_INVALID);
+				const std::size_t at = codes.size();
+				codes.resize(at + n);
+				depths.resize(at + n);
+				logodds.resize(at + n);
+				flags.resize(at + n);
+				d2.resize(at + n);
+				if (COLOR) rgb.resize(3 * (at + n));
+				if (n) {
+					rc = call(at, n, &n, &next);
+					if (UFO_B200_OK != rc) return fail(rc);
+					ufo_b200_last_nearest_stats(m, &st);
+					if (st.revision != revision) return fail(UFO_B200_E_INVALID);
+				}
+				d2_next = next;
+				want *= 2;
+				return n > 0 || fetch();
+			}
+		};
+		explicit NNIterator(std::shared_ptr<State> s) : s_(std::move(s)) { load(); }
+		bool atEnd() const { return !s_ || i_ >= s_->codes.size(); }
+		void load()
+		{
+			if (s_ && i_ >= s_->codes.size() && !s_->fetch()) return;
+			if (atEnd()) return;
+			value_.occupancy = s_->logodds[i_];
+			if constexpr (COLOR) value_.color = Color(s_->rgb[3 * i_], s_->rgb[3 * i_ + 1], s_->rgb[3 * i_ + 2]);
+			// getChildCenter from the root down (octree.h:625-633), as the reference iterator accumulates it
+			Point3 c(0.0, 0.0, 0.0);
+			for (DepthType d = s_->levels; d > getDepth(); --d) {
+				unsigned idx = unsigned(s_->codes[i_] >> (3 * (d - 1))) & 7u;
+				double hs = s_->half_size[d - 1];
+				c[0] += (idx & 1u) ? hs : -hs;
+				c[1] += (idx & 2u) ? hs : -hs;
+				c[2] += (idx & 4u) ? hs : -hs;
+			}
+			center_ = c;
+		}
+		std::shared_ptr<State> s_;
+		std::size_t i_ = 0;
+		value_type value_{};
+		Point3 center_;
+	};
+	using NNTreeIterator = NNIterator;
+	using NNLeafIterator = NNIterator;
+
+	// beginNNTree / beginNNLeaves with the reference's overloads and defaults (the point comes before the
+	// volume).  A first shell that fails (no device, depth_levels < 5, a non-finite point) gives an empty
+	// sequence with its status in lastStatus().
+	NNIterator beginNNTree(Point3 const& coord, bool occupied_space = true, bool free_space = true,
+	                       bool unknown_space = false, bool contains = false, DepthType min_depth = 0) const
+	{
+		return nearest(false, coord, {}, occupied_space, free_space, unknown_space, contains, min_depth);
+	}
+	NNIterator beginNNTree(Point3 const& coord, ufo::geometry::BoundingVar const& bounding_volume,
+	                       bool occupied_space = true, bool free_space = true, bool unknown_space = false,
+	                       bool contains = false, DepthType min_depth = 0) const
+	{
+		return nearest(false, coord, {ufo::geometry::toRecord(bounding_volume)}, occupied_space, free_space, unknown_space,
+		               contains, min_depth);
+	}
+	NNIterator beginNNTree(Point3 const& coord, ufo::geometry::BoundingVolume const& bounding_volume,
+	                       bool occupied_space = true, bool free_space = true, bool unknown_space = false,
+	                       bool contains = false, DepthType min_depth = 0) const
+	{
+		return nearest(false, coord, ufo::geometry::toRecords(bounding_volume), occupied_space, free_space, unknown_space,
+		               contains, min_depth);
+	}
+	NNIterator endNNTree() const noexcept { return NNIterator(); }
+	NNIterator beginNNLeaves(Point3 const& coord, bool occupied_space = true, bool free_space = true,
+	                         bool unknown_space = false, bool contains = false, DepthType min_depth = 0) const
+	{
+		return nearest(true, coord, {}, occupied_space, free_space, unknown_space, contains, min_depth);
+	}
+	NNIterator beginNNLeaves(Point3 const& coord, ufo::geometry::BoundingVar const& bounding_volume,
+	                         bool occupied_space = true, bool free_space = true, bool unknown_space = false,
+	                         bool contains = false, DepthType min_depth = 0) const
+	{
+		return nearest(true, coord, {ufo::geometry::toRecord(bounding_volume)}, occupied_space, free_space, unknown_space,
+		               contains, min_depth);
+	}
+	NNIterator beginNNLeaves(Point3 const& coord, ufo::geometry::BoundingVolume const& bounding_volume,
+	                         bool occupied_space = true, bool free_space = true, bool unknown_space = false,
+	                         bool contains = false, DepthType min_depth = 0) const
+	{
+		return nearest(true, coord, ufo::geometry::toRecords(bounding_volume), occupied_space, free_space, unknown_space,
+		               contains, min_depth);
+	}
+	NNIterator endNNLeaves() const noexcept { return NNIterator(); }
+
+	//
 	// File / wire format (octree.h:776-864): whole map or the part inside an AABB, truncated at
 	// min_depth (0..4); compress = true packs the node stream as one LZ4 block like the reference
 	// (needs liblz4.so.1 at run time, else false).
@@ -1282,6 +1479,25 @@ class MapFacade
 		ufo_b200_query(map_, &c, &d, 1, &v.logodds, &v.flags, COLOR ? v.rgb : nullptr);
 		return v;
 	}
+	NNIterator nearest(bool leaves, Point3 const& coord, std::vector<ufo_b200_volume> bv, bool occupied, bool free_space,
+	                   bool unknown, bool contains, DepthType min_depth) const
+	{
+		auto s = std::make_shared<typename NNIterator::State>();
+		s->map = this;
+		for (int i = 0; i < 3; ++i) s->point[i] = coord[i];
+		s->bv = std::move(bv);
+		s->leaves = leaves;
+		s->occupied = occupied;
+		s->free_space = free_space;
+		s->unknown = unknown;
+		s->contains = contains;
+		s->min_depth = min_depth;
+		s->levels = getTreeDepthLevels();
+		for (DepthType d = 0; d < 22; ++d) s->half_size[d] = getNodeHalfSize(d);
+		s->occupied_thres_log = model()[0];
+		s->free_thres_log = model()[1];
+		return NNIterator(std::move(s));
+	}
 	Iterator iterate(bool leaves, std::vector<ufo_b200_volume> const& bv, bool occupied, bool free_space, bool unknown,
 	                 bool contains, DepthType min_depth) const
 	{
@@ -1472,7 +1688,7 @@ class MapFacade
 	ufo_b200_params params_{};
 	mutable double model_[6] = {0, 0, 0, 0, 0, 0};
 	bool minmax_enabled_ = false;
-	int last_status_ = 0;
+	mutable int last_status_ = 0;  // mutable: a nearest-first iterator reports a map changed under it
 };
 }  // namespace detail
 

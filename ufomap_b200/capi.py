@@ -113,6 +113,15 @@ class TreeStats(C.Structure):
                 ("known_max", C.c_double * 3), ("ms_device", C.c_float), ("reserved2", C.c_float)]
 
 
+class NearestStats(C.Structure):
+    """ufo_b200_nearest_stats: the work of the last nearest-first shell."""
+    _fields_ = [("bricks_visited", C.c_uint64), ("upper_visited", C.c_uint64), ("shells", C.c_uint32),
+                ("rebuilt", C.c_int32), ("revision", C.c_uint64), ("ms_device", C.c_float), ("ms_rebuild", C.c_float)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 # every symbol include/ufomap_b200.h declares
 SYMBOLS = [
     "ufo_b200_default_params", "ufo_b200_create", "ufo_b200_destroy", "ufo_b200_last_error",
@@ -140,6 +149,7 @@ SYMBOLS = [
     "ufo_b200_retain_bv", "ufo_b200_retain", "ufo_b200_page_out_bv", "ufo_b200_page_in", "ufo_b200_page_info",
     "ufo_b200_pool_stats", "ufo_b200_last_update_stats", "ufo_b200_image_part_bv", "ufo_b200_image_assemble",
     "ufo_b200_read_header", "ufo_b200_read", "ufo_b200_read_file", "ufo_b200_clone", "ufo_b200_tree_info",
+    "ufo_b200_nearest", "ufo_b200_last_nearest_stats",
 ]
 
 # ufo_b200_volume: one shape of a bounding volume (type in BoundingVar order, members in v)
@@ -355,6 +365,9 @@ def load():
     lib.ufo_b200_pool_stats.argtypes = [vp, C.POINTER(PoolCounts)]
     lib.ufo_b200_clone.argtypes = [vp, C.POINTER(vp)]
     lib.ufo_b200_tree_info.argtypes = [vp, C.POINTER(TreeStats)]
+    lib.ufo_b200_nearest.argtypes = [vp, vp, vp, sz, i32, i32, i32, i32, i32, u32, dbl, sz, vp, vp, vp, vp, vp, vp, sz,
+                                     C.POINTER(sz), C.POINTER(C.c_double)]
+    lib.ufo_b200_last_nearest_stats.argtypes = [vp, C.POINTER(NearestStats)]
     lib.ufo_b200_version.restype = C.c_char_p
     _lib = lib
     return lib
@@ -832,6 +845,44 @@ class Map:
                                                   C.byref(n)))
             assert n.value == cnt
         return codes, depths, occ, flags, rgb
+
+    def nearest(self, point, volume=None, leaves=True, occupied=True, free=True, unknown=False, contains=False,
+                min_depth=0, d2_from=0.0, want=1):
+        """One shell of beginNNLeaves (leaves=True) / beginNNTree from `point`: the nodes of iterate()
+        with d2_from <= d2 < d2_next, sorted by (d2, iterate's order), at least `want` of them unless
+        fewer remain.  Returns (codes, depths u8, logodds f32, flags u8, rgb u8[n,3], d2 f64, d2_next);
+        d2_next is +inf when the iteration is done.  Two library calls: one counts, one fills the arrays
+        (it repeats the search on the kept tree shape); last_nearest_stats() reports the first."""
+        bv, bp, nb = self._bv(volume)
+        pt = np.ascontiguousarray(point, np.float64).reshape(3)
+        args = (pt.ctypes.data, bp, nb, int(bool(leaves)), int(bool(occupied)), int(bool(free)), int(bool(unknown)),
+                int(bool(contains)), int(min_depth), float(d2_from), int(want))
+        n, nxt = C.c_size_t(), C.c_double()
+        self._check(self.lib.ufo_b200_nearest(self.h, *args, None, None, None, None, None, None, 0, C.byref(n),
+                                              C.byref(nxt)))
+        self._near_stats = NearestStats()
+        self._check(self.lib.ufo_b200_last_nearest_stats(self.h, C.byref(self._near_stats)))
+        cnt = n.value
+        codes, depths = np.empty(cnt, np.uint64), np.empty(cnt, np.uint8)
+        occ, flags = np.empty(cnt, np.float32), np.empty(cnt, np.uint8)
+        rgb, d2 = np.zeros((cnt, 3), np.uint8), np.empty(cnt, np.float64)
+        if cnt:
+            self._check(self.lib.ufo_b200_nearest(self.h, *args, codes.ctypes.data, depths.ctypes.data, occ.ctypes.data,
+                                                  flags.ctypes.data, rgb.ctypes.data if self.color else None,
+                                                  d2.ctypes.data, cnt, C.byref(n), C.byref(nxt)))
+            assert n.value == cnt
+        return codes, depths, occ, flags, rgb, d2, nxt.value
+
+    def nearest_shells(self, point, volume=None, want=1, **kw):
+        """Every shell of nearest() from d2 = 0 on, in order (a generator)."""
+        d2_from = 0.0
+        while d2_from != math.inf:
+            *shell, d2_from = self.nearest(point, volume, d2_from=d2_from, want=want, **kw)
+            yield tuple(shell)
+
+    def last_nearest_stats(self):
+        """ufo_b200_last_nearest_stats of the counting call of the last nearest()."""
+        return self._near_stats.as_dict()
 
     def set_value_volume_bv(self, shape, occupancy, min_depth=0):
         """setValueVolume(BoundingVar, occupancy probability, min_depth) for one shape record."""

@@ -22,6 +22,8 @@
 // bits of the block meta word) is written as eight voxels -- value-equivalent, larger.
 #pragma once
 
+#include <cuda/std/tuple>
+
 #include "ufo_device.cuh"
 #include "ufo_volume.cuh"
 
@@ -632,6 +634,105 @@ __global__ void __launch_bounds__(64) k_brick_info(DeviceMap M, uint32_t n_brick
 			if (m) atomicMax(&out->box[t - 4], m);
 		}
 	}
+}
+
+// ---------------------------------------------------------------------------
+// Nearest-first iteration (beginNNTree / beginNNLeaves, occupancy_map_base.h:169-245): the nodes of
+// beginTree / beginLeaves in non-decreasing squared distance from a point, delivered in shells
+// lo <= d2 < hi.  The distance is the reference's squaredDistance (iterator/octree_nearest.h:198-202):
+// the point minus the point clamped (std::clamp) to [centre - hs, centre + hs], then (x*x + y*y) + z*z,
+// all in doubles without contraction.  A child's cube lies inside its parent's, so no node is nearer
+// than its parent: a brick whose cube is at hi or beyond holds no node of the shell.
+UFO_HD double node_d2(const double p[3], const double c[3], double hs)
+{
+	double s[3];
+	for (int i = 0; i < 3; ++i) {
+		const double lo = dop::sub(c[i], hs), hi = dop::add(c[i], hs);
+		const double q = p[i] < lo ? lo : (hi < p[i] ? hi : p[i]);
+		s[i] = dop::sub(p[i], q);
+	}
+	return vsqnorm(Vec3{s[0], s[1], s[2]});
+}
+
+struct NearShell {
+	double p[3];
+	double lo, hi;
+};
+
+// Sort key of a shell record: d2 (non-negative, so its bits order as the value), then the order of
+// beginTree / beginLeaves -- code ascending, depth descending (codes are aligned to their depth).
+struct NearKey {
+	unsigned long long d2;
+	unsigned long long code;
+	uint8_t neg_depth;  // ~depth
+};
+
+struct NearKeyParts {
+	__host__ __device__ cuda::std::tuple<unsigned long long&, unsigned long long&, uint8_t&> operator()(NearKey& k) const
+	{
+		return {k.d2, k.code, k.neg_depth};
+	}
+};
+
+// The shell's records of the candidate bricks bricks[0, n): one CTA of 64 threads per brick runs the
+// descent of k_brick_iter (brick_descend / block_records, the brick's parent being descended into) and
+// keeps the records with lo <= d2 < hi.  They are appended at *count (one atomic per CTA), in no
+// particular order; records past cap are counted, not written, and the host repeats with room.
+template <bool COLOR, bool G>
+__global__ void __launch_bounds__(64) k_brick_nearest(DeviceMap M, const uint32_t* bricks, uint32_t n, IterArgs a, NearShell q,
+                                                      NearKey* keys, IterRec* recs, unsigned long long* count,
+                                                      unsigned long long cap)
+{
+	__shared__ BrickWalk S;
+	__shared__ uint32_t s_warp[2];
+	__shared__ unsigned long long s_base;
+	if (blockIdx.x >= n) return;
+	const uint32_t brick = bricks[blockIdx.x], t = threadIdx.x;
+	BlockShape B;
+	brick_descend<COLOR, G>(M, brick, a, S, B);
+	const uint32_t j3 = t >> 3, k3 = t & 7u;
+	const double bc[3] = {S.center[0], S.center[1], S.center[2]};
+	double c3[3];
+	child_center(bc, M.g.half_size[3], j3, c3);
+	const double d2_4 = t == 0 && S.ret4 ? node_d2(q.p, bc, M.g.half_size[4]) : 0.0;
+	const double d2_3 = k3 == 0 && S.ret3[j3] ? node_d2(q.p, c3, M.g.half_size[3]) : 0.0;
+	const bool keep4 = t == 0 && S.ret4 && q.lo <= d2_4 && d2_4 < q.hi;
+	const bool keep3 = k3 == 0 && S.ret3[j3] && q.lo <= d2_3 && d2_3 < q.hi;
+	const unsigned long long blk_code = S.rec4.code | ((unsigned long long)t << 6);
+	uint32_t mine = (keep4 ? 1u : 0u) + (keep3 ? 1u : 0u);
+	block_walk<COLOR, G>(M, a, S, B, blk_code, [&](uint32_t, const IterRec&, const double* c, uint32_t d) {
+		const double d2 = node_d2(q.p, c, M.g.half_size[d]);
+		if (q.lo <= d2 && d2 < q.hi) ++mine;
+	});
+	const uint32_t lane = t & 31u, warp = t >> 5;
+	uint32_t incl = mine;
+#pragma unroll
+	for (uint32_t off = 1; off < 32; off <<= 1) {
+		const uint32_t y = __shfl_up_sync(0xffffffffu, incl, off);
+		if (lane >= off) incl += y;
+	}
+	if (lane == 31) s_warp[warp] = incl;
+	__syncthreads();
+	if (t == 0) {
+		const uint32_t total = s_warp[0] + s_warp[1];
+		s_base = total ? atomicAdd(count, (unsigned long long)total) : 0ull;
+	}
+	__syncthreads();
+	if (!mine) return;
+	unsigned long long at = s_base + (incl - mine) + (warp ? s_warp[0] : 0u);
+	auto put = [&](const IterRec& r, double d2) {
+		if (at < cap) {
+			keys[at] = NearKey{(unsigned long long)__double_as_longlong(d2), r.code, (uint8_t)~((r.meta >> 24) & 31u)};
+			recs[at] = r;
+		}
+		++at;
+	};
+	if (keep4) put(S.rec4, d2_4);
+	if (keep3) put(S.rec3[j3], d2_3);
+	block_walk<COLOR, G>(M, a, S, B, blk_code, [&](uint32_t, const IterRec& r, const double* c, uint32_t d) {
+		const double d2 = node_d2(q.p, c, M.g.half_size[d]);
+		if (q.lo <= d2 && d2 < q.hi) put(r, d2);
+	});
 }
 
 // ---------------------------------------------------------------------------

@@ -16,7 +16,10 @@
 #include <dlfcn.h>
 
 #include <algorithm>
+#include <chrono>
+#include <functional>
 #include <numeric>
+#include <queue>
 #include <climits>
 #include <cmath>
 #include <cstdarg>
@@ -251,6 +254,11 @@ struct ufo_b200_map {
 	uint32_t route_parity = 0, route_cap_m = 0, route_cap_h = 0;
 	int route_stage = 0;  // 0 idle, 1 marked (waiting for the apply calls), 2 applied
 	double min_change[3], max_change[3];
+	// nearest-first iteration: every call that writes the pools or the thresholds bumps the revision;
+	// the tree shape above the bricks (TreeShape) is kept with the revision it was built at
+	uint64_t revision = 1;
+	std::shared_ptr<struct TreeShape> shape;
+	ufo_b200_nearest_stats nearest_stats{};
 	std::string err;
 	int sm_count = 132;
 	int ray_blocks_per_sm = 4, walk_blocks_per_sm = 4;
@@ -608,6 +616,9 @@ void keep_created(Map* m)
 // stamps are cleared to 0, and an id of 0 would make every brick or node look already listed.
 void new_scan_id(Map* m) { if (++m->M.scan_id == 0) m->M.scan_id = 1; }
 void new_up_epoch(Map* m) { if (++m->M.up_epoch == 0) m->M.up_epoch = 1; }
+// Every call that writes the pools or the thresholds: a tree shape kept for the nearest search is stale
+// from here on.
+void bump_revision(Map* m) { ++m->revision; }
 
 // depth 3 / 4 of the touched bricks from their blocks
 void launch_brick_agg(Map* m)
@@ -1921,6 +1932,7 @@ int ufo_b200_insert_pointcloud(ufo_b200_map* m, const double origin[3], const vo
                                int async)
 {
 	return guarded(m, [&]() {
+		bump_revision(m);
 		return do_insert(m, origin, points, false, n, nullptr, layout, max_range, depth,
 		                 simple_ray_casting, early_stopping, discrete, async);
 	});
@@ -1932,6 +1944,7 @@ int ufo_b200_insert_device(ufo_b200_map* m, const double origin[3], const void* 
                            int async)
 {
 	return guarded(m, [&]() {
+		bump_revision(m);
 		return do_insert(m, origin, d_points, true, n, nullptr, layout, max_range, depth,
 		                 simple_ray_casting, early_stopping, discrete, async);
 	});
@@ -1944,6 +1957,7 @@ int ufo_b200_insert_pointcloud_frame(ufo_b200_map* m, const double origin[3], co
 {
 	if (m && !frame_pose) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
+		bump_revision(m);
 		return do_insert(m, origin, points, false, n, frame_pose, layout, max_range, depth,
 		                 simple_ray_casting, early_stopping, discrete, async);
 	});
@@ -1955,6 +1969,7 @@ int ufo_b200_insert_pointcloud2(ufo_b200_map* m, const double origin[3], const u
 {
 	if (m && !cloud) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
+		bump_revision(m);
 		return do_insert(m, origin, cloud->data, cloud->on_device != 0, cloud->n, frame_pose, 4, max_range,
 		                 depth, simple_ray_casting, early_stopping, discrete, async, cloud);
 	});
@@ -2833,6 +2848,7 @@ int ufo_b200_set_value_volume(ufo_b200_map* m, const double box6[6], double occu
 {
 	if (!m || !box6) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
+		bump_revision(m);
 		const int allowed = set_value_volume_allowed(m, min_depth);
 		if (allowed != UFO_B200_OK) return allowed;
 		const Geometry& g = m->M.g;
@@ -2886,6 +2902,7 @@ int ufo_b200_set_value_volume_bv(ufo_b200_map* m, const ufo_b200_volume* bv, dou
 	const int allowed = set_value_volume_allowed(m, min_depth);
 	if (allowed != UFO_B200_OK) return allowed;
 	return guarded(m, [&]() {
+		bump_revision(m);
 		const Geometry& g = m->M.g;
 		const Volume hv{as_records(bv), 1, {}, {}};
 		const double c0[3] = {0.0, 0.0, 0.0};
@@ -3027,6 +3044,7 @@ int ufo_b200_set_sensor_model(ufo_b200_map* m, const double p[6])
 {
 	if (!m || !p) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
+		bump_revision(m);
 		sync_map(m);
 		m->occ_thr_log = to_logit(p[0]);
 		m->free_thr_log = to_logit(p[1]);
@@ -3044,6 +3062,7 @@ int ufo_b200_set_sensor_model_field(ufo_b200_map* m, int index, double probabili
 {
 	if (!m || index < 0 || index > 5) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
+		bump_revision(m);
 		sync_map(m);
 		double* field[6] = {&m->occ_thr_log, &m->free_thr_log, &m->hit_log, &m->miss_log, &m->cmin_log, &m->cmax_log};
 		*field[index] = to_logit(probability);
@@ -3155,6 +3174,7 @@ int ufo_b200_set_shard(ufo_b200_map* m, uint32_t rank, uint32_t world)
 {
 	if (!m || (world > 1 && rank >= world)) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
+		bump_revision(m);
 		sync_map(m);
 		if (m->n_bricks != 0) {
 			m->set_error("ufo_b200_set_shard must be called on an empty map");
@@ -3170,6 +3190,7 @@ int ufo_b200_clear(ufo_b200_map* m)
 {
 	if (!m) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() {
+		bump_revision(m);
 		CK(cudaSetDevice(m->device));
 		try {
 			sync_map(m);
@@ -3221,6 +3242,7 @@ int ufo_b200_clear_resize(ufo_b200_map* m, double resolution, uint32_t depth_lev
 	int rc = ufo_b200_clear(m);
 	if (rc != UFO_B200_OK) return rc;
 	return guarded(m, [&]() {
+		bump_revision(m);
 		m->params.resolution = resolution;
 		m->params.depth_levels = depth_levels;
 		m->M.g = make_geometry(resolution, depth_levels);
@@ -3294,6 +3316,7 @@ int ufo_b200_route_mark(ufo_b200_map* m, const double origin[3], const void* poi
                         double max_range, int on_device, int self_too)
 {
 	return guarded(m, [&]() {
+		bump_revision(m);
 		return do_route_mark(m, origin, points, on_device != 0, n, layout, max_range, 0, 0, 0, 0, 0, 1, self_too, false);
 	});
 }
@@ -3303,6 +3326,7 @@ int ufo_b200_route_mark_ex(ufo_b200_map* m, const double origin[3], const void* 
                            int discrete, uint64_t index_base, uint32_t index_stride, int on_device, int self_too)
 {
 	return guarded(m, [&]() {
+		bump_revision(m);
 		return do_route_mark(m, origin, points, on_device != 0, n, layout, max_range, depth, simple_ray_casting,
 		                     early_stopping, discrete, index_base, index_stride, self_too, true);
 	});
@@ -3325,7 +3349,7 @@ int ufo_b200_route_sent(ufo_b200_map* m, uint32_t counts[3])
 
 int ufo_b200_route_apply(ufo_b200_map* m, uint32_t first_source, uint32_t n_sources, int last)
 {
-	return guarded(m, [&]() { return do_route_apply(m, first_source, n_sources, last); });
+	return guarded(m, [&]() { bump_revision(m); return do_route_apply(m, first_source, n_sources, last); });
 }
 
 int ufo_b200_ipc_export(void* dev_ptr, void* handle64)
@@ -3692,13 +3716,14 @@ void iter_walk(IterWalk& w, int32_t idx, uint32_t d, unsigned long long code, co
 	}
 }
 
-// What iterate and tree_info share: `pass(d_info)` enqueues the size pass over the live bricks; their
-// info and keys come back, the bricks of the tree are sorted into Morton order, the shape above them is
-// built (build_upper), its nodes get their values (ufo_b200_query's) and iter_walk walks w.a over it.
-// w.plan must point at plan.
+// What iterate, tree_info and the nearest search share: `pass(d_info)` enqueues the size pass over the
+// live bricks; their info and keys come back, the bricks of the tree are sorted into Morton order, the
+// shape above them is built (build_upper) and its nodes get their values (ufo_b200_query's) in occ /
+// flags / rgb.  Returns false when no brick is part of the tree (plan.nodes stays empty).
 template <class Pass>
-void walk_above_bricks(Map* m, IterWalk& w, ExportPlan& plan, std::vector<BrickInfo>& info, std::vector<unsigned long long>& keys,
-                       std::vector<unsigned long long>& brick_codes, Pass&& pass)
+bool build_shape(Map* m, ExportPlan& plan, std::vector<BrickInfo>& info, std::vector<unsigned long long>& keys,
+                 std::vector<unsigned long long>& brick_codes, std::vector<float>& occ, std::vector<uint8_t>& flags,
+                 std::vector<uint32_t>& rgb, Pass&& pass)
 {
 	cudaStream_t s = m->stream;
 	const uint32_t nb = m->n_bricks;
@@ -3710,10 +3735,6 @@ void walk_above_bricks(Map* m, IterWalk& w, ExportPlan& plan, std::vector<BrickI
 	plan.g = &m->M.g;
 	info.assign(nb, BrickInfo{});
 	plan.info = info.data();
-	w.a.occ_thr = m->M.occ_thr;
-	w.a.free_thr = m->M.free_thr;
-	w.default_flags = m->M.default_flags;
-	w.offs.assign(nb, ~0ull);
 	DevBuf b_info, b_qcodes, b_qdepths, b_qocc, b_qflags, b_qrgb;
 	keys.assign(nb, 0ull);
 	if (nb) {
@@ -3743,18 +3764,15 @@ void walk_above_bricks(Map* m, IterWalk& w, ExportPlan& plan, std::vector<BrickI
 		plan.order[i] = sorted[i].second;
 	}
 	plan.codes = brick_codes.data();
-	if (sorted.empty()) {
-		iter_walk(w, -1, L, 0ull, c0, 0.0f, w.default_flags, 0u, true);
-		return;
-	}
+	if (sorted.empty()) return false;
 	build_upper(plan, L, 0, sorted.size(), c0);
 	// values of the nodes above the bricks: ufo_b200_query's, one batch
 	const size_t nu = plan.nodes.size();
 	std::vector<unsigned long long> qc(nu);
 	std::vector<uint32_t> qd(nu), qrgb(nu, 0u);
 	upper_codes(plan, 0, L, 0ull, qc, qd);
-	w.occ.resize(nu);
-	w.flags.resize(nu);
+	occ.resize(nu);
+	flags.resize(nu);
 	unsigned long long* d_qcodes = b_qcodes.alloc<unsigned long long>(nu);
 	uint32_t* d_qdepths = b_qdepths.alloc<uint32_t>(nu);
 	float* d_qocc = b_qocc.alloc<float>(nu);
@@ -3764,11 +3782,30 @@ void walk_above_bricks(Map* m, IterWalk& w, ExportPlan& plan, std::vector<BrickI
 	CK(cudaMemcpyAsync(d_qdepths, qd.data(), 4 * nu, cudaMemcpyHostToDevice, s));
 	k_query<<<(uint32_t)((nu + 255) / 256), 256, 0, s>>>(m->M, d_qcodes, d_qdepths, (uint32_t)nu, d_qocc, d_qflags, d_qrgb);
 	CK(cudaGetLastError());
-	CK(cudaMemcpyAsync(w.occ.data(), d_qocc, 4 * nu, cudaMemcpyDeviceToHost, s));
-	CK(cudaMemcpyAsync(w.flags.data(), d_qflags, nu, cudaMemcpyDeviceToHost, s));
+	CK(cudaMemcpyAsync(occ.data(), d_qocc, 4 * nu, cudaMemcpyDeviceToHost, s));
+	CK(cudaMemcpyAsync(flags.data(), d_qflags, nu, cudaMemcpyDeviceToHost, s));
 	if (color) CK(cudaMemcpyAsync(qrgb.data(), d_qrgb, 4 * nu, cudaMemcpyDeviceToHost, s));
 	CK(cudaStreamSynchronize(s));
-	w.rgb = std::move(qrgb);
+	rgb = std::move(qrgb);
+	return true;
+}
+
+// What iterate and tree_info share: build_shape, then iter_walk walks w.a over the shape.  w.plan must
+// point at plan.
+template <class Pass>
+void walk_above_bricks(Map* m, IterWalk& w, ExportPlan& plan, std::vector<BrickInfo>& info, std::vector<unsigned long long>& keys,
+                       std::vector<unsigned long long>& brick_codes, Pass&& pass)
+{
+	const uint32_t L = m->M.g.depth_levels;
+	const double c0[3] = {0.0, 0.0, 0.0};
+	w.a.occ_thr = m->M.occ_thr;
+	w.a.free_thr = m->M.free_thr;
+	w.default_flags = m->M.default_flags;
+	w.offs.assign(m->n_bricks, ~0ull);
+	if (!build_shape(m, plan, info, keys, brick_codes, w.occ, w.flags, w.rgb, pass)) {
+		iter_walk(w, -1, L, 0ull, c0, 0.0f, w.default_flags, 0u, true);
+		return;
+	}
 	const UpNode& r = plan.nodes[0];
 	iter_walk(w, 0, L, 0ull, c0, r.has ? w.occ[0] : r.occ, w.flags[0], r.has ? w.rgb[0] : r.rgb, !r.has);
 }
@@ -3957,6 +3994,248 @@ int tree_info(Map* m, ufo_b200_tree_stats* out)
 }
 }  // namespace
 
+// The pruned tree shape above the bricks with the values of its nodes (build_shape), kept on the map
+// for the nearest search and valid while the map's revision stays `revision`.
+struct TreeShape {
+	uint64_t revision = 0;
+	bool any = false;  // some brick is part of the tree (else the root is a default leaf)
+	ExportPlan plan;
+	std::vector<BrickInfo> info;
+	std::vector<unsigned long long> keys, brick_codes;
+	std::vector<float> occ;
+	std::vector<uint8_t> flags;
+	std::vector<uint32_t> rgb;
+};
+
+namespace
+{
+// the shape for the map's current revision: built by the first call after a change, kept after that
+const TreeShape& current_shape(Map* m, bool* rebuilt)
+{
+	*rebuilt = false;
+	if (m->shape && m->shape->revision == m->revision) return *m->shape;
+	m->shape.reset();
+	auto sh = std::make_shared<TreeShape>();
+	const uint32_t nb = m->n_bricks;
+	cudaStream_t s = m->stream;
+	IterArgs da{};  // the size pass is run for the shape and the brick payloads only
+	da.occ_thr = m->M.occ_thr;
+	da.free_thr = m->M.free_thr;
+	da.occupied = da.free_ = da.unknown = 1;
+	sh->any = build_shape(m, sh->plan, sh->info, sh->keys, sh->brick_codes, sh->occ, sh->flags, sh->rgb, [&](BrickInfo* d_info) {
+		if (m->M.color) k_brick_iter<true, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, nullptr, nullptr);
+		else k_brick_iter<false, false><<<nb, 64, 0, s>>>(m->M, nb, da, d_info, nullptr, nullptr);
+		++m->launches;
+	});
+	sh->plan.info = sh->info.data();
+	sh->plan.codes = sh->brick_codes.data();
+	sh->revision = m->revision;
+	m->shape = std::move(sh);
+	*rebuilt = true;
+	return *m->shape;
+}
+
+// One entry of the host search: a node above the bricks (idx into plan.nodes), a default leaf (idx < 0)
+// or, at depth 4, a brick of the tree (idx = its slot).
+struct NearItem {
+	double d2;
+	int32_t idx;
+	uint32_t d;
+	unsigned long long code;
+	double c[3];
+	bool operator>(const NearItem& o) const { return d2 > o.d2; }
+};
+
+struct NearOut {
+	double d2;
+	IterRec r;
+};
+
+bool near_less(const NearOut& x, const NearOut& y)
+{
+	if (x.d2 != y.d2) return x.d2 < y.d2;
+	if (x.r.code != y.r.code) return x.r.code < y.r.code;
+	return ((x.r.meta >> 24) & 31u) > ((y.r.meta >> 24) & 31u);
+}
+
+// One shell of the nearest-first iteration.  The host runs a best-first search over the cached shape
+// above the bricks with iter_walk's rules: it keeps the returned nodes of depth >= 5 (and default leaves)
+// and collects the bricks in order of their cube's distance.  It stops once the nodes and bricks it has
+// taken reach a target count; hi is then the key of the nearest entry not taken.  A key is a lower bound
+// of the distance of every node below the entry: the entry's own distance, lowered by a slack far above
+// the rounding of the accumulated centres (a child's cube can stick out of its parent's by an ulp).  So
+// every node nearer than hi lies in a taken brick or was taken itself, and the shell, cut at the nodes'
+// own distances, never misses one.  k_brick_nearest takes the shell's records out of
+// the taken bricks; when the shell holds fewer than `want` nodes the target doubles and the bricks are
+// searched again with the larger hi.
+int nearest(Map* m, const double p[3], const IterArgs& args, double lo, size_t want, std::vector<NearOut>& out, double* hi_out)
+{
+	out.clear();
+	*hi_out = INFINITY;
+	ufo_b200_nearest_stats& st = m->nearest_stats;
+	st = ufo_b200_nearest_stats{};
+	if (m->M.g.depth_levels < 5) {
+		m->set_error("nearest iteration needs depth_levels >= 5");
+		return UFO_B200_E_UNSUPPORTED;
+	}
+	CK(cudaSetDevice(m->device));
+	sync_map(m);
+	st.revision = m->revision;
+	const uint32_t L = m->M.g.depth_levels;
+	const Geometry& g = m->M.g;
+	const double c0[3] = {0.0, 0.0, 0.0};
+	if (args.min_depth > L || !vol_hits(args.vol, c0, g.half_size[L]) || !(lo < INFINITY)) return UFO_B200_OK;
+	cudaStream_t s = m->stream;
+	const auto t0 = std::chrono::steady_clock::now();
+	bool rebuilt = false;
+	const TreeShape& sh = current_shape(m, &rebuilt);
+	st.rebuilt = rebuilt ? 1 : 0;
+	if (rebuilt) st.ms_rebuild = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+	const ExportPlan& plan = sh.plan;
+	IterArgs a = args;
+	a.occ_thr = m->M.occ_thr;
+	a.free_thr = m->M.free_thr;
+	const uint32_t dfl = m->M.default_flags;
+
+	const double slack = 1e-9 * (g.half_size[L] + std::max(std::fabs(p[0]), std::max(std::fabs(p[1]), std::fabs(p[2]))));
+	auto key = [&](double d2) {
+		const double r = std::sqrt(d2) - slack;
+		return r > 0.0 ? r * r : 0.0;
+	};
+	std::priority_queue<NearItem, std::vector<NearItem>, std::greater<NearItem>> heap;
+	heap.push(NearItem{key(node_d2(p, c0, g.half_size[L])), sh.any ? 0 : -1, L, 0ull, {0.0, 0.0, 0.0}});
+	std::vector<uint32_t> bricks;  // taken, by slot
+	size_t taken = 0, kept = 0;
+	double last = -INFINITY;
+	auto take = [&]() {
+		const NearItem it = heap.top();
+		heap.pop();
+		last = it.d2;
+		if (it.d == 4 && it.idx >= 0) {
+			bricks.push_back((uint32_t)it.idx);
+			if (it.d2 >= lo) ++taken;
+			return;
+		}
+		++st.upper_visited;
+		const UpNode* n = it.idx >= 0 ? &plan.nodes[it.idx] : nullptr;
+		const bool leaf = !n || !n->has;
+		const float v = !n ? 0.0f : (n->has ? sh.occ[it.idx] : n->occ);
+		const uint32_t fl = n ? sh.flags[it.idx] : dfl;
+		const uint32_t rgb = !n ? 0u : (n->has ? sh.rgb[it.idx] : n->rgb);
+		if (!vol_hits(a.vol, it.c, g.half_size[it.d]) || !iter_valid(a, it.d, v, fl)) return;
+		const double d2 = node_d2(p, it.c, g.half_size[it.d]);
+		if (iter_returns(a, it.d, leaf, v, fl) && d2 >= lo) {
+			out.push_back(NearOut{d2, iter_rec(it.code, v, rgb, it.d, fl, leaf)});
+			++taken;
+		}
+		if (it.d <= a.min_depth || leaf) return;
+		for (uint32_t i = 0; i < 8; ++i) {
+			NearItem c{};
+			c.d = it.d - 1;
+			child_center(it.c, g.half_size[c.d], i, c.c);
+			c.code = it.code | ((unsigned long long)i << (3 * c.d));
+			c.d2 = key(node_d2(p, c.c, g.half_size[c.d]));
+			const int32_t ch = n->child[i];
+			c.idx = ch < 0 ? -1 : (it.d == 5 ? (int32_t)plan.order[ch] : ch);
+			heap.push(c);
+		}
+	};
+
+	const bool color = m->M.color != 0;
+	Volume hv = args.vol;
+	const bool general = volume_is_general(hv);
+	DeviceVolume dvol;
+	IterArgs da = a;
+	da.vol = dvol.upload(hv, s);
+	DevBuf b_bricks, b_count, b_keys[2], b_recs[2], b_tmp;
+	unsigned long long* d_count = b_count.alloc<unsigned long long>(1);
+	size_t rec_cap = 0;
+	NearKey* d_keys[2] = {nullptr, nullptr};
+	IterRec* d_recs[2] = {nullptr, nullptr};
+	Events ev;
+	bool timed = false;
+	std::vector<IterRec> dev_recs;
+	std::vector<NearKey> dev_keys;
+	want = std::max<size_t>(want, 1);
+	size_t target = want;
+	double hi = INFINITY;
+	for (;;) {
+		while (!heap.empty() && taken < target) take();
+		while (!heap.empty() && heap.top().d2 <= last) take();  // hi above every key taken
+		hi = heap.empty() ? INFINITY : heap.top().d2;
+		// the nodes taken above the bricks that lie beyond hi belong to a later shell
+		kept = (size_t)std::count_if(out.begin(), out.end(), [&](const NearOut& r) { return r.d2 < hi; });
+		unsigned long long cnt = 0;
+		if (!bricks.empty()) {
+			const uint32_t nbk = (uint32_t)bricks.size();
+			uint32_t* d_bricks = b_bricks.alloc<uint32_t>(nbk);
+			CK(cudaMemcpyAsync(d_bricks, bricks.data(), 4ull * nbk, cudaMemcpyHostToDevice, s));
+			const NearShell q{{p[0], p[1], p[2]}, lo, hi};
+			for (;;) {
+				CK(cudaMemsetAsync(d_count, 0, 8, s));
+				if (!timed) CK(cudaEventRecord(ev.e[0], s));
+				timed = true;
+				if (color && general)
+					k_brick_nearest<true, true><<<nbk, 64, 0, s>>>(m->M, d_bricks, nbk, da, q, d_keys[0], d_recs[0], d_count, rec_cap);
+				else if (color)
+					k_brick_nearest<true, false><<<nbk, 64, 0, s>>>(m->M, d_bricks, nbk, da, q, d_keys[0], d_recs[0], d_count, rec_cap);
+				else if (general)
+					k_brick_nearest<false, true><<<nbk, 64, 0, s>>>(m->M, d_bricks, nbk, da, q, d_keys[0], d_recs[0], d_count, rec_cap);
+				else
+					k_brick_nearest<false, false><<<nbk, 64, 0, s>>>(m->M, d_bricks, nbk, da, q, d_keys[0], d_recs[0], d_count, rec_cap);
+				CK(cudaGetLastError());
+				++m->launches;
+				st.bricks_visited += nbk;
+				++st.shells;
+				CK(cudaMemcpyAsync(&cnt, d_count, 8, cudaMemcpyDeviceToHost, s));
+				CK(cudaStreamSynchronize(s));
+				if (cnt <= rec_cap) break;
+				rec_cap = std::max<size_t>(cnt, 2 * rec_cap);  // room for the whole shell, then again
+				for (int i = 0; i < 2; ++i) {
+					d_keys[i] = b_keys[i].alloc<NearKey>(rec_cap);
+					d_recs[i] = b_recs[i].alloc<IterRec>(rec_cap);
+				}
+			}
+		}
+		if (kept + cnt >= want || heap.empty()) {
+			*hi_out = hi;
+			if (cnt) {
+				// (d2, code, ~depth), then one copy back
+				size_t tmp_bytes = 0;
+				CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_keys[0], d_keys[1], d_recs[0], d_recs[1], (int)cnt,
+				                                   NearKeyParts{}, s));
+				void* d_tmp = b_tmp.alloc<unsigned char>(tmp_bytes);
+				CK(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_keys[0], d_keys[1], d_recs[0], d_recs[1], (int)cnt,
+				                                   NearKeyParts{}, s));
+				++m->launches;
+				dev_keys.resize(cnt);
+				dev_recs.resize(cnt);
+				CK(cudaMemcpyAsync(dev_keys.data(), d_keys[1], sizeof(NearKey) * cnt, cudaMemcpyDeviceToHost, s));
+				CK(cudaMemcpyAsync(dev_recs.data(), d_recs[1], sizeof(IterRec) * cnt, cudaMemcpyDeviceToHost, s));
+			}
+			if (timed) CK(cudaEventRecord(ev.e[1], s));
+			CK(cudaStreamSynchronize(s));
+			if (timed) CK(cudaEventElapsedTime(&st.ms_device, ev.e[0], ev.e[1]));
+			break;
+		}
+		target = 2 * std::max(target, taken);
+	}
+	// merge the records of the levels above the bricks (few) into the sorted brick records
+	out.erase(std::remove_if(out.begin(), out.end(), [&](const NearOut& r) { return !(r.d2 < hi); }), out.end());
+	std::sort(out.begin(), out.end(), near_less);
+	std::vector<NearOut> dev(dev_recs.size());
+	for (size_t i = 0; i < dev.size(); ++i) {
+		double d2;
+		std::memcpy(&d2, &dev_keys[i].d2, 8);
+		dev[i] = NearOut{d2, dev_recs[i]};
+	}
+	std::vector<NearOut> merged(out.size() + dev.size());
+	std::merge(out.begin(), out.end(), dev.begin(), dev.end(), merged.begin(), near_less);
+	out.swap(merged);
+	return UFO_B200_OK;
+}
+}  // namespace
+
 extern "C" {
 
 int ufo_b200_iterate(ufo_b200_map* m, int leaves_only, int occupied, int free_space, int unknown, int contains, uint32_t min_depth,
@@ -3984,6 +4263,61 @@ int ufo_b200_tree_info(ufo_b200_map* m, ufo_b200_tree_stats* out)
 {
 	if (!m || !out) return UFO_B200_E_INVALID;
 	return guarded(m, [&]() { return tree_info(m, out); });
+}
+
+int ufo_b200_nearest(ufo_b200_map* m, const double point[3], const ufo_b200_volume* bv, size_t n_bv, int leaves_only,
+                     int occupied, int free_space, int unknown, int contains, uint32_t min_depth, double d2_from,
+                     size_t want, uint64_t* codes, uint8_t* depths, float* logodds, uint8_t* flags, uint8_t* rgb,
+                     double* d2, size_t cap, size_t* n, double* d2_next)
+{
+	if (!m || !n || !d2_next || !point) return UFO_B200_E_INVALID;
+	*n = 0;
+	*d2_next = INFINITY;
+	if (cap && (!codes || !depths || !logodds || !flags || !d2)) return UFO_B200_E_INVALID;
+	if (!std::isfinite(point[0]) || !std::isfinite(point[1]) || !std::isfinite(point[2]) || std::isnan(d2_from)) {
+		m->set_error("nearest: the point must be finite and d2_from a number");
+		return UFO_B200_E_INVALID;
+	}
+	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
+	return guarded(m, [&]() {
+		IterArgs a{};
+		a.vol = Volume{as_records(bv), (uint32_t)n_bv, {}, {}};
+		a.min_depth = min_depth;
+		a.leaves_only = leaves_only != 0;
+		a.occupied = occupied != 0;
+		a.free_ = free_space != 0;
+		a.unknown = unknown != 0;
+		a.contains = contains != 0;
+		std::vector<NearOut> recs;
+		double hi = INFINITY;
+		const int rc = nearest(m, point, a, d2_from, want, recs, &hi);
+		if (rc != UFO_B200_OK) return rc;
+		*n = recs.size();
+		*d2_next = hi;
+		if (codes && !recs.empty() && recs.size() <= cap) {
+			for (size_t i = 0; i < recs.size(); ++i) {
+				const IterRec& r = recs[i].r;
+				codes[i] = r.code;
+				depths[i] = (uint8_t)((r.meta >> 24) & 31u);
+				logodds[i] = r.occ;
+				flags[i] = (uint8_t)(r.meta >> 29);
+				d2[i] = recs[i].d2;
+				if (rgb) {
+					rgb[3 * i] = (uint8_t)r.meta;
+					rgb[3 * i + 1] = (uint8_t)(r.meta >> 8);
+					rgb[3 * i + 2] = (uint8_t)(r.meta >> 16);
+				}
+			}
+		}
+		return (int)UFO_B200_OK;
+	});
+}
+
+int ufo_b200_last_nearest_stats(ufo_b200_map* m, ufo_b200_nearest_stats* out)
+{
+	if (!m || !out) return UFO_B200_E_INVALID;
+	*out = m->nearest_stats;
+	return UFO_B200_OK;
 }
 
 }  // extern "C"
@@ -4618,6 +4952,7 @@ int ufo_b200_read_data_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_b
 		return UFO_B200_E_INVALID;
 	}
 	return guarded(m, [&]() {
+		bump_revision(m);
 		const Volume vol{as_records(bv), (uint32_t)n_bv};
 		if (!compressed) return import_stream(m, static_cast<const uint8_t*>(data), size, vol);
 		std::vector<uint8_t> raw;
@@ -4648,7 +4983,7 @@ int ufo_b200_read(ufo_b200_map* m, const void* image, size_t size)
 		m->set_error("read between ufo_b200_route_mark and the last ufo_b200_route_apply of the pass");
 		return UFO_B200_E_INVALID;
 	}
-	return guarded(m, [&]() { return read_image(m, static_cast<const uint8_t*>(image), size); });
+	return guarded(m, [&]() { bump_revision(m); return read_image(m, static_cast<const uint8_t*>(image), size); });
 }
 
 int ufo_b200_read_file(ufo_b200_map* m, const char* filename)
@@ -4659,6 +4994,7 @@ int ufo_b200_read_file(ufo_b200_map* m, const char* filename)
 		return UFO_B200_E_INVALID;
 	}
 	return guarded(m, [&]() {
+		bump_revision(m);
 		FILE* f = fopen(filename, "rb");
 		if (!f) {
 			m->set_error("cannot open %s", filename);
@@ -4787,6 +5123,7 @@ int write_nodes(Map* m, const uint64_t* codes, const uint32_t* depths, const uin
                 const uint8_t* rgb, size_t n, int async)
 {
 	return guarded(m, [&]() {
+		bump_revision(m);
 		CK(cudaSetDevice(m->device));
 		const Geometry& g = m->M.g;
 		std::vector<unsigned long long> offs(n + 1);
@@ -4889,6 +5226,7 @@ int ufo_b200_insert_rays(ufo_b200_map* m, const double* origins, const double* e
 	const int rc = write_allowed(m, depth);
 	if (rc != UFO_B200_OK) return rc;
 	return guarded(m, [&]() {
+		bump_revision(m);
 		CK(cudaSetDevice(m->device));
 		const Geometry& g = m->M.g;
 		// record region of every ray: an upper bound of the walk's records.  Every step of the walk
@@ -5427,7 +5765,7 @@ int ufo_b200_retain_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv, 
 {
 	if (!m) return UFO_B200_E_INVALID;
 	if (!volume_ok(m, bv, n_bv)) return UFO_B200_E_INVALID;
-	return guarded(m, [&]() { return retain(m, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, out); });
+	return guarded(m, [&]() { bump_revision(m); return retain(m, Volume{as_records(bv), (uint32_t)n_bv, {}, {}}, out); });
 }
 
 int ufo_b200_retain(ufo_b200_map* m, const double box6[6], ufo_b200_retain_stats* out)
@@ -5447,7 +5785,7 @@ int ufo_b200_page_out_bv(ufo_b200_map* m, const ufo_b200_volume* bv, size_t n_bv
 int ufo_b200_page_in(ufo_b200_map* m, const void* blob, size_t size, ufo_b200_retain_stats* out)
 {
 	if (!m || (!blob && size)) return UFO_B200_E_INVALID;
-	return guarded(m, [&]() { return page_in(m, blob, size, out); });
+	return guarded(m, [&]() { bump_revision(m); return page_in(m, blob, size, out); });
 }
 
 int ufo_b200_page_info(const void* blob, size_t size, ufo_b200_page_header* out)
