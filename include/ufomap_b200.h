@@ -523,7 +523,7 @@ typedef struct {
 	uint64_t blocks_in_map;   /* pool occupancy                            */
 	uint64_t bricks_in_map;
 	uint64_t device_bytes;    /* device memory held by the map             */
-	uint64_t regrows;         /* pool growth events during this insert     */
+	uint64_t regrows;         /* pool growth events during this insert (routed: mark and apply phases of the pass) */
 	uint64_t launches;        /* kernels launched by this insert           */
 	uint64_t result_bytes;    /* bytes of per-scan counters copied device -> host by this insert */
 	uint64_t touched_lines;   /* 128-byte lines of leaf data the update read (HBM moves whole lines): lines holding a touched octet, less saturated lines (ufo_b200_last_update_stats) */
@@ -628,7 +628,9 @@ int ufo_b200_set_shard(ufo_b200_map* m, uint32_t rank, uint32_t world);
  *                           control plane, e.g. torch.distributed.all_gather_object)
  *   ufo_b200_route_connect  peer_inboxes[r] = device pointer of rank r's inbox as seen from this
  *                           process (its own for r == rank)
- *   ufo_b200_route_mark     enqueue: H2D, K1, fused walk, forwarding of foreign marks.  self_too != 0:
+ *   ufo_b200_route_mark     H2D, K1, fused walk, then a wait for the marking kernels: if a pool ran
+ *                           full, it grows and the marking runs again before anything is
+ *                           published; then enqueues the forwarding of foreign marks.  self_too != 0:
  *                           the rank's own marks go through its inbox as well, which lets the
  *                           owner apply several sensors one after the other (clamping makes the
  *                           order matter).  Mono maps, insert depth 0, plain insertion; a colour
@@ -650,8 +652,13 @@ int ufo_b200_set_shard(ufo_b200_map* m, uint32_t rank, uint32_t world);
  *                           whole-brick records and hit records this rank wrote into inboxes
  *                           (its own included) in its last mark pass
  * The union of the ranks' value fields equals the single-GPU map (tests/test_gpu_route.py,
- * tests/test_gpu_route_discrete.py).  Pools do not grow during a routed pass: size the map with
- * initial_bricks.  Maps that have seen out-of-tree keys are rejected.  Between passes the ranks
+ * tests/test_gpu_route_discrete.py).  Pools grow during a routed pass as on one map, so
+ * initial_bricks is a starting size: route_mark grows them while marking (above), and an apply call
+ * whose pool runs full backs off with the later calls of the pass, which are replayed in their order
+ * after the growth at the rank's next synchronising call (the next route_mark, wait, a query or a
+ * writer).  ufo_b200_last_scan_stats.regrows counts the growths of both phases of the last pass.
+ * The inbox does not grow: a region too small for a pass is UFO_B200_E_NOMEM at the next
+ * synchronising call.  Maps that have seen out-of-tree keys are rejected.  Between passes the ranks
  * also take setValueVolume, write batches and readData (each applies what it owns; pools grow there
  * as on one map), and ufo_b200_image_part_bv / ufo_b200_image_assemble give the union's file image. */
 int ufo_b200_route_inbox_bytes(uint32_t world, uint32_t cap_bricks, uint32_t cap_hits, size_t* bytes);

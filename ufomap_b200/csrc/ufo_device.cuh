@@ -50,6 +50,7 @@ struct Counters {
 	uint32_t k3_cursor;    // touched entries claimed by k_update_brick's warps beyond their first (zeroed before each launch)
 	uint32_t max_span;     // longest ray of the scan in dominant-axis steps (sets the shell thickness)
 	uint32_t n_touched_alt;  // routed mode: length of DeviceMap::touched_alt
+	uint32_t route_call;     // routed mode: the last apply call of the pass whose k_inbox ran (did not back off)
 	uint32_t n_dirty;        // dense mode: length of DeviceMap::vol_list (also: node list of insert depth 5/6, bricks of a write batch)
 	uint32_t list_count[3];  // dirty-list lengths of the upper-level pass (rotating by depth % 3)
 	uint32_t n_rays;

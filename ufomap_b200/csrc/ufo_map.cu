@@ -120,8 +120,14 @@ struct PendingScan {
 	bool valid = false;
 	ScanArgs a{};
 	bool use_color = false, need_table = false, simple = false, has_vol = false;
-	bool routed = false;  // routed multi-GPU pass: cannot be repeated locally after a pool overflow
+	bool routed = false;  // routed multi-GPU pass (ufo_route.cuh)
 	bool applying = false;  // routed pass: the first apply call has run
+	// routed pass: the apply calls enqueued so far (sources, scan id), replayed in their order from the
+	// first one that backed off after a pool growth
+	struct RouteCall {
+		uint32_t first, count, scan_id;
+	};
+	std::vector<RouteCall> calls;
 	bool dense = false;   // marks go to the dense scan volume
 	VolumeArgs vol{};
 	float set_value = 0.0f;
@@ -600,6 +606,9 @@ void grow_pools(Map* m, uint32_t overflow, uint32_t want_bricks, uint32_t want_u
 		M.up_cap = nc;
 		upper_hash(m, std::min(m->h_ctr->n_upper, oc));
 	}
+	// a pass that continues after the growth (the routed mark and apply phases) reads its masks
+	// through mask_base, which points into the old miss_mask unless the pass marks into the volume
+	M.mask_base = M.dense ? M.vol : M.miss_mask;
 	CK(cudaGetLastError());
 }
 
@@ -1242,6 +1251,77 @@ void enqueue_scan(Map* m, PendingScan& p)
 	p.valid = true;
 }
 
+// k_inbox, its colour pass and K3 of apply call `call` of a routed pass (ufo_route.cuh)
+void enqueue_route_call(Map* m, uint32_t call)
+{
+	DeviceMap& M = m->M;
+	cudaStream_t s = m->stream;
+	const PendingScan::RouteCall& c = m->pending.calls[call];
+	ScanArgs t{};
+	if (M.color) {
+		// apply table for the hit records of these sources: at most count * cap_h keys, half full
+		const uint32_t size = std::min(m->route_tab_size, std::max(1u << 12, next_pow2(2ull * c.count * m->route_cap_h)));
+		CK(cudaMemsetAsync(m->d_route_tab_keys.p, 0xff, (size_t)size * sizeof(unsigned long long), s));
+		CK(cudaMemsetAsync(m->d_route_tab_min.p, 0xff, (size_t)size * sizeof(uint32_t), s));
+		t.tab_keys = m->d_route_tab_keys.p;
+		t.tab_min = m->d_route_tab_min.p;
+		t.tab_mask = size - 1;
+	}
+	k_inbox<<<m->sm_count * 4, 256, 0, s>>>(M, c.first, c.count, t, call);
+	++m->launches;
+	if (M.color) {
+		k_inbox_color<<<m->sm_count * 4, 256, 0, s>>>(M, c.first, c.count, t);
+		++m->launches;
+	}
+	launch_update(m, m->pending.a.miss, false);
+}
+
+// A routed pass whose apply calls ran into a full pool (overflow flags `ov`; keep_created has run).
+// k_inbox of call route_call could not place every record, and from there on K3, the upper seeds
+// and the later calls backed off.  Grows the pools and replays those calls in their order under
+// their own scan ids: the failed call keeps the touched list it built (its bricks carry its scan id,
+// so touching them again lists nothing twice) and ORs its masks in again.  The inbox regions they
+// read stay valid until the peers' mark of pass k+2 (DESIGN.md section 6).  The upper levels are then
+// propagated again, under a new epoch, from every brick the pass's calls touched: the seeds of the
+// calls that backed off are lost, and the levels of the last call already ran over the seeds before
+// them.  A full upper-node pool alone takes the same propagation.  Leaves the counters' read-back
+// in flight.
+void regrow_routed(Map* m, uint32_t ov)
+{
+	DeviceMap& M = m->M;
+	cudaStream_t s = m->stream;
+	PendingScan& p = m->pending;
+	const uint32_t from = m->h_ctr->route_call;
+	grow_pools(m, ov, m->h_ctr->n_bricks, m->h_ctr->n_upper);
+	// allocation cursors back to the slots kept, flags cleared; the touched list and statistics stay
+	static_assert(offsetof(Counters, overflow) == offsetof(Counters, n_bricks) + 2 * sizeof(uint32_t), "cursor layout");
+	m->h_ctr->n_bricks = m->n_bricks;
+	m->h_ctr->n_upper = m->n_upper;
+	m->h_ctr->overflow = 0;
+	CK(cudaMemcpyAsync(&M.ctr->n_bricks, &m->h_ctr->n_bricks, 3 * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+	if (ov & 2u) {
+		for (uint32_t k = from; k < p.calls.size(); ++k) {
+			M.scan_id = p.calls[k].scan_id;
+			if (k != from) k_route_next_apply<<<1, 1, 0, s>>>(M.ctr);
+			enqueue_route_call(m, k);
+		}
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		if (m->h_ctr->overflow) return;  // full again: the caller grows and replays once more
+		keep_created(m);
+	}
+	new_up_epoch(m);
+	k_reset_upper_pass<<<1, 1, 0, s>>>(M.ctr, m->n_upper);
+	CK(cudaMemsetAsync(&M.ctr->n_touched, 0, sizeof(uint32_t), s));
+	const uint32_t first = p.calls.front().scan_id;
+	k_touch_pass<<<m->sm_count * 4, 256, 0, s>>>(M, m->n_bricks, first, p.calls.back().scan_id - first + 1u);
+	launch_upper(m);
+	m->launches += 2;
+	CK(cudaEventRecord(m->ev[6], s));
+	CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+}
+
 // Waits for the scan in flight, repeats it if a device pool overflowed, and folds its counters
 // into the host view.  Throws MapError if the scan cannot be completed.
 void finalize_scan(Map* m)
@@ -1270,10 +1350,10 @@ void finalize_scan(Map* m)
 		const uint32_t ov = m->h_ctr->overflow;
 		if (!ov) break;
 		++p.regrows;
-		if (p.regrows > 16 || (ov & (16u | 128u)) || p.routed) {
+		if (p.regrows > 16 || (ov & (16u | 128u)) || (p.routed && (ov & ~6u))) {
 			if (ov & 128u) m->set_error("insert depth >= 5 with rays that leave the map (out-of-tree nodes) is not supported");
 			else if (ov & 16u) m->set_error("internal error: a ray walk exceeded its record bound");
-			else if (p.routed) m->set_error("routed mode: a device pool overflowed (flags %u); create the map with a larger initial_bricks", ov);
+			else if (p.routed && (ov & ~6u)) m->set_error("routed mode: an apply call failed (overflow flags %u)", ov);
 			else m->set_error("device pools keep overflowing");
 			p.valid = false;
 			m->stats_pending = false;
@@ -1282,7 +1362,9 @@ void finalize_scan(Map* m)
 		}
 		try {
 			keep_created(m);
-			if (ov == 4u) {
+			if (p.routed) {
+				regrow_routed(m, ov);
+			} else if (ov == 4u) {
 				// only the upper-node pool overflowed: the leaves are updated, repeat the propagation
 				grow_pools(m, 4u, 0, m->h_ctr->n_upper);
 				new_up_epoch(m);
@@ -1633,9 +1715,6 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 	a.points = on_device ? points : m->d_points[stg].p;
 	if (copied) m->stage = stg;
 	bind_scan_buffers(m, p, fused);
-	// a routed pass cannot be repeated after a record buffer overflow: K1 reserves without a
-	// bound, and the buffer is sized to the reservation before the walk (below)
-	if (records) a.seg_cap = ~0ull;
 	m->stats = ufo_b200_scan_stats{};
 	m->stats.points = n;
 	m->launches = 0;
@@ -1646,37 +1725,65 @@ int do_route_mark(Map* m, const double origin[3], const void* points, bool on_de
 	route_fill_table(m);
 	m->h_route_flag[0] = 0;
 	CK(cudaEventRecord(m->ev[0], s));
-	CK(cudaMemcpyAsync(M.route, m->h_route, sizeof(RouteTable), cudaMemcpyHostToDevice, s));
 	if (copied) CK(cudaStreamWaitEvent(s, m->ev_copied, 0));
-	new_scan_id(m);
-	push_counters(m);
-	if (p.need_table) {
-		CK(cudaMemsetAsync(m->d_tab_keys.p, 0xff, (size_t)m->tab_size * sizeof(unsigned long long), s));
-		CK(cudaMemsetAsync(m->d_tab_min.p, 0xff, (size_t)m->tab_size * sizeof(uint32_t), s));
-	}
-	if (n) {
-		const uint32_t grid = (uint32_t)((n + 255) / 256);
-		k_points<<<grid, 256, 0, s>>>(M, a);
-		++m->launches;
-		if (use_color) {
-			k_route_hits<<<grid, 256, 0, s>>>(M, a, (unsigned long long)index_base, index_stride);
+	// Marking creates bricks, own and foreign, and K1 and k_expand_nodes write hit records straight
+	// into the peers' inboxes, which the peers read right after the barrier.  So the marking is waited
+	// for here: if a pool ran full, it grows and the marking runs again under a new scan id (OR into
+	// masks, find-or-create of bricks: idempotent) from fresh outbox cursors (the table push), and
+	// only the complete pass is published.
+	const auto fail = [&](const char* why) {
+		m->set_error("%s", why);
+		p.valid = false;
+		m->poisoned = true;  // the marks of the failed attempt are still in the masks
+		m->route_stage = 0;
+		throw MapError{UFO_B200_E_NOMEM};
+	};
+	for (;;) {
+		CK(cudaMemcpyAsync(M.route, m->h_route, sizeof(RouteTable), cudaMemcpyHostToDevice, s));
+		new_scan_id(m);
+		push_counters(m);
+		if (p.need_table) {
+			CK(cudaMemsetAsync(m->d_tab_keys.p, 0xff, (size_t)m->tab_size * sizeof(unsigned long long), s));
+			CK(cudaMemsetAsync(m->d_tab_min.p, 0xff, (size_t)m->tab_size * sizeof(uint32_t), s));
+		}
+		if (n) {
+			const uint32_t grid = (uint32_t)((n + 255) / 256);
+			// K1 reserves the walk's records without a bound; the buffer is sized to the reservation
+			if (records) a.seg_cap = ~0ull;
+			k_points<<<grid, 256, 0, s>>>(M, a);
 			++m->launches;
-		}
-		if (m->profiling) CK(cudaEventRecord(m->ev[2], s));
-		if (fused) {
-			launch_rays_fused(m, a);
-		} else {
-			if (records) {
-				CK(cudaMemcpyAsync(&m->h_ctr->seg_total, &M.ctr->seg_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-				CK(cudaStreamSynchronize(s));
-				ensure_seg(m, std::max<unsigned long long>(m->h_ctr->seg_total, 1024));
-				a.seg = m->d_seg.p;
-				a.seg_cap = m->seg_cap;
+			if (use_color) {
+				k_route_hits<<<grid, 256, 0, s>>>(M, a, (unsigned long long)index_base, index_stride);
+				++m->launches;
 			}
-			launch_rays_records(m, a, p.simple);
+			if (m->profiling) CK(cudaEventRecord(m->ev[2], s));
+			if (fused) {
+				launch_rays_fused(m, a);
+			} else {
+				if (records) {
+					CK(cudaMemcpyAsync(&m->h_ctr->seg_total, &M.ctr->seg_total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+					CK(cudaStreamSynchronize(s));
+					ensure_seg(m, std::max<unsigned long long>(m->h_ctr->seg_total, 1024));
+					a.seg = m->d_seg.p;
+					a.seg_cap = m->seg_cap;
+				}
+				launch_rays_records(m, a, p.simple);
+			}
+		} else if (m->profiling) {
+			CK(cudaEventRecord(m->ev[2], s));
 		}
-	} else if (m->profiling) {
-		CK(cudaEventRecord(m->ev[2], s));
+		CK(cudaGetLastError());
+		CK(cudaMemcpyAsync(&m->h_ctr->n_bricks, &M.ctr->n_bricks, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		const uint32_t ov = m->h_ctr->overflow;
+		if (!(ov & 6u) || (ov & ~6u)) break;  // complete, or a flag no growth clears (the next finalize_scan reports it)
+		if (++p.regrows > 16) fail("device pools keep overflowing");
+		try {
+			keep_created(m);
+			grow_pools(m, ov, m->h_ctr->n_bricks, m->h_ctr->n_upper);
+		} catch (std::bad_alloc&) {
+			fail("block pool cannot grow beyond 2^32 slots");
+		}
 	}
 	k_outbox<<<m->sm_count * 4, 256, 0, s>>>(M);
 	k_outbox_publish<<<1, 32, 0, s>>>(M);
@@ -1714,25 +1821,11 @@ int do_route_apply(Map* m, uint32_t first, uint32_t count, int last)
 		new_up_epoch(m);
 		p.applying = true;
 	} else {
-		CK(cudaMemsetAsync(&M.ctr->n_touched, 0, sizeof(uint32_t), s));
-	}
-	ScanArgs t{};
-	if (M.color) {
-		// apply table for the hit records of these sources: at most count * cap_h keys, half full
-		const uint32_t size = std::min(m->route_tab_size, std::max(1u << 12, next_pow2(2ull * count * m->route_cap_h)));
-		CK(cudaMemsetAsync(m->d_route_tab_keys.p, 0xff, (size_t)size * sizeof(unsigned long long), s));
-		CK(cudaMemsetAsync(m->d_route_tab_min.p, 0xff, (size_t)size * sizeof(uint32_t), s));
-		t.tab_keys = m->d_route_tab_keys.p;
-		t.tab_min = m->d_route_tab_min.p;
-		t.tab_mask = size - 1;
-	}
-	k_inbox<<<m->sm_count * 4, 256, 0, s>>>(M, first, count, t);
-	++m->launches;
-	if (M.color) {
-		k_inbox_color<<<m->sm_count * 4, 256, 0, s>>>(M, first, count, t);
+		k_route_next_apply<<<1, 1, 0, s>>>(M.ctr);
 		++m->launches;
 	}
-	launch_update(m, p.a.miss, false);
+	p.calls.push_back({first, count, M.scan_id});
+	enqueue_route_call(m, (uint32_t)p.calls.size() - 1);
 	launch_upper_seed(m);
 	if (last) {
 		if (m->profiling) CK(cudaEventRecord(m->ev[5], s));

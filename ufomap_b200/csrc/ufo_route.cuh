@@ -34,6 +34,12 @@
 //                  sensors' clouds one after the other.
 // Inbox regions are double-buffered by scan parity; the barrier of scan k+1 orders the reads of
 // scan k before the writes of scan k+2.
+//
+// The pools grow during a pass as they do on one GPU.  route_mark waits for the marking kernels
+// and, if a pool ran full, grows it and marks again before anything reaches an inbox header
+// (k_outbox_publish).  An apply call whose k_inbox runs into a full pool backs off with every later
+// call of the pass; the host replays them at its next synchronising call, from the regions the
+// peers published, which stay valid until the peers' mark of pass k+2.
 #pragma once
 
 #include "ufo_kernels.cuh"
@@ -132,10 +138,22 @@ __global__ void __launch_bounds__(256) k_route_hits(DeviceMap M, ScanArgs a, uns
 	route_hit(M, owner, pack_key(k.x, k.y, k.z), (uint32_t)(index_base + (unsigned long long)i * index_stride), rgb);
 }
 
-// applies the records of sources [first, first + count).  Colour maps: hit records only enter the
-// apply table t (minimum global index per voxel); k_inbox_color applies them.
-__global__ void __launch_bounds__(256) k_inbox(DeviceMap M, uint32_t first, uint32_t count, ScanArgs t)
+// An apply call after the first one starts from an empty touched list -- unless a call before it
+// backed off: that call's list stays, for its replay after the pool growth (finalize_scan).
+__global__ void k_route_next_apply(Counters* c)
 {
+	if (!(c->overflow & ~4u)) c->n_touched = 0;
+}
+
+// applies the records of sources [first, first + count), apply call `call` of the pass.  Colour maps:
+// hit records only enter the apply table t (minimum global index per voxel); k_inbox_color applies
+// them.  A brick pool that runs full leaves the records it could not place unapplied and flags the
+// map; K3, the upper seed and every later call of the pass then back off, and the host grows the pool
+// and replays the calls from this one on (finalize_scan).  route_call tells it which call that is.
+__global__ void __launch_bounds__(256) k_inbox(DeviceMap M, uint32_t first, uint32_t count, ScanArgs t, uint32_t call)
+{
+	if (__ldg(&M.ctr->overflow) & ~4u) return;  // an earlier call of the pass backed off: replayed as a whole
+	if (blockIdx.x == 0 && threadIdx.x == 0) M.ctr->route_call = call;
 	const uint32_t lane = threadIdx.x & 31;
 	constexpr uint32_t FULL = 0xffffffffu;
 	const RouteTable* R = M.route;
@@ -185,10 +203,30 @@ __global__ void __launch_bounds__(256) k_inbox(DeviceMap M, uint32_t first, uint
 	}
 }
 
+// The bricks a routed pass touched -- stamped by its apply calls, scan ids first .. first + n - 1 --
+// become the touched list again, so that the upper levels of a replayed pass are seeded from them.
+// (Scan ids skip 0, the stamp of a brick no scan touched.)
+__global__ void __launch_bounds__(256) k_touch_pass(DeviceMap M, uint32_t n_bricks, uint32_t first, uint32_t n)
+{
+	const uint32_t lane = threadIdx.x & 31;
+	const uint32_t stride = gridDim.x * blockDim.x;
+	for (uint32_t b0 = blockIdx.x * blockDim.x; b0 < n_bricks; b0 += stride) {
+		const uint32_t b = b0 + threadIdx.x, st = b < n_bricks ? M.brick_stamp[b] : 0u;
+		const bool in = st != 0u && st - first < n;
+		const uint32_t bal = __ballot_sync(0xffffffffu, in);
+		if (!bal) continue;
+		uint32_t base = 0;
+		if (lane == 0) base = atomicAdd(&M.ctr->n_touched, (uint32_t)__popc(bal));
+		base = __shfl_sync(0xffffffffu, base, 0);
+		if (in) M.touched[base + __popc(bal & ((1u << lane) - 1u))] = b;
+	}
+}
+
 // colour maps, after k_inbox: the record that holds its voxel's minimum global index sets the hit
 // bit and blends its colour, as k_hits does on one GPU (same guard against blending twice)
 __global__ void __launch_bounds__(256) k_inbox_color(DeviceMap M, uint32_t first, uint32_t count, ScanArgs t)
 {
+	if (__ldg(&M.ctr->overflow) & ~4u) return;  // k_inbox could not place every record: the call is replayed
 	const RouteTable* R = M.route;
 	for (uint32_t s = first; s < first + count; ++s) {
 		const RouteBox box = R->in[s];
