@@ -32,6 +32,8 @@ constexpr uint32_t kNone = 0xffffffffu;     // "no such brick / node"
 // touched_mi flag, set by k_gather for a brick without a hit this scan: k_update_brick does not
 // stage its hit masks.  Lists built elsewhere leave it clear, so their bricks stage them.
 constexpr uint32_t kMiNoHits = 1u << 31;
+// touched_mi / touched_mi2 of a paired pass: the brick was not marked by that scan
+constexpr uint32_t kMiAbsent = kNone;
 
 // aggregate of an inner node: max log-odds of the subtree + contains_* flags
 // (occupancy_map_base.h:1179-1224).  flags: bit0 contains_free, bit1 contains_unknown.
@@ -66,6 +68,7 @@ struct Counters {
 	unsigned long long touched_d3;
 	unsigned long long touched_bricks;
 	unsigned long long upper_nodes;
+	unsigned long long upper_pair[2];  // paired pass: upper nodes above the bricks of its first / second scan
 	unsigned long long bbox[6];  // order-preserving encoding of min xyz / max xyz of this scan
 	// dense fused walk, profiling level 2 only (k_walk_mark<COUNT = true>): block records pushed,
 	// global mask reductions issued, of those the ones that found the word empty, dirty-bit reductions
@@ -76,7 +79,8 @@ struct Counters {
 	unsigned long long e_visits, e_nodes, e_free;
 	uint32_t e_rounds, e_converged, e_low[2];
 	// k_update statistics spread over slots: [slot][0 voxels, 1 hit voxels, 2 octets, 3 blocks,
-	// 4 first-touched blocks, 5 bricks, 6 depth-3 nodes, 7 128 B leaf lines read]
+	// 4 first-touched blocks, 5 bricks, 6 depth-3 nodes, 7 128 B leaf lines read]; a paired pass counts
+	// its first scan in slots 0..31 and its second in 32..63
 	unsigned long long stat[64][8];
 };
 
@@ -144,6 +148,16 @@ struct DeviceMap {
 	uint32_t* touched_mi;   // [brick_cap] where the free-space masks of touched[i] are: mask_base + (mi & ~kMiNoHits) * 64
 	uint32_t* hit_stamp;    // [brick_cap] scan id of the last scan that set a hit bit of the brick
 	unsigned long long* mask_base;  // per scan: miss_mask (mi = brick slot) or the dense scan volume (mi = volume brick)
+	// Paired pass (two consecutive scans, one leaf update): the second scan marks into a second dense
+	// volume (mask_base2) and a second hit-mask array; touched_mi2[i] locates its masks of touched[i]
+	// (kMiAbsent: not marked by it, and likewise touched_mi for the first scan).  touch_idx[brick] is the
+	// brick's entry in the touched list of the last dense gather, pair_id the first scan's id while the
+	// second one gathers (0 otherwise)
+	unsigned long long* mask_base2;
+	unsigned long long* hit_mask2;
+	uint32_t* touched_mi2;
+	uint32_t* touch_idx;
+	uint32_t pair_id;
 	// Dense scan volume (ufo_walk.cuh): block masks of the cube of bricks around the sensor that a
 	// range-limited scan can reach, brick-major ([volume brick][64 blocks in Morton order]), so that
 	// the ray walk marks with a computed address and no lookup.  vol_dirty: one bit per volume brick.

@@ -1224,6 +1224,25 @@ __global__ void __launch_bounds__(256) k_upper_seed(DeviceMap M, uint32_t* list,
 	}
 }
 
+// Paired pass, after K4: the upper nodes above the bricks of one of its scans (`second`: touched_mi2),
+// which is what K4 of that scan alone would have recomputed.  Each node is counted by the first
+// thread that stamps it with `epoch`, an id no propagation pass uses; a thread stops at a node
+// stamped before it, whose ancestors are counted already.
+__global__ void __launch_bounds__(256) k_upper_count(DeviceMap M, uint32_t second, uint32_t epoch)
+{
+	if (__ldg(&M.ctr->overflow)) return;
+	const uint32_t n = __ldg(&M.ctr->n_touched);
+	unsigned long long cnt = 0;
+	for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
+		if ((second ? M.touched_mi2[e] : M.touched_mi[e]) == kMiAbsent) continue;
+		for (uint32_t p = M.brick_parent[M.touched[e]]; p != kNone && atomicExch(&M.up_stamp[p], epoch) != epoch;
+		     p = ld_volatile_u32(&M.up_parent[p]))
+			++cnt;
+	}
+	cnt = __reduce_add_sync(0xffffffffu, (uint32_t)cnt);
+	if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&M.ctr->upper_pair[second], cnt);
+}
+
 // Recomputes the nodes of `in` (all at depth d) from their child slots and reports them to their
 // parents (-> `out`).  Eight lanes per node, one child each.  Counters rotate three ways:
 // level d reads list_count[d % 3], appends to [(d + 1) % 3] and clears [(d + 2) % 3]

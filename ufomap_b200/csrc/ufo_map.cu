@@ -19,6 +19,7 @@
 #include <chrono>
 #include <functional>
 #include <numeric>
+#include <optional>
 #include <queue>
 #include <climits>
 #include <cmath>
@@ -129,6 +130,10 @@ struct PendingScan {
 	};
 	std::vector<RouteCall> calls;
 	bool dense = false;   // marks go to the dense scan volume
+	// marked, leaf update (K3, K4) not enqueued yet: the next insert may share it (a paired pass), any
+	// other call enqueues it alone (finalize_scan)
+	bool defer = false;
+	bool flushed = false;  // a deferred scan whose leaf update was enqueued alone
 	VolumeArgs vol{};
 	float set_value = 0.0f;
 	uint32_t early = 0;  // early_stopping of a scan on a map that opted in (ufo_early.cuh); 0: off
@@ -176,6 +181,12 @@ struct ufo_b200_map {
 	DevMem<uint32_t> uh_vals;
 	DevMem<unsigned long long> vol, vol_dirty;
 	DevMem<uint32_t> vol_list;
+	// the second scan's dense volume of a paired pass, allocated by the first pair; no_pair once that
+	// failed (the map then runs one scan per pass)
+	DevMem<unsigned long long> vol2, vol2_dirty;
+	DevMem<uint32_t> vol2_list;
+	uint32_t vol2_db_cap = 0;
+	bool no_pair = false;
 	// change masks (a pool array): kept while detection is switched off, M.chg_mask only while recording
 	unsigned long long* chg_mask = nullptr;
 	bool chg_recording = false;
@@ -233,7 +244,7 @@ struct ufo_b200_map {
 	int no_dense = 0;       // UFO_B200_MARK=probe, or a scan left the volume: fused walk through the brick hash
 	uint32_t vol_db_cap = 0;  // bricks per axis the allocated scan volume can hold
 	uint64_t launches = 0;
-	cudaEvent_t ev[8]{};
+	cudaEvent_t ev[10]{};  // [8]: start of the leaf update, [9]: end of a deferred scan's marking
 	bool ev_valid = false, ev7_valid = false, h2d_valid = false;
 	ufo_b200_scan_stats stats{};       // scan in flight / last scan
 	ufo_b200_scan_stats done_stats{};  // last scan whose counters are folded into the host view
@@ -245,6 +256,13 @@ struct ufo_b200_map {
 	float value_floor = 0.0f;
 	bool stats_pending = false;
 	PendingScan pending;
+	// Paired pass: `pending` is its second scan; the first one's scan id, touched entries and counters
+	// up to its marking are kept here.  held_stats: the second scan's counters, which
+	// completed_scan_stats reports one insert after the first scan's
+	bool paired = false;
+	uint32_t first_id = 0, first_touched = 0;
+	ufo_b200_scan_stats first_stats{}, held_stats{};
+	bool held = false;
 	bool poisoned = false;
 	// routed multi-GPU mode
 	DevMem<unsigned char> route_inbox;  // this rank's inbox: [2 parities][world sources] regions
@@ -438,6 +456,9 @@ const PoolArray kPool[] = {
 	{UFO_POOL_ARRAY(M.leaf), 64 * 64, 0, Pool::Brick, Have::Always, Retain::Compact},
 	{UFO_POOL_ARRAY(M.miss_mask), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
 	{UFO_POOL_ARRAY(M.hit_mask), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.hit_mask2), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
+	{UFO_POOL_ARRAY(M.touched_mi2), 1, 0, Pool::Brick, Have::Always, Retain::Renew},
+	{UFO_POOL_ARRAY(M.touch_idx), 1, 0, Pool::Brick, Have::Always, Retain::Renew},
 	{UFO_POOL_ARRAY(M.meta), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
 	{UFO_POOL_ARRAY(M.line_max), 64, 0, Pool::Brick, Have::Always, Retain::Compact},
 	{UFO_POOL_ARRAY(M.brick_parent), 1, 0xff, Pool::Brick, Have::Always, Retain::Renew},
@@ -563,10 +584,12 @@ void free_pools(Map* m)
 		if (*a.owner(m)) reshape(m, a, pool_cap(m, a.pool), 0, 0, nullptr);
 }
 
-void push_counters(Map* m)
+// `touched`: entries of the touched list to keep (the first scan's, when the second of a pair marks)
+void push_counters(Map* m, uint32_t touched = 0)
 {
 	// host view -> device allocation counters, clears the per-scan part
 	Counters c{};
+	c.n_touched = touched;
 	c.n_blocks = m->n_blocks;
 	c.n_bricks = m->n_bricks;
 	c.n_upper = m->n_upper;
@@ -712,15 +735,51 @@ void ensure_scan_buffers(Map* m, size_t n, bool need_table, bool records, bool f
 	}
 }
 
+// K3's counters of one scan: statistics slots [lo, hi) (a paired pass counts its scans apart)
+void update_counts(Map* m, ufo_b200_scan_stats& st, const Counters& c, int lo, int hi, unsigned long long upper)
+{
+	unsigned long long sum[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+	for (int sl = lo; sl < hi; ++sl)
+		for (int k = 0; k < 8; ++k) sum[k] += c.stat[sl][k];
+	st.touched_voxels = sum[0];
+	st.hit_voxels = sum[1];
+	st.touched_octets = sum[2];
+	st.touched_blocks = sum[3];
+	st.touched_d3 = sum[6];
+	st.touched_bricks = sum[5];
+	st.touched_lines = sum[7];
+	st.upper_nodes = upper;
+	m->n_blocks += (uint32_t)sum[4];
+	st.blocks_in_map = m->n_blocks;
+}
+
+// the change box of a scan whose counters are in c
+void fold_bbox(Map* m, const Counters& c)
+{
+	for (int i = 0; i < 3; ++i) {
+		if (c.bbox[i] != ~0ull) m->min_change[i] = std::min(m->min_change[i], decode_ordered(c.bbox[i]));
+		if (c.bbox[3 + i] != 0ull) m->max_change[i] = std::max(m->max_change[i], decode_ordered(c.bbox[3 + i]));
+	}
+}
+
+// event times of a scan's marking (profiling level 1 and up)
+void marking_times(Map* m, ufo_b200_scan_stats& st)
+{
+	cudaEventElapsedTime(&st.ms_points, m->ev[0], m->ev[2]);
+	if (m->ev7_valid) {
+		cudaEventElapsedTime(&st.ms_rays, m->ev[2], m->ev[7]);
+		cudaEventElapsedTime(&st.ms_scatter, m->ev[7], m->ev[3]);
+	} else {
+		cudaEventElapsedTime(&st.ms_rays, m->ev[2], m->ev[3]);
+	}
+}
+
 void finish_stats(Map* m)
 {
 	// called after the stream is idle and h_ctr holds the end-of-scan counters
 	if (!m->stats_pending) return;
 	const Counters& c = *m->h_ctr;
 	ufo_b200_scan_stats& st = m->stats;
-	unsigned long long sum[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-	for (int sl = 0; sl < kStatSlots; ++sl)
-		for (int k = 0; k < 8; ++k) sum[k] += c.stat[sl][k];
 	st.rays = c.n_rays;
 	st.visits = c.visits;
 	m->walk_stats = ufo_b200_walk_stats{c.walk_records, c.walk_mask_reds, c.walk_words, c.walk_dirty_reds};
@@ -750,42 +809,33 @@ void finish_stats(Map* m)
 			cudaEventElapsedTime(&es.ms_mark, m->ev[4], m->ev[3]);
 		}
 	}
-	st.touched_voxels = sum[0];
-	st.hit_voxels = sum[1];
-	st.touched_octets = sum[2];
-	st.touched_blocks = sum[3];
-	st.touched_d3 = sum[6];
-	st.touched_bricks = sum[5];
-	st.touched_lines = sum[7];
-	st.upper_nodes = c.upper_nodes;
-	m->n_blocks += (uint32_t)sum[4];
+	if (m->paired) {
+		update_counts(m, m->first_stats, c, 0, kStatSlots / 2, c.upper_pair[0]);
+		update_counts(m, st, c, kStatSlots / 2, kStatSlots, c.upper_pair[1]);
+	} else {
+		update_counts(m, st, c, 0, kStatSlots, c.upper_nodes);
+	}
 	m->n_bricks = std::min(c.n_bricks, m->M.brick_cap);
 	m->n_upper = std::min(c.n_upper, m->M.up_cap);
-	st.blocks_in_map = m->n_blocks;
 	st.bricks_in_map = m->n_bricks;
 	st.device_bytes = m->device_bytes;
-	if (c.n_rays || sum[0]) {
-		for (int i = 0; i < 3; ++i) {
-			if (c.bbox[i] != ~0ull) m->min_change[i] = std::min(m->min_change[i], decode_ordered(c.bbox[i]));
-			if (c.bbox[3 + i] != 0ull)
-				m->max_change[i] = std::max(m->max_change[i], decode_ordered(c.bbox[3 + i]));
-		}
-	}
+	if (c.n_rays || st.touched_voxels) fold_bbox(m, c);
 	if (m->ev_valid) {
 		cudaEventElapsedTime(&st.ms_total, m->ev[0], m->ev[6]);
+		if (m->pending.flushed) {
+			// device time of a deferred scan: its marking and its leaf update, not the wait between
+			float mark = 0.0f, update = 0.0f;
+			cudaEventElapsedTime(&mark, m->ev[0], m->ev[9]);
+			cudaEventElapsedTime(&update, m->ev[8], m->ev[6]);
+			st.ms_total = mark + update;
+		}
 		if (m->h2d_valid) cudaEventElapsedTime(&st.ms_h2d, m->ev_copy0, m->ev_copied);
 		if (m->write_pass) {
 			cudaEventElapsedTime(&st.ms_update, m->ev[3], m->ev[5]);
 			cudaEventElapsedTime(&st.ms_propagate, m->ev[5], m->ev[6]);
 		} else if (m->profiling) {
-			cudaEventElapsedTime(&st.ms_points, m->ev[0], m->ev[2]);
-			if (m->ev7_valid) {
-				cudaEventElapsedTime(&st.ms_rays, m->ev[2], m->ev[7]);
-				cudaEventElapsedTime(&st.ms_scatter, m->ev[7], m->ev[3]);
-			} else {
-				cudaEventElapsedTime(&st.ms_rays, m->ev[2], m->ev[3]);
-			}
-			cudaEventElapsedTime(&st.ms_update, m->ev[3], m->ev[5]);
+			marking_times(m, st);
+			cudaEventElapsedTime(&st.ms_update, m->ev[8], m->ev[5]);
 			cudaEventElapsedTime(&st.ms_propagate, m->ev[5], m->ev[6]);
 		}
 	}
@@ -801,7 +851,8 @@ void ensure_seg(Map* m, unsigned long long want)
 }
 
 // K3 over the scan's touched list: persistent warps, the list length is read on the device.
-void launch_update(Map* m, float miss, bool set_mode = false)
+// pair: the touched list of a paired pass (mono maps, scans only)
+void launch_update(Map* m, float miss, bool set_mode = false, bool pair = false)
 {
 	CK(cudaMemsetAsync(&m->M.ctr->k3_cursor, 0, sizeof(uint32_t), m->stream));
 	m->M.k3_stat = nullptr;
@@ -820,6 +871,7 @@ void launch_update(Map* m, float miss, bool set_mode = false)
 		const uint32_t per_sm = UbShape<false>::kMinBlocks, T = UbShape<false>::kWarps * 32;
 		const uint32_t grid = (uint32_t)m->sm_count * (m->k3_blocks ? std::min<uint32_t>(per_sm, (uint32_t)m->k3_blocks) : per_sm);
 		if (set_mode) k_update_brick<false, true><<<grid, T, 0, m->stream>>>(m->M, miss);
+		else if (pair) k_update_brick<false, false, true><<<grid, T, 0, m->stream>>>(m->M, miss);
 		else k_update_brick<false, false><<<grid, T, 0, m->stream>>>(m->M, miss);
 	}
 	++m->launches;
@@ -947,11 +999,71 @@ void wipe_volume(Map* m)
 	CK(cudaMemsetAsync(m->vol_dirty.p, 0, m->vol_dirty.bytes, m->stream));
 }
 
-// called with the stream idle; binds the volume to this scan's sensor position
-void setup_volume(Map* m, PendingScan& p, uint32_t db)
+// Second dense volume of a paired pass, for db bricks per axis; false (and no pairs from then on)
+// when it cannot be allocated.  Called with the stream idle.
+bool ensure_volume2(Map* m, uint32_t db)
+{
+	if (db <= m->vol2_db_cap) return true;
+	const size_t nb = (size_t)db * db * db;
+	try {
+		m->vol2.ensure(m, nb * 64 * sizeof(unsigned long long), 0);
+		m->vol2_dirty.ensure(m, (nb / 64 + 1) * sizeof(unsigned long long), 0);
+		m->vol2_list.ensure(m, (nb / 64 + 1) * sizeof(uint32_t), 0);
+	} catch (CudaError&) {
+		cudaGetLastError();  // an allocation failure is not sticky
+		m->vol2.release(m);
+		m->vol2_dirty.release(m);
+		m->vol2_list.release(m);
+		m->vol2_db_cap = 0;
+		m->no_pair = true;
+		return false;
+	}
+	m->vol2_db_cap = db;
+	return true;
+}
+
+// empties the second dense volume and the second hit masks
+void wipe_volume2(Map* m)
+{
+	if (m->vol2.p) {
+		CK(cudaMemsetAsync(m->vol2.p, 0, m->vol2.bytes, m->stream));
+		CK(cudaMemsetAsync(m->vol2_dirty.p, 0, m->vol2_dirty.bytes, m->stream));
+	}
+	CK(cudaMemsetAsync(m->M.hit_mask2, 0, (size_t)m->M.brick_cap * 64 * sizeof(unsigned long long), m->stream));
+}
+
+// While the second scan of a pair marks, the marking kernels see its volume and hit masks in place of
+// the first's; restored when the object goes.
+struct SecondMarks {
+	Map* m;
+	unsigned long long *vol, *dirty;
+	uint32_t* list;
+	explicit SecondMarks(Map* m_) : m(m_), vol(m_->M.vol), dirty(m_->M.vol_dirty), list(m_->M.vol_list)
+	{
+		DeviceMap& M = m->M;
+		M.vol = m->vol2.p;
+		M.vol_dirty = m->vol2_dirty.p;
+		M.vol_list = m->vol2_list.p;
+		std::swap(M.hit_mask, M.hit_mask2);
+		M.pair_id = m->first_id;
+	}
+	~SecondMarks()
+	{
+		DeviceMap& M = m->M;
+		M.vol = vol;
+		M.vol_dirty = dirty;
+		M.vol_list = list;
+		std::swap(M.hit_mask, M.hit_mask2);
+		M.pair_id = 0;
+	}
+};
+
+// called with the stream idle; binds the volume to this scan's sensor position (the second volume
+// has been allocated by ensure_volume2)
+void setup_volume(Map* m, PendingScan& p, uint32_t db, bool second = false)
 {
 	DeviceMap& M = m->M;
-	if (db > m->vol_db_cap) {
+	if (!second && db > m->vol_db_cap) {
 		const size_t nb = (size_t)db * db * db;
 		m->vol.ensure(m, nb * 64 * sizeof(unsigned long long), 0);
 		m->vol_dirty.ensure(m, (nb / 64 + 1) * sizeof(unsigned long long), 0);
@@ -1008,6 +1120,7 @@ __global__ void k_reset_upper_pass(Counters* c, uint32_t n_upper)
 	c->overflow = 0;
 	c->list_count[0] = c->list_count[1] = c->list_count[2] = 0;
 	c->upper_nodes = 0;
+	c->upper_pair[0] = c->upper_pair[1] = 0;
 	c->n_upper = n_upper;
 }
 
@@ -1175,7 +1288,57 @@ void bind_scan_buffers(Map* m, PendingScan& p, bool fused)
 	}
 }
 
-// Enqueues every kernel of one scan and the read-back of its counters; never waits.
+// The upper levels of a pass and, for a paired pass, each scan's count of them (k_upper_count)
+void launch_upper_pass(Map* m)
+{
+	launch_upper(m);
+	if (!m->paired || m->M.g.depth_levels < 5) return;
+	for (uint32_t k = 0; k < 2; ++k) {
+		new_up_epoch(m);
+		k_upper_count<<<m->sm_count * 2, 256, 0, m->stream>>>(m->M, k, m->M.up_epoch);
+		++m->launches;
+	}
+}
+
+// K3 and K4 of an enqueued scan (of both scans of a paired pass) and the read-back of the counters
+void enqueue_update(Map* m, PendingScan& p)
+{
+	DeviceMap& M = m->M;
+	cudaStream_t s = m->stream;
+	const ScanArgs& a = p.a;
+	CK(cudaEventRecord(m->ev[8], s));
+	// K3 and K4 run off the device-side touched list; if a pool overflowed while marking they
+	// back off by themselves and the scan is repeated by finalize_scan() after the growth.
+	const bool aliases = M.alias_miss != nullptr;
+	const uint32_t agrid = (uint32_t)m->sm_count * 4;
+	if (aliases) {
+		k_alias_apply<<<agrid, 256, 0, s>>>(M, M.hit, 1);
+		++m->launches;
+	}
+	if (m->paired) {
+		M.mask_base2 = m->vol2.p;
+		M.pair_id = m->first_id;
+	}
+	launch_update(m, p.has_vol ? p.set_value : a.miss, p.has_vol, m->paired);
+	M.pair_id = 0;
+	if (aliases) {
+		k_alias_apply<<<agrid, 256, 0, s>>>(M, a.miss, 0);
+		k_alias_refresh<<<agrid, 256, 0, s>>>(M);
+		launch_brick_agg(m);
+		m->launches += 3;
+	}
+	if (m->profiling) CK(cudaEventRecord(m->ev[5], s));
+	launch_upper_pass(m);
+	CK(cudaEventRecord(m->ev[6], s));
+	m->ev_valid = true;
+	CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+	m->stats_pending = true;
+	p.valid = true;
+}
+
+// Enqueues every kernel of one scan and the read-back of its counters; never waits.  A deferred scan
+// (p.defer) stops after its marking; m->paired: the scan is the second of a pair and marks into the
+// second volume, then the pass updates the leaves of both.
 void enqueue_scan(Map* m, PendingScan& p)
 {
 	if (p.write) {
@@ -1194,7 +1357,9 @@ void enqueue_scan(Map* m, PendingScan& p)
 	M.mask_base = M.dense ? M.vol : M.miss_mask;
 	bind_scan_buffers(m, p, fused);
 	m->ev7_valid = false;
-	push_counters(m);
+	push_counters(m, m->paired ? m->first_touched : 0u);
+	std::optional<SecondMarks> second;
+	if (m->paired) second.emplace(m);
 	if (p.need_table) {
 		CK(cudaMemsetAsync(m->d_tab_keys.p, 0xff, (size_t)m->tab_size * sizeof(unsigned long long), s));
 		CK(cudaMemsetAsync(m->d_tab_min.p, 0xff, (size_t)m->tab_size * sizeof(uint32_t), s));
@@ -1226,29 +1391,17 @@ void enqueue_scan(Map* m, PendingScan& p)
 		CK(cudaEventRecord(m->ev[2], s));
 	}
 	if (m->profiling) CK(cudaEventRecord(m->ev[3], s));
+	second.reset();
 	CK(cudaGetLastError());
-	// K3 and K4 run off the device-side touched list; if a pool overflowed while marking they
-	// back off by themselves and the scan is repeated by finalize_scan() after the growth.
-	const bool aliases = M.alias_miss != nullptr;
-	const uint32_t agrid = (uint32_t)m->sm_count * 4;
-	if (aliases) {
-		k_alias_apply<<<agrid, 256, 0, s>>>(M, M.hit, 1);
-		++m->launches;
+	if (p.defer) {
+		CK(cudaEventRecord(m->ev[9], s));
+		m->ev_valid = true;
+		CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+		m->stats_pending = true;
+		p.valid = true;
+		return;
 	}
-	launch_update(m, p.has_vol ? p.set_value : a.miss, p.has_vol);
-	if (aliases) {
-		k_alias_apply<<<agrid, 256, 0, s>>>(M, a.miss, 0);
-		k_alias_refresh<<<agrid, 256, 0, s>>>(M);
-		launch_brick_agg(m);
-		m->launches += 3;
-	}
-	if (m->profiling) CK(cudaEventRecord(m->ev[5], s));
-	launch_upper(m);
-	CK(cudaEventRecord(m->ev[6], s));
-	m->ev_valid = true;
-	CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
-	m->stats_pending = true;
-	p.valid = true;
+	enqueue_update(m, p);
 }
 
 // k_inbox, its colour pass and K3 of apply call `call` of a routed pass (ufo_route.cuh)
@@ -1322,12 +1475,69 @@ void regrow_routed(Map* m, uint32_t ov)
 	CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
 }
 
+// The second scan of a pair could not be marked completely (a full pool; K3 and K4 backed off): the
+// first scan's leaf update runs alone, the second's marks are wiped, and the caller repeats it as a scan
+// of its own.  Called with the stream idle, after keep_created.
+void split_pair(Map* m, uint32_t ov)
+{
+	DeviceMap& M = m->M;
+	cudaStream_t s = m->stream;
+	PendingScan& p = m->pending;
+	const uint32_t want_bricks = m->h_ctr->n_bricks;  // what the second scan's marking reached: the caller's growth
+	const ufo_b200_scan_stats second = m->stats;
+	m->paired = false;
+	m->stats = m->first_stats;
+	new_scan_id(m);
+	new_up_epoch(m);
+	M.mask_base = M.vol;
+	push_counters(m, m->first_touched);
+	PendingScan first = p;
+	first.has_vol = false;
+	enqueue_update(m, first);
+	CK(cudaStreamSynchronize(s));
+	while (m->h_ctr->overflow == 4u) {  // only the upper-node pool can overflow here
+		keep_created(m);
+		grow_pools(m, 4u, 0, m->h_ctr->n_upper);
+		new_up_epoch(m);
+		k_reset_upper_pass<<<1, 1, 0, s>>>(M.ctr, m->n_upper);
+		launch_upper(m);
+		CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+	}
+	finish_stats(m);
+	// what the first scan's marking counted stays; the pass added its leaf update
+	ufo_b200_scan_stats& a = m->stats;
+	const ufo_b200_scan_stats& f = m->first_stats;
+	a.rays = f.rays;
+	a.visits = f.visits;
+	a.ms_total = f.ms_total;
+	a.ms_points = f.ms_points;
+	a.ms_rays = f.ms_rays;
+	a.ms_scatter = f.ms_scatter;
+	m->done_stats = a;
+	m->held = false;
+	wipe_volume2(m);
+	keep_created(m);
+	// grow_pools sizes the brick pool by what the second scan's marking reached, and rebuilds both
+	// hashes from the live slots: the upper nodes include those the first scan's K4 just created
+	m->h_ctr->n_bricks = std::max(want_bricks, m->n_bricks);
+	m->h_ctr->n_upper = m->n_upper;
+	m->stats = second;
+	if (p.dense) setup_volume(m, p, volume_bricks(m, p));
+}
+
 // Waits for the scan in flight, repeats it if a device pool overflowed, and folds its counters
-// into the host view.  Throws MapError if the scan cannot be completed.
+// into the host view.  A deferred scan gets its leaf update enqueued first.  Throws MapError if the
+// scan cannot be completed.
 void finalize_scan(Map* m)
 {
-	CK(cudaStreamSynchronize(m->stream));
 	PendingScan& p = m->pending;
+	if (p.valid && p.defer) {
+		p.defer = false;
+		p.flushed = true;
+		enqueue_update(m, p);
+	}
+	CK(cudaStreamSynchronize(m->stream));
 	if (!p.valid) {
 		finish_stats(m);
 		return;
@@ -1369,7 +1579,7 @@ void finalize_scan(Map* m)
 				grow_pools(m, 4u, 0, m->h_ctr->n_upper);
 				new_up_epoch(m);
 				k_reset_upper_pass<<<1, 1, 0, m->stream>>>(M.ctr, m->n_upper);
-				launch_upper(m);
+				launch_upper_pass(m);
 				CK(cudaEventRecord(m->ev[6], m->stream));
 				CK(cudaMemcpyAsync(m->h_ctr, M.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, m->stream));
 			} else {
@@ -1377,6 +1587,7 @@ void finalize_scan(Map* m)
 				// consumed (every later kernel backed off).  Grow and run the whole pass again under a
 				// new scan id (marking is idempotent: OR into masks, find-or-create of bricks).  Only
 				// scans set the flags other than 2 and 4.
+				if (m->paired) split_pair(m, ov);
 				if (ov & 64u) {
 					// a mark fell outside the scan volume (cannot happen for rays within max_range; kept
 					// as a safety net): wipe the volume and repeat through the brick hash
@@ -1419,7 +1630,51 @@ void finalize_scan(Map* m)
 	m->stats.result_bytes = sizeof(Counters) * (1 + p.regrows);
 	p.valid = false;
 	finish_stats(m);
-	m->done_stats = m->stats;
+	if (m->paired) {
+		m->paired = false;
+		m->done_stats = m->first_stats;
+		m->held_stats = m->stats;
+		m->held = true;
+	} else {
+		m->done_stats = m->stats;
+		m->held = false;
+	}
+}
+
+// The deferred scan's marking is complete (stream idle, no pool overflowed) and the next scan pairs
+// with it: its counters so far become the first scan's, and the pass goes on with the second.
+void hold_first(Map* m)
+{
+	const Counters& c = *m->h_ctr;
+	ufo_b200_scan_stats& st = m->first_stats;
+	st = m->stats;
+	st.rays = c.n_rays;
+	st.visits = c.visits;
+	keep_created(m);
+	st.bricks_in_map = m->n_bricks;
+	st.device_bytes = m->device_bytes;
+	if (c.n_rays) fold_bbox(m, c);
+	if (m->ev_valid) {
+		cudaEventElapsedTime(&st.ms_total, m->ev[0], m->ev[9]);
+		if (m->h2d_valid) cudaEventElapsedTime(&st.ms_h2d, m->ev_copy0, m->ev_copied);
+		if (m->profiling) marking_times(m, st);
+	}
+	st.regrows = m->pending.regrows;
+	st.launches = m->launches;
+	st.result_bytes = sizeof(Counters) * (1 + m->pending.regrows);
+	m->first_id = m->M.scan_id;
+	m->first_touched = c.n_touched;
+	m->paired = true;
+	m->stats_pending = false;
+	m->pending.valid = false;
+}
+
+// completed_scan_stats: the pair's second scan once a later call has been made
+void release_held(Map* m)
+{
+	if (!m->held) return;
+	m->done_stats = m->held_stats;
+	m->held = false;
 }
 
 // every brick of the map becomes the "touched list" (whole-map passes: threshold changes)
@@ -1473,7 +1728,9 @@ void rebuild_flags(Map* m)
 
 int sync_map(Map* m)
 {
+	release_held(m);
 	finalize_scan(m);
+	release_held(m);
 	return UFO_B200_OK;
 }
 
@@ -1534,8 +1791,30 @@ int do_insert(Map* m, const double origin[3], const void* points, bool on_device
 	const bool copied = !on_device && bytes;
 	const uint32_t stg = m->stage ^ 1u;
 	if (copied) stage_points(m, stg, points, bytes);
+	// Consecutive asynchronous scans of the plain kind share one leaf update (DESIGN.md section 4,
+	// "Paired scans"): the first is marked and deferred, the second marks into the second volume and
+	// the pass updates the leaves of both.  A scan of any other kind runs on its own.
+	PendingScan probe;
+	probe.a.max_range = max_range;
+	const uint32_t pair_db = volume_bricks(m, probe);
+	const DeviceMap& Mc = m->M;
+	const bool eligible = async && !vol && !Mc.color && depth == 0 && !discrete && !simple && !early_stopping && pair_db &&
+	                      !Mc.alias_miss && !Mc.chg_mask && Mc.shard_world <= 1 && Mc.route_world <= 1 && !m->force_records &&
+	                      m->profiling < 2 && !m->no_pair;
+	release_held(m);
+	bool pairing = false;
+	if (eligible && m->pending.valid && m->pending.defer) {
+		CK(cudaStreamSynchronize(m->stream));
+		pairing = !m->h_ctr->overflow && ensure_volume2(m, pair_db);
+	}
 	// one integration in flight at most (insertPointCloudWait, occupancy_map_base.h:315)
-	finalize_scan(m);
+	if (pairing) {
+		// what can fail is allocated first: until hold_first the deferred scan stays what it was
+		ensure_scan_buffers(m, n, false, false, true);
+		hold_first(m);
+	} else {
+		finalize_scan(m);
+	}
 
 	DeviceMap& M = m->M;
 	cudaStream_t s = m->stream;
@@ -1582,8 +1861,9 @@ int do_insert(Map* m, const double origin[3], const void* points, bool on_device
 	if (fused) {
 		const uint32_t db = volume_bricks(m, p);
 		p.dense = db != 0;
-		if (p.dense) setup_volume(m, p, db);
+		if (p.dense) setup_volume(m, p, db, pairing);
 	}
+	p.defer = eligible && !pairing && p.dense;
 	if (records) {
 		// first guess for the record buffer: 48 records per ray; grown on demand
 		ensure_seg(m, std::max<unsigned long long>(m->seg_cap, std::max<unsigned long long>(n, 1024) * 48ull));
@@ -2134,6 +2414,19 @@ int ufo_b200_done(ufo_b200_map* m, int* done)
 	if (m->device == -2) return UFO_B200_E_CUDA;
 	cudaError_t e = cudaStreamQuery(m->stream);
 	if (e == cudaSuccess) {
+		// a deferred scan still waits for its leaf update: enqueued now, so that a caller polling this
+		// function gets to "done"
+		if (m->pending.valid && m->pending.defer) {
+			const int rc = guarded(m, [&]() {
+				CK(cudaSetDevice(m->device));
+				m->pending.defer = false;
+				m->pending.flushed = true;
+				enqueue_update(m, m->pending);
+				return (int)UFO_B200_OK;
+			});
+			*done = 0;
+			return rc;
+		}
 		// the stream is idle; if the scan ran into a full pool it is not integrated yet: grow and repeat
 		// it now, so that a caller polling this function always gets to "done"
 		if (m->pending.valid && m->h_ctr->overflow) {

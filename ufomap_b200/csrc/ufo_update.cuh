@@ -45,11 +45,12 @@ __device__ __forceinline__ unsigned long long octet_unbits8(uint32_t c8, uint32_
 // for bit), so that an unchanged sector leaves no dirty line in the L2; an uninitialised octet
 // (`init` false, its leaves read as 0.0 without a load) is always written.  Returns true when the
 // store was skipped.  SET always writes, and so do colour maps (K3 leaves their colour path as it was).
-template <bool SET = false, bool CLEAN = false>
+// PAIR: a second scan's hits h8b and misses m8b follow, in the order two passes would apply them.
+template <bool SET = false, bool CLEAN = false, bool PAIR = false>
 __device__ __forceinline__ bool update_octet(const DeviceMap& M, float miss, float* lp, uint32_t m8,
                                              uint32_t h8, float4 a0, float4 a1, float& omax,
                                              uint32_t& oflags, size_t blk = 0, uint32_t oct = 0,
-                                             bool init = false)
+                                             bool init = false, uint32_t m8b = 0, uint32_t h8b = 0)
 {
 	float v[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
 	const float v0[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
@@ -64,6 +65,21 @@ __device__ __forceinline__ bool update_octet(const DeviceMap& M, float miss, flo
 			float hv = apply_update(M, v[j], M.hit);
 			v[j] = ((h8 >> j) & 1u) ? hv : v[j];
 		}
+	}
+	if (PAIR) {
+#pragma unroll
+		for (int j = 0; j < 8; ++j) {
+			float mv = apply_update(M, v[j], miss);
+			v[j] = ((m8 >> j) & 1u) ? mv : v[j];
+		}
+		if (h8b) {
+#pragma unroll
+			for (int j = 0; j < 8; ++j) {
+				float hv = apply_update(M, v[j], M.hit);
+				v[j] = ((h8b >> j) & 1u) ? hv : v[j];
+			}
+		}
+		m8 = m8b;
 	}
 #pragma unroll
 	for (int j = 0; j < 8; ++j) {
@@ -141,6 +157,8 @@ __device__ __forceinline__ bool alias_source(const DeviceMap& M, uint32_t brick,
 	return ((x | y | z) & ~km) != 0;
 }
 
+// A paired pass stages the second scan's miss masks in `hm` and reads the hit masks of both scans from
+// global memory (most bricks have none): the slab, and so the kernel's shared memory, keeps its size.
 struct __align__(128) WarpSlab {
 	unsigned long long mm[64];
 	unsigned long long hm[64];
@@ -150,6 +168,25 @@ struct __align__(128) WarpSlab {
 // list entry of a loaded octet: (block << 3) | octet, plus
 constexpr uint32_t kEntInit = 1u << 9;      // the octet is initialised (its leaves are loaded; otherwise 0.0)
 constexpr uint32_t kEntTouched = 1u << 10;  // the scan marked a voxel of it (otherwise only its max is needed)
+constexpr uint32_t kEntHitA = 1u << 11;     // paired pass: the block has a hit of the first scan
+constexpr uint32_t kEntHitB = 1u << 12;     // paired pass: the block has a hit of the second scan
+
+// octets of a block holding a bit of the linear-order voxel mask u
+__device__ __forceinline__ uint32_t mask_octets(unsigned long long u)
+{
+	uint32_t t = 0;
+#pragma unroll
+	for (uint32_t o = 0; o < 8; ++o) {
+		const uint32_t base = ((o & 1u) << 1) | ((o & 2u) << 2) | ((o & 4u) << 3);
+		t |= (((u >> base) & 0x330033ull) ? 1u : 0u) << o;
+	}
+	return t;
+}
+// depth-3 nodes (groups of eight block lanes) with a lane set in ballot b
+__device__ __forceinline__ uint32_t ballot_groups(uint32_t b)
+{
+	return ((b & 0xffu) ? 1u : 0u) + ((b & 0xff00u) ? 1u : 0u) + ((b & 0xff0000u) ? 1u : 0u) + ((b & 0xff000000u) ? 1u : 0u);
+}
 
 // K3: one WARP per brick of the scan's TOUCHED LIST (the cost of a scan does not depend on the size
 // of the map), no CTA-wide barrier at all: a warp waiting for its leaf sectors never holds others at
@@ -226,7 +263,11 @@ struct UbShape {
 	static constexpr int kMinBlocks = COLOR ? UFO_UB_MINBLOCKS_COLOR : UFO_UB_MINBLOCKS;
 };
 
-template <bool COLOR, bool SET = false>
+// PAIR: one pass over the touched list of two consecutive scans (DESIGN.md section 4, "Paired
+// scans"): entry i holds the first scan's masks at touched_mi[i] and the second's at touched_mi2[i],
+// and every voxel gets hit, miss of the first scan, then hit, miss of the second, as two passes
+// would apply them.  Each scan's counters go to its own half of the statistics slots.
+template <bool COLOR, bool SET = false, bool PAIR = false>
 __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::kMinBlocks) k_update_brick(DeviceMap M, float miss)
 {
 	constexpr int WARPS = UbShape<COLOR>::kWarps;
@@ -242,28 +283,43 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 
 	// lane 0: (brick, touched_mi) of the two stages.  A brick flagged kMiNoHits has no hit bit: its
 	// hit masks are not staged, the lanes zero the slab's copy instead (zero_hits)
-	uint32_t st_brick0 = kNone, st_brick1 = kNone, st_mi0 = 0, st_mi1 = 0;
+	uint32_t st_brick0 = kNone, st_brick1 = kNone, st_mi0 = 0, st_mi1 = 0, st_mj0 = 0, st_mj1 = 0;
 	auto issue = [&](uint32_t stage, uint32_t e) {
-		const uint32_t brick = M.touched[e], mi = M.touched_mi[e];
+		const uint32_t brick = M.touched[e], mi = M.touched_mi[e], mj = PAIR ? M.touched_mi2[e] : 0u;
 		if (stage == 0) {
 			st_brick0 = brick;
 			st_mi0 = mi;
+			st_mj0 = mj;
 		} else {
 			st_brick1 = brick;
 			st_mi1 = mi;
+			st_mj1 = mj;
 		}
-		const bool hits = !(mi & kMiNoHits);
 		fence_proxy_async();
-		mbar_expect_tx(&S.bar[stage], 512u + (hits ? 512u : 0u) + 256u + 512u);
-		bulk_load(S.slab[stage].mm, M.mask_base + (size_t)(mi & ~kMiNoHits) * 64, 512u, &S.bar[stage]);
-		if (hits) bulk_load(S.slab[stage].hm, M.hit_mask + (size_t)brick * 64, 512u, &S.bar[stage]);
+		if (PAIR) {
+			const bool a = mi != kMiAbsent, b = mj != kMiAbsent;
+			mbar_expect_tx(&S.bar[stage], (a ? 512u : 0u) + (b ? 512u : 0u) + 256u + 512u);
+			if (a) bulk_load(S.slab[stage].mm, M.mask_base + (size_t)(mi & ~kMiNoHits) * 64, 512u, &S.bar[stage]);
+			if (b) bulk_load(S.slab[stage].hm, M.mask_base2 + (size_t)(mj & ~kMiNoHits) * 64, 512u, &S.bar[stage]);
+		} else {
+			const bool hits = !(mi & kMiNoHits);
+			mbar_expect_tx(&S.bar[stage], 512u + (hits ? 512u : 0u) + 256u + 512u);
+			bulk_load(S.slab[stage].mm, M.mask_base + (size_t)(mi & ~kMiNoHits) * 64, 512u, &S.bar[stage]);
+			if (hits) bulk_load(S.slab[stage].hm, M.hit_mask + (size_t)brick * 64, 512u, &S.bar[stage]);
+		}
 		bulk_load(S.slab[stage].meta, M.meta + (size_t)brick * 64, 256u, &S.bar[stage]);
 		bulk_load(S.slab[stage].q, M.line_max + (size_t)brick * 64, 512u, &S.bar[stage]);
 	};
 	// all lanes, before the stage's list is built (a __syncwarp in between)
 	auto zero_hits = [&](uint32_t stage) {
-		if (__shfl_sync(FULL, stage == 0 ? st_mi0 : st_mi1, 0) & kMiNoHits)
+		const uint32_t mi = __shfl_sync(FULL, stage == 0 ? st_mi0 : st_mi1, 0);
+		if (PAIR) {  // a scan that did not mark the brick: its miss masks are zero
+			const uint32_t mj = __shfl_sync(FULL, stage == 0 ? st_mj0 : st_mj1, 0);
+			if (mi == kMiAbsent) reinterpret_cast<ulonglong2*>(S.slab[stage].mm)[lane] = make_ulonglong2(0ull, 0ull);
+			if (mj == kMiAbsent) reinterpret_cast<ulonglong2*>(S.slab[stage].hm)[lane] = make_ulonglong2(0ull, 0ull);
+		} else if (mi & kMiNoHits) {
 			reinterpret_cast<ulonglong2*>(S.slab[stage].hm)[lane] = make_ulonglong2(0ull, 0ull);
+		}
 	};
 	// Bricks are claimed, not dealt: a warp starts with touched entry gw and then takes the next
 	// unclaimed entry (k3_cursor counts the claims beyond the first n_warps entries).  A brick next
@@ -282,6 +338,7 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 	__syncwarp();
 
 	unsigned int s_vox = 0, s_hit = 0, s_oct = 0, s_blk = 0, s_new = 0, s_lin = 0;
+	unsigned int s_vox2 = 0, s_hit2 = 0, s_oct2 = 0, s_blk2 = 0, s_new2 = 0;  // PAIR: the second scan's
 	// saturated lines (see apply_update): a miss-only leaf line whose 32 voxels all sit at clamp_min is
 	// left as it is, so it is neither loaded nor written.  Exact only when the map holds no value below
 	// clamp_min (M.sat_skip, kept by the host) and the marks land in the tree (fold).  Mono maps only:
@@ -292,20 +349,38 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 	// lane = block lane of either half: touched octets of the brick in `slab` and the octets to load
 	// (touched, and the initialised octets of their lines), list by warp prefix sums.  t8 = the touched
 	// octets that are loaded | the touched octets of saturated lines << 8 (not loaded)
-	auto build_list = [&](const WarpSlab& slab, uint16_t* list, uint32_t (&t8)[2], uint32_t (&excl)[2], uint32_t& total) {
+	// PAIR: brick, mi, mj of the slab (their hit masks are read here)
+	auto build_list = [&](const WarpSlab& slab, uint16_t* list, uint32_t (&t8)[2], uint32_t (&excl)[2], uint32_t& total,
+	                      uint32_t brick, uint32_t mi, uint32_t mj) {
 		total = 0;
 #pragma unroll
 		for (uint32_t h = 0; h < 2; ++h) {
 			const uint32_t blk = h * 32 + lane;
-			const unsigned long long hm = slab.hm[blk], u = slab.mm[blk] | hm;
-			uint32_t t = 0, ld = 0, init = 0, sk = 0;
+			unsigned long long hm = slab.hm[blk], u = slab.mm[blk] | hm, ha = 0, hb = 0;
+			if (PAIR) {
+				const size_t b = (size_t)brick * 64 + blk;
+				ha = (mi & kMiNoHits) ? 0ull : M.hit_mask[b];
+				hb = (mj & kMiNoHits) ? 0ull : M.hit_mask2[b];
+				hm = ha | hb;
+				u = slab.mm[blk] | slab.hm[blk] | hm;
+			}
+			uint32_t t = 0, ld = 0, init = 0, sk = 0, eh = 0;
 			if (u) {
-#pragma unroll
-				for (uint32_t o = 0; o < 8; ++o) {
-					const uint32_t base = ((o & 1u) << 1) | ((o & 2u) << 2) | ((o & 4u) << 3);
-					t |= (((u >> base) & 0x330033ull) ? 1u : 0u) << o;
+				if (PAIR) {
+					const unsigned long long ua = slab.mm[blk] | ha, ub = slab.hm[blk] | hb;
+					const uint32_t ta = mask_octets(ua), tb = mask_octets(ub);
+					t = ta | tb;
+					s_vox += __popcll(ua);
+					s_hit += __popcll(ha);
+					s_oct += __popc(ta);
+					s_vox2 += __popcll(ub);
+					s_hit2 += __popcll(hb);
+					s_oct2 += __popc(tb);
+					eh = (ha ? kEntHitA : 0u) | (hb ? kEntHitB : 0u);
+				} else {
+					t = mask_octets(u);
 				}
-				if (!COLOR) {  // colour maps skip nothing and count in the leaf loop
+				if (!COLOR && !PAIR) {  // colour maps skip nothing and count in the leaf loop
 					s_vox += __popcll(u);
 					s_hit += __popcll(hm);
 					s_oct += __popc(t);
@@ -341,7 +416,7 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				while (bits) {
 					const uint32_t o = __ffs(bits) - 1;
 					bits &= bits - 1;
-					list[at++] = (uint16_t)((blk << 3) | o | (((init >> o) & 1u) ? kEntInit : 0u) | (((t >> o) & 1u) ? kEntTouched : 0u));
+					list[at++] = (uint16_t)((blk << 3) | o | (((init >> o) & 1u) ? kEntInit : 0u) | (((t >> o) & 1u) ? kEntTouched | eh : 0u));
 				}
 			}
 			total += __shfl_sync(FULL, incl, 31);
@@ -351,7 +426,8 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 	uint32_t t8[2], excl[2], total = 0;     // the brick being processed
 	uint32_t t8n[2], excln[2], totaln = 0;  // the warp's next brick (its list is built one brick early)
 	mbar_wait(&S.bar[0], 0u);
-	build_list(S.slab[0], S.list[0], t8, excl, total);
+	build_list(S.slab[0], S.list[0], t8, excl, total, __shfl_sync(FULL, st_brick0, 0), __shfl_sync(FULL, st_mi0, 0),
+	           __shfl_sync(FULL, st_mj0, 0));
 	__syncwarp();
 	for (uint32_t it = 0;; ++it) {
 		const uint32_t st = it & 1u;
@@ -362,7 +438,8 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			claim = n_warps + atomicAdd(&M.ctr->k3_cursor, 1u);
 		}
 		const uint32_t brick = __shfl_sync(FULL, st == 0 ? st_brick0 : st_brick1, 0);
-		const uint32_t mi = __shfl_sync(FULL, st == 0 ? st_mi0 : st_mi1, 0) & ~kMiNoHits;
+		const uint32_t mi_raw = __shfl_sync(FULL, st == 0 ? st_mi0 : st_mi1, 0), mi = mi_raw & ~kMiNoHits;
+		const uint32_t mj_raw = PAIR ? __shfl_sync(FULL, st == 0 ? st_mj0 : st_mj1, 0) : 0u, mj = mj_raw & ~kMiNoHits;
 		const WarpSlab& slab = S.slab[st];
 		const uint16_t* list = S.list[st];
 		const size_t b0 = (size_t)brick * 64;
@@ -419,11 +496,19 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 					S.omax[idx] = fmaxf(fmaxf(fmaxf(p.x, p.y), fmaxf(p.z, p.w)), fmaxf(fmaxf(q.x, q.y), fmaxf(q.z, q.w)));
 					continue;
 				}
-				const uint32_t m8 = octet_bits8(slab.mm[t], o), h8 = octet_bits8(slab.hm[t], o);
+				const uint32_t m8 = octet_bits8(slab.mm[t], o);
+				uint32_t h8, m8b = 0, h8b = 0;
+				if (PAIR) {
+					h8 = (en[f] & kEntHitA) ? octet_bits8(M.hit_mask[b0 + t], o) : 0u;
+					m8b = octet_bits8(slab.hm[t], o);
+					h8b = (en[f] & kEntHitB) ? octet_bits8(M.hit_mask2[b0 + t], o) : 0u;
+				} else {
+					h8 = octet_bits8(slab.hm[t], o);
+				}
 				float omax;
 				uint32_t ofl;
-				const bool clean = update_octet<SET, !COLOR>(M, miss, M.leaf + (b0 + t) * 64 + 8 * o, m8, h8, a0[f], a1[f], omax, ofl,
-				                                     b0 + t, o, (en[f] & kEntInit) != 0u);
+				const bool clean = update_octet<SET, !COLOR, PAIR>(M, miss, M.leaf + (b0 + t) * 64 + 8 * o, m8, h8, a0[f], a1[f], omax,
+				                                               ofl, b0 + t, o, (en[f] & kEntInit) != 0u, m8b, h8b);
 				S.omax[idx] = omax;
 				// the entry has been consumed: the slot carries the flags back (bit 2: not written back)
 				S.list[st][idx] = (uint16_t)(ofl | (clean ? 4u : 0u));
@@ -443,10 +528,11 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			zero_hits(st ^ 1u);
 			__syncwarp();
 			mbar_wait(&S.bar[st ^ 1u], ((it + 1u) >> 1) & 1u);
-			build_list(S.slab[st ^ 1u], S.list[st ^ 1u], t8n, excln, totaln);
+			const uint32_t brick_n = __shfl_sync(FULL, st == 0 ? st_brick1 : st_brick0, 0);
+			build_list(S.slab[st ^ 1u], S.list[st ^ 1u], t8n, excln, totaln, brick_n, __shfl_sync(FULL, st == 0 ? st_mi1 : st_mi0, 0),
+			           __shfl_sync(FULL, st == 0 ? st_mj1 : st_mj0, 0));
 #if UFO_UB_PREFETCH
 			__syncwarp();
-			const uint32_t brick_n = __shfl_sync(FULL, st == 0 ? st_brick1 : st_brick0, 0);
 			const float* leaf_n = M.leaf + (size_t)brick_n * 64 * 64;
 			for (uint32_t i = lane; i < totaln; i += 32) {
 				const uint32_t en = S.list[st ^ 1u][i], off = ((en >> 3) & 63u) * 64 + 8 * (en & 7u);
@@ -461,13 +547,20 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 		float agg_occ[2];
 		uint32_t agg_fl[2], agg_rgb[2];
 		uint32_t n_clean = 0;  // profiling level 2: this lane's sectors that were not written back
+		uint32_t mk[2] = {0u, 0u};  // PAIR: bit 0 the first scan marked the block, bit 1 the second
 #pragma unroll
 		for (uint32_t h = 0; h < 2; ++h) {
 			const uint32_t blk = h * 32 + lane;
 			const size_t b = b0 + blk;
-			const unsigned long long hm = slab.hm[blk];
+			unsigned long long hm = slab.hm[blk], ha = 0, hb = 0;
+			if (PAIR) {
+				ha = (mi_raw & kMiNoHits) ? 0ull : M.hit_mask[b];
+				hb = (mj_raw & kMiNoHits) ? 0ull : M.hit_mask2[b];
+				mk[h] = ((slab.mm[blk] | ha) ? 1u : 0u) | ((slab.hm[blk] | hb) ? 2u : 0u);
+				hm = ha | hb;
+			}
 			const uint32_t mt = slab.meta[blk];
-			const bool marked = (slab.mm[blk] | hm) != 0ull;
+			const bool marked = PAIR ? mk[h] != 0u : (slab.mm[blk] | hm) != 0ull;
 			float my_occ = 0.0f;
 			uint32_t my_fl = M.default_flags, my_rgb = 0;
 			if (marked) {
@@ -520,12 +613,28 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 					my_rgb = rms_rgb(newc, 8);
 					M.rgb2[b] = my_rgb;
 				}
-				M.meta[b] = (newmeta & 0xffffffu) | (mt & 0xff0000u) | (M.scan_id << 24);
-				M.mask_base[(size_t)mi * 64 + blk] = 0ull;  // masks cleared for the next scan
-				if (hm) M.hit_mask[b] = 0ull;
-				s_blk += 1;
+				if (PAIR) {
+					// the block carries the id of the last scan that marked it, as after two passes
+					M.meta[b] = (newmeta & 0xffffffu) | (mt & 0xff0000u) | (((mk[h] & 2u) ? M.scan_id : M.pair_id) << 24);
+					if (slab.mm[blk]) M.mask_base[(size_t)mi * 64 + blk] = 0ull;
+					if (slab.hm[blk]) M.mask_base2[(size_t)mj * 64 + blk] = 0ull;
+					if (ha) M.hit_mask[b] = 0ull;
+					if (hb) M.hit_mask2[b] = 0ull;
+					s_blk += mk[h] & 1u;
+					s_blk2 += mk[h] >> 1;
+					// a first-touched block counts for the first scan that marked it
+					if (!(mt & 0xff0000u)) {
+						s_new += mk[h] & 1u;
+						s_new2 += mk[h] == 2u ? 1u : 0u;
+					}
+				} else {
+					M.meta[b] = (newmeta & 0xffffffu) | (mt & 0xff0000u) | (M.scan_id << 24);
+					M.mask_base[(size_t)mi * 64 + blk] = 0ull;  // masks cleared for the next scan
+					if (hm) M.hit_mask[b] = 0ull;
+					s_blk += 1;
+					s_new += (mt & 0xff0000u) ? 0u : 1u;
+				}
 				s_lin += ((t & 0x0fu) ? 1u : 0u) + ((t & 0xf0u) ? 1u : 0u);  // leaf lines read
-				s_new += (mt & 0xff0000u) ? 0u : 1u;
 				my_occ = bmax;
 				my_fl = bfl | 0x100u;
 			} else if (fold && (mt & 0xff0000u)) {
@@ -579,6 +688,11 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 				rgb4 = rms_rgb(cc, 8);
 			}
 			const uint32_t ub0 = __ballot_sync(FULL, u3[0] != 0 && (lane & 7) == 0), ub1 = __ballot_sync(FULL, u3[1] != 0 && (lane & 7) == 0);
+			uint32_t d3a = 0, d3b = 0;  // PAIR: depth-3 nodes marked by each scan
+			if (PAIR) {
+				d3a = ballot_groups(__ballot_sync(FULL, mk[0] & 1u)) + ballot_groups(__ballot_sync(FULL, mk[1] & 1u));
+				d3b = ballot_groups(__ballot_sync(FULL, mk[0] & 2u)) + ballot_groups(__ballot_sync(FULL, mk[1] & 2u));
+			}
 			if ((lane & 7) == 0) {
 #pragma unroll
 				for (int h = 0; h < 2; ++h) {
@@ -589,9 +703,22 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 			if (lane == 0) {
 				M.brick_sum4[brick] = {m4, f4};
 				if (COLOR) M.brick_rgb4[brick] = rgb4;
-				unsigned long long* slot = M.ctr->stat[brick % kStatSlots];
-				atomicAdd(&slot[5], 1ull);
-				atomicAdd(&slot[6], (unsigned long long)(__popc(ub0) + __popc(ub1)));
+				if (PAIR) {
+					unsigned long long* sa = M.ctr->stat[brick % (kStatSlots / 2)];
+					unsigned long long* sb = M.ctr->stat[kStatSlots / 2 + brick % (kStatSlots / 2)];
+					if (mi_raw != kMiAbsent) {
+						atomicAdd(&sa[5], 1ull);
+						atomicAdd(&sa[6], (unsigned long long)d3a);
+					}
+					if (mj_raw != kMiAbsent) {
+						atomicAdd(&sb[5], 1ull);
+						atomicAdd(&sb[6], (unsigned long long)d3b);
+					}
+				} else {
+					unsigned long long* slot = M.ctr->stat[brick % kStatSlots];
+					atomicAdd(&slot[5], 1ull);
+					atomicAdd(&slot[6], (unsigned long long)(__popc(ub0) + __popc(ub1)));
+				}
 			}
 		}
 		if (!COLOR && M.k3_stat) {
@@ -629,9 +756,27 @@ __global__ void __launch_bounds__(UbShape<COLOR>::kWarps * 32, UbShape<COLOR>::k
 		s_blk += __shfl_xor_sync(FULL, s_blk, o);
 		s_new += __shfl_xor_sync(FULL, s_new, o);
 		s_lin += __shfl_xor_sync(FULL, s_lin, o);
+		if (PAIR) {
+			s_vox2 += __shfl_xor_sync(FULL, s_vox2, o);
+			s_hit2 += __shfl_xor_sync(FULL, s_hit2, o);
+			s_oct2 += __shfl_xor_sync(FULL, s_oct2, o);
+			s_blk2 += __shfl_xor_sync(FULL, s_blk2, o);
+			s_new2 += __shfl_xor_sync(FULL, s_new2, o);
+		}
+	}
+	if (PAIR && lane == 0) {
+		// the leaf lines read are the pass's: they count for its last scan
+		unsigned long long* slot = M.ctr->stat[kStatSlots / 2 + gw % (kStatSlots / 2)];
+		if (s_vox2) atomicAdd(&slot[0], (unsigned long long)s_vox2);
+		if (s_hit2) atomicAdd(&slot[1], (unsigned long long)s_hit2);
+		if (s_oct2) atomicAdd(&slot[2], (unsigned long long)s_oct2);
+		if (s_blk2) atomicAdd(&slot[3], (unsigned long long)s_blk2);
+		if (s_new2) atomicAdd(&slot[4], (unsigned long long)s_new2);
+		if (s_lin) atomicAdd(&slot[7], (unsigned long long)s_lin);
+		s_lin = 0;
 	}
 	if (lane == 0) {
-		unsigned long long* slot = M.ctr->stat[gw % kStatSlots];
+		unsigned long long* slot = M.ctr->stat[gw % (PAIR ? kStatSlots / 2 : kStatSlots)];
 		if (s_vox) atomicAdd(&slot[0], (unsigned long long)s_vox);
 		if (s_hit) atomicAdd(&slot[1], (unsigned long long)s_hit);
 		if (s_oct) atomicAdd(&slot[2], (unsigned long long)s_oct);

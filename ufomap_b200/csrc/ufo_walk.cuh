@@ -109,6 +109,12 @@ __global__ void __launch_bounds__(256) k_gather(DeviceMap M)
 			}
 			const uint32_t slot = brick_find_or_create(M, key);
 			if (slot == kNone) continue;  // pool exhausted: flagged, the scan is repeated
+			const uint32_t mi = vb | (M.hit_stamp[slot] == M.scan_id ? 0u : kMiNoHits);
+			if (M.pair_id && M.brick_stamp[slot] == M.pair_id) {
+				// second scan of a pair, brick already listed by the first: one entry, both mask slabs
+				M.touched_mi2[M.touch_idx[slot]] = mi;
+				continue;
+			}
 			M.brick_stamp[slot] = M.scan_id;
 			// one list-cursor atomic per group of lanes, not per brick (same-address atomics serialise)
 			const uint32_t peers = __activemask();
@@ -118,7 +124,9 @@ __global__ void __launch_bounds__(256) k_gather(DeviceMap M)
 			base = __shfl_sync(peers, base, leader);
 			const uint32_t i = base + __popc(peers & ((1u << lane) - 1u));
 			M.touched[i] = slot;
-			M.touched_mi[i] = vb | (M.hit_stamp[slot] == M.scan_id ? 0u : kMiNoHits);
+			M.touched_mi[i] = M.pair_id ? kMiAbsent : mi;
+			M.touched_mi2[i] = M.pair_id ? mi : kMiAbsent;
+			M.touch_idx[slot] = i;
 		}
 	}
 }
